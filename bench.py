@@ -2,14 +2,16 @@
 """bench.py — BASELINE.json metric on the BASELINE configs, one JSON line on stdout (rank 0).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--only infer,train,spp_nms,nms,lib,cpu]
+                  [--dump-outputs DIR]
   torchrun ... bench.py --gpus N ...        (one rank per GPU)
 
 Headline (config 2, `metric`/`value`/`e2e`/`roofline`): a step = one pass of the hot path (Model.forward + Detect decode,
-reference models/yolo.py) over one synthetic batch "YOLOv3 640x640 bs=32 inference on 1 B200, synthetic input, random-init
-weights"; weak scaling: bs 32 per GPU, no data-path collective.
+reference models/yolo.py) over one synthetic batch "YOLOv3 640x640 bs=32 inference on 1 H100, synthetic input, random-init
+weights"; weak scaling: bs 32 per GPU, no data-path collective.  Every leg times exactly --steps steps.
   value      images/s, inputs resident in HBM (fp32 NCHW), CUDA-graph replay, CUDA-event timing, max over ranks
   e2e        images/s through yolov3_b200.Pipeline with HOST uint8 images: H2D + forward + decode + NMS + D2H per step
-  roofline   conv kernels (tensor bound): algorithmic conv FLOPs / event-timed conv_tc launch time, vs MEASURED_PEAKS
+  roofline   conv kernels (tensor bound): algorithmic conv FLOPs / event-timed conv_tc launch time, vs MEASURED_PEAKS.json
+             when present, else the H100 SXM data-sheet peak
   parity_rel_l2   z of the timed bs-32 engine vs the CPU reference/oracle forward on the same images and weights (the run
                   fails above 2e-2)
 Extra keys (the other BASELINE configs, tools/bench_workloads.py):
@@ -19,7 +21,10 @@ Extra keys (the other BASELINE configs, tools/bench_workloads.py):
   nms        config 5: five thresholds x single/multi-label on synthetic [32,25200,85]
   gpu_library_baseline   the reference itself on this GPU through PyTorch+cuDNN / torchvision / torch DDP (informational)
   cpu_baseline / --impl reference: the reference's own torch-CPU Model + non_max_suppression from the staged copy
-             (baseline/_ref, kind "reference"), else the oracle port (kind "port"), on the host cores, bounded sample.
+             (oracle/_ref, kind "reference"), else the oracle port (kind "port"), on the host cores, bounded sample.
+--dump-outputs DIR  after the timed steps: what the headline path returned in its last timed step, as float32 .npy files —
+             z_sample.npy = z[:, rows] ([bs, 4096, 85], the decoded predictions at 4096 fixed seeded anchor rows) and
+             z_rows.npy (those row indices).  Inputs and weights are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -50,31 +55,6 @@ def peaks():
     from bench_workloads import peaks as _p
 
     return _p()
-
-
-def recorded_conv_traffic():
-    """`roofline.traffic`: DRAM bytes of the conv_tc launches of ONE forward (bs 32) from the committed ncu capture of
-    tools/run_forward.py (profiles/r02_ncu_conv_tc_dram.csv: dram__bytes_read.sum + dram__bytes_write.sum per launch) — a recorded
-    capture of the same kernels, not a counter of this run (no profiler runs inside the timed process); null when absent."""
-    import csv
-
-    p = ROOT / "profiles" / "r02_ncu_conv_tc_dram.csv"
-    if not p.exists():
-        return {"traffic": None, "traffic_note": "no committed ncu DRAM capture (profiles/r02_ncu_conv_tc_dram.csv)"}
-    try:
-        rows = [r for r in csv.DictReader(l for l in p.read_text().splitlines() if not l.startswith("=="))]
-        tot, n = 0.0, 0
-        for r in rows:
-            if r.get("Metric Name") in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                v = float(r["Metric Value"].replace(",", ""))
-                v *= {"byte": 1, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}.get(r["Metric Unit"], 1)
-                tot += v
-                n += 1
-        launches = n // 2
-        return {"traffic": tot, "traffic_unit": "bytes per step (sum over the conv_tc launches of one forward)",
-                "traffic_launches": launches, "traffic_source": "profiles/r02_ncu_conv_tc_dram.csv (ncu capture, recorded)"}
-    except Exception as e:  # noqa: BLE001
-        return {"traffic": None, "traffic_note": f"could not parse the committed capture: {e!r}"}
 
 
 def workload_config(world):
@@ -163,7 +143,7 @@ def build_model(device):
 # ------------------------------------------------------------------------------------------ CPU legs (checker / baseline only)
 class CpuReference:
     """The reference's torch-CPU forward for the bench model: the reference's OWN ``Model`` from the staged copy
-    (baseline/_ref, ``kind = "reference"``) when present, else the oracle port (``kind = "port"``), holding the same weights
+    (oracle/_ref, ``kind = "reference"``) when present, else the oracle port (``kind = "port"``), holding the same weights
     as the GPU model (``params``), fused, fp32, inference mode.  Thread count: calibrated AT the batch that is timed."""
 
     def __init__(self, params=None):
@@ -182,7 +162,7 @@ class CpuReference:
                 from models.yolo import Model as RefModel
                 from utils.general import non_max_suppression as ref_nms
 
-                m = RefModel(str(ref_shim.REFERENCE_ROOT / "models" / CFG))
+                m = RefModel(str(ref_shim.reference_root() / "models" / CFG))
                 if params is not None:
                     missing, unexpected = m.load_state_dict(params, strict=False)
                     assert not unexpected and all("num_batches_tracked" in k for k in missing), (missing[:3], unexpected[:3])
@@ -296,7 +276,7 @@ def library_baseline(dev, rank, world, bs=32, img=640, steps=10, train_bs=8):
     torch.optim.SGD under bf16 autocast.  Informational: this is the bar a kernel library sets on the same hardware."""
     shim = _reference_modules()
     if shim is None:
-        return {"unavailable": "reference not staged (baseline/_ref missing: run oracle/stage_reference.py in the build container)"}
+        return {"unavailable": "reference not staged (oracle/_ref missing: see oracle/stage_reference.py)"}
     from models.yolo import Model as RefModel
     from utils.general import non_max_suppression as ref_nms
     from utils.loss import ComputeLoss as RefLoss
@@ -308,7 +288,7 @@ def library_baseline(dev, rank, world, bs=32, img=640, steps=10, train_bs=8):
 
     res = {"impl": "ultralytics/yolov3 @ 97b87b1 (staged copy) on torch " + torch.__version__ + " / cuDNN " + str(torch.backends.cudnn.version())}
     torch.backends.cudnn.benchmark = True
-    cfg = str(shim.REFERENCE_ROOT / "models" / "yolov3.yaml")
+    cfg = str(shim.reference_root() / "models" / "yolov3.yaml")
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     try:
         torch.manual_seed(0)
@@ -337,9 +317,10 @@ def library_baseline(dev, rank, world, bs=32, img=640, steps=10, train_bs=8):
             torch.cuda.synchronize()
             t0 = time.perf_counter()
             n_done = 0
-            for i in range(0, bs, 4):  # 4 images per call keeps the reference's wall-clock break (general.py:746) out of reach
-                ref_nms(pred[i:i + 4], conf, iou, multi_label=ml, max_det=300)
-                n_done += 4
+            for _ in range(steps):  # a step = the bs images; 4 per call keeps the reference's wall-clock break (general.py:746) away
+                for i in range(0, bs, 4):
+                    ref_nms(pred[i:i + 4], conf, iou, multi_label=ml, max_det=300)
+                    n_done += 4
             torch.cuda.synchronize()
             dt = time.perf_counter() - t0
             nms[f"conf{conf}_iou{iou}_{'multi' if ml else 'single'}"] = {"input_boxes_per_s": world * n_done * 25200 / dt,
@@ -379,7 +360,7 @@ def library_baseline(dev, rank, world, bs=32, img=640, steps=10, train_bs=8):
         if world > 1:
             dist.barrier()
         e0.record()
-        n = max(3, steps // 2)
+        n = steps
         for _ in range(n):
             step()
         e1.record()
@@ -394,6 +375,19 @@ def library_baseline(dev, rank, world, bs=32, img=640, steps=10, train_bs=8):
     return res
 
 
+def dump_outputs(out_dir, z, n_rows=4096):
+    """z [bs, anchors, 85] fp32 of one step -> DIR/z_sample.npy (a fixed seeded set of anchor rows of every image, ~45 MB at
+    bs 32) and DIR/z_rows.npy (the row indices)."""
+    import numpy as np
+    import torch
+
+    rows = torch.randperm(z.shape[1], generator=torch.Generator().manual_seed(0))[:n_rows].sort().values
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    np.save(out / "z_sample.npy", z[:, rows.to(z.device)].float().cpu().numpy())
+    np.save(out / "z_rows.npy", rows.numpy().astype(np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -403,6 +397,7 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--only", default="all", help="comma list of legs besides the headline: train,spp_nms,nms,lib,cpu (default all)")
     ap.add_argument("--per-op", default=None, help="write the per-launch timing table (JSON) to this path")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs (.npy) to DIR")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     legs = {"train", "spp_nms", "nms", "lib", "cpu"} if args.only == "all" else set(filter(None, args.only.split(","))) - {"none"}
@@ -433,7 +428,7 @@ def main():
     params_host = model.state_dict()  # for the CPU parity / baseline leg (taken before anything can go wrong on the device)
     eng = model.engine(BS, IMG, IMG, torch.float32)
     n_launch = _lib.lib().y3_model_num_launches(eng.handle)
-    # two distinct resident input batches (157 MB each > 126 MB L2), alternated so no step re-reads a cached input.  The first
+    # two distinct resident input batches (157 MB each > 50 MB L2), alternated so no step re-reads a cached input.  The first
     # images of batch 0 come from a CPU generator: the parity leg runs the CPU reference on exactly those images.
     n_par = 2
     x_par = torch.rand(n_par, 3, IMG, IMG, generator=torch.Generator().manual_seed(1))
@@ -462,6 +457,8 @@ def main():
     e1.record()
     torch.cuda.synchronize()
     ms_total = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng.z)  # before any further replay overwrites the last timed step's z
     clocks = None
     if rank == 0:
         # the clock samples must come from this workload: keep replaying it (untimed) until >= 0.6 s of load were observed
@@ -519,7 +516,7 @@ def main():
     if rank == 0:
         from yolov3_b200.profile import time_ops
 
-        per_op = time_ops(eng, xs[0], iters=max(3, min(10, args.steps)))
+        per_op = time_ops(eng, xs[0], iters=args.steps)
     del pipe, graphs
     model._engines.clear()
     del eng
@@ -543,13 +540,13 @@ def main():
     if "nms" in legs:
         leg("nms", lambda: {"workload": f"synthetic [bs {BS}/GPU, 25200, 85] fp32 (SURVEY §8d config 5), max_det 300, device-resident, "
                                         "sync-free y3_nms_batched; iou 0.6 at conf <= 0.01 else 0.45", "unit": "input boxes/s",
-                            **W.nms_sweep_workload(dev, rank, world, bs=BS)})
+                            **W.nms_sweep_workload(dev, rank, world, bs=BS, reps=args.steps)})
     if "spp_nms" in legs:
-        leg("spp_nms", lambda: W.spp_nms_workload(dev, rank, world, bs=8, img=IMG, steps=max(10, args.steps), warmup=args.warmup))
+        leg("spp_nms", lambda: W.spp_nms_workload(dev, rank, world, bs=8, img=IMG, steps=args.steps, warmup=args.warmup))
     if "train" in legs:
-        leg("train", lambda: W.train_step_workload(dev, rank, world, bs=8, img=IMG, steps=max(5, min(10, args.steps)), warmup=3))
+        leg("train", lambda: W.train_step_workload(dev, rank, world, bs=8, img=IMG, steps=args.steps, warmup=3))
     if "lib" in legs:
-        leg("gpu_library_baseline", lambda: library_baseline(dev, rank, world, bs=BS, img=IMG, steps=max(5, min(10, args.steps))))
+        leg("gpu_library_baseline", lambda: library_baseline(dev, rank, world, bs=BS, img=IMG, steps=args.steps))
 
     if rank != 0:
         if world > 1:
@@ -567,8 +564,7 @@ def main():
                 "kernel": f"conv_tc_kernel ({sum(1 for o in per_op if o['kind'] == 'conv_tc')} launches/step)",
                 "kernel_ms_per_step": conv_ms, "kernel_share_of_step": conv_ms / all_ms,
                 "whole_step_frac": GFLOP_PER_IMG * 1e9 * (value / world) / (pk["tf_sustained"] * 1e12),
-                "peak_source": pk["source"] + " sustained bf16 (MEASURED_PEAKS.json)",
-                **recorded_conv_traffic()}
+                "peak_source": pk["source"]}
     dec = [o for o in per_op if o["kind"] == "decode"]
     if dec:  # Detect decode: read the head logits + write z = 17.1 MB/image algorithmic
         roofline["decode_hbm"] = {"bound": "hbm", "achieved": dec[0]["gbs"], "peak": pk["hbm"], "unit": "GB/s",
@@ -589,7 +585,7 @@ def main():
         cpu = {"value": probe.shape[0] / dt, "unit": UNIT, "cores": ref.threads, "kind": ref.kind,
                "sample": f"8 of the {BS} images of a step, one timed pass after warm-up and thread calibration "
                          f"(img/s by thread count: {ref.tried}); "
-                         + ("reference models.yolo.Model from baseline/_ref" if ref.kind == "reference" else "oracle port")}
+                         + ("reference models.yolo.Model from oracle/_ref" if ref.kind == "reference" else "oracle port")}
         zr = z_ref[:n_par].double()
         parity = float((z_par.double() - zr).norm() / zr.norm())
 

@@ -1,4 +1,4 @@
-/* yolov3_b200 — C ABI of the Blackwell-native (sm_100a) YOLOv3 detection hot path.
+/* yolov3_b200 — C ABI of the Hopper-native (sm_90a) YOLOv3 detection hot path.
  *
  * The reference (ultralytics/yolov3, pure Python) has no FFI: its seams for this path are Python call signatures
  * (SURVEY.md §8b).  This header is the drop-in boundary a binding for those seams attaches to; each entry point cites
@@ -25,7 +25,7 @@ extern "C" {
 #define Y3_OK 0
 #define Y3_ERR_BAD_ARG (-1)     /* shape/alignment/enum not supported by this path */
 #define Y3_ERR_CUDA (-2)        /* a CUDA runtime/driver call failed (message in y3_last_error) */
-#define Y3_ERR_UNSUPPORTED (-3) /* device is not sm_100 (no fallback path exists by design) */
+#define Y3_ERR_UNSUPPORTED (-3) /* device is not sm_90 (no fallback path exists by design) */
 
 #define Y3_ACT_NONE 0
 #define Y3_ACT_SILU 1
@@ -47,7 +47,7 @@ int64_t y3_abi_sizeof(int32_t which);
 int y3_set_pdl(int32_t on);
 /* Kernel-variant switch of y3_bn_act_bwd (non-upsample layers): 1 (default) = the cp.async shared-memory-ring kernels (three
  * work units requested ahead per thread), 0 = the register-staged ones.  Same unit order and arithmetic: results are
- * bit-identical (profiles/r02_ab_shot_kernel_variants.jsonl).  Env Y3_BN_ASYNC=0/1 sets the initial value.  Returns the
+ * bit-identical (tests/test_bn_variants_gpu.py).  Env Y3_BN_ASYNC=0/1 sets the initial value.  Returns the
  * previous setting.  A tuning switch with no counterpart in the reference. */
 int y3_set_bn_async(int32_t on);
 
@@ -55,7 +55,7 @@ int y3_set_bn_async(int32_t on);
  * Conv + folded-BN + SiLU (+ residual add, + nearest-2x upsample, + concat-offset store, or fp32 head store).
  * Replaces Conv.forward_fuse (models/common.py:77-81) after BaseModel.fuse (models/yolo.py:163-172), the shortcut add
  * of Bottleneck.forward (common.py:163-165), nn.Upsample+Concat (models/yolov3.yaml:43-44,51-52) and Detect.m[i]
- * (models/yolo.py:96-98).  tcgen05 implicit GEMM; c_in % 16 == 0, c_out_pad = c_out rounded up to the tile N.
+ * (models/yolo.py:96-98).  wgmma implicit GEMM; c_in % 16 == 0, c_out_pad = c_out rounded up to the tile N.
  * ksize 1|3 with stride 1, or ksize 3 with stride 2 (h, w even); pad = ksize/2.
  */
 typedef struct y3_conv_desc {
@@ -95,11 +95,11 @@ int y3_conv_dgrad_s2(const y3_conv_desc* d, y3_stream_t stream);
 #define Y3_W_XPAIR 1
 int y3_conv_weight_layout(const y3_conv_desc* d);
 /* The kernel variant y3_conv_bn_act_fwd would launch for a descriptor (host-only query: pointers are checked for
- * alignment but never dereferenced, no tensor map is encoded, no GPU needed): tile shape, CTA pairs (cta_group::2), TMA-store
- * epilogue, halo reuse (one A box per filter row), weights resident in shared memory, epilogue warp groups, x-paired
- * stride-2 weights, tile counts and grid.  For tests and for reading the selection heuristics off a model. */
+ * alignment but never dereferenced, no tensor map is encoded, no GPU needed): tile shape, halo reuse (one A box per
+ * filter row), weights resident in shared memory, x-paired stride-2 weights, tile counts and grid.  For tests and for
+ * reading the selection heuristics off a model. */
 typedef struct y3_conv_plan_info {
-  int32_t block_n, block_k, pair, staged, halo, resident_weights, epilogue_groups, xpair;
+  int32_t block_n, block_k, halo, resident_weights, xpair;
   int32_t m_tiles, n_tiles, k_blocks, grid;
 } y3_conv_plan_info;
 int y3_conv_plan(const y3_conv_desc* d, y3_conv_plan_info* out);
@@ -335,7 +335,7 @@ typedef struct y3_wgrad_desc {
 int y3_conv_wgrad(const y3_wgrad_desc* d, y3_stream_t stream);
 /* 1 if the direct stride-2 form (stride = 2) can tile an input of h x w (an 80-pixel tw x th patch must divide the output) */
 int y3_conv_wgrad_s2_supported(int32_t h, int32_t w);
-/* 1 if y3_conv_wgrad accepts Y3_DW_TAP_MAJOR for this c_in (the tcgen05 kernel is in use), else 0 */
+/* 1 if y3_conv_wgrad accepts Y3_DW_TAP_MAJOR for this c_in (the wgmma kernel is in use), else 0 */
 int y3_conv_wgrad_tap_major(int32_t c_in);
 /* dst (+)= src over the interior pixels of two padded NHWC bf16 slices of equal [n,h,w,c] (gradient fan-in) */
 int y3_add_nhwc(const void* src, int32_t src_ld, int32_t src_coff, void* dst, int32_t dst_ld, int32_t dst_coff, int32_t n,

@@ -10,10 +10,10 @@ here from the published ultralytics 8.x formulas (SURVEY.md Appendix B) and unit
 ``tests/golden/make_golden.py`` (``gen_iou``: float64 CIoU cross-check, ``torchvision.ops.box_iou``; ``gen_forward``: fused
 vs unfused forward through ``fuse_conv_and_bn``) and re-checked from the fixtures by ``tests/test_oracle_golden.py``.
 
-Consumers: ``tests/golden/make_golden.py`` (golden-vector generation in the build container, reference at
-``/root/reference``); ``bench.py --impl reference`` / its ``cpu_baseline`` leg and ``tests/test_zz_reference_seam_gpu.py``,
-which run the reference from the byte-for-byte staged copy ``baseline/_ref/`` (``oracle/stage_reference.py``; git-ignored,
-travels to the GPU box with the snapshot).  Nothing under ``yolov3_b200/`` imports this.
+Consumers: ``tests/golden/make_golden.py`` (golden-vector generation where the original checkout is readable) and
+``bench.py --impl reference`` / its ``cpu_baseline`` and ``gpu_library_baseline`` legs, which run the reference from the
+byte-for-byte staged copy ``oracle/_ref/`` (``oracle/stage_reference.py``; git-ignored) when the original is not there.
+Tests use only the ``ModelEMA`` / ``xywh2xyxy`` restatements below.  Nothing under ``yolov3_b200/`` imports this.
 """
 from __future__ import annotations
 
@@ -29,9 +29,13 @@ from pathlib import Path
 import torch
 import torch.nn as nn
 
-_REPO = Path(__file__).resolve().parents[1]
-# the read-only checkout in the build container, else the staged copy that ships to the GPU box
-REFERENCE_ROOT = Path("/root/reference") if (Path("/root/reference") / "models" / "yolo.py").exists() else _REPO / "baseline" / "_ref"
+from stage_reference import DST, SRC, readable  # noqa: E402  (same directory)
+
+
+def reference_root() -> Path:
+    """the original checkout where it is readable, else the copy oracle/stage_reference.py made.  Resolved on call, so that
+    importing this module (the tests use its ModelEMA / xywh2xyxy) looks at no path outside the repository."""
+    return SRC if readable(SRC / "models" / "yolo.py") else DST
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -450,9 +454,10 @@ def install():
             import seaborn  # noqa: F401
         except ImportError:
             _module("seaborn")
-    if str(REFERENCE_ROOT) not in sys.path:
-        sys.path.insert(0, str(REFERENCE_ROOT))
+    root = str(reference_root())
+    if root not in sys.path:
+        sys.path.insert(0, root)
 
 
 def reference_available() -> bool:
-    return (REFERENCE_ROOT / "models" / "yolo.py").exists()
+    return readable(reference_root() / "models" / "yolo.py")

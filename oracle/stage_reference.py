@@ -1,17 +1,14 @@
-"""TEST / BASELINE INFRASTRUCTURE ONLY — stages the UNMODIFIED reference (ultralytics/yolov3, read-only at /root/reference)
-under the git-ignored ``baseline/_ref/`` so that it travels to the GPU box with the repo snapshot (``/root/reference`` does
-not exist there).  Nothing under ``yolov3_b200/`` ever imports it; the only consumers are ``bench.py --impl reference`` /
-``bench.py``'s ``cpu_baseline`` leg (the reference's own ``Model`` / ``non_max_suppression`` timed on the host cores) and the
-seam test ``tests/test_zz_reference_seam_gpu.py`` (the reference's detect/val loop bodies with our backend swapped in).
+"""TEST / BASELINE INFRASTRUCTURE ONLY — stages the UNMODIFIED reference (ultralytics/yolov3, the read-only checkout at ``SRC``
+where it exists) under the git-ignored ``oracle/_ref/`` so that a machine without the original checkout can still run it.  Nothing
+under ``yolov3_b200/`` ever imports it; the only consumers are ``bench.py --impl reference`` / ``bench.py``'s ``cpu_baseline``
+and ``gpu_library_baseline`` legs (the reference's own ``Model`` / ``non_max_suppression``), which fall back to the oracle
+port when nothing is staged.  The tests never need it: what they compare against is stored under ``tests/golden/``.
 
-Why a file copy and not ``pip install --target baseline/_ref /root/reference``: tried (round 2) — the reference's
-pyproject.toml declares no ``version`` (setuptools: "`project` must contain ['version'] properties") and its layout is a
-flat script tree (``models/``, ``utils/``, ``detect.py`` at top level: not an installable distribution), so metadata
-generation fails before anything is built.  The reference is meant to be run from a clone (its README); a clone of the
-needed files is what this makes.  Files are copied byte for byte, never edited; ``baseline/_ref/`` is listed in .gitignore so
-no reference source enters this repository's history.
+A file copy, not ``pip install``: the reference's pyproject.toml declares no ``version`` and its layout is a flat script tree
+(``models/``, ``utils/``, ``detect.py`` at top level), so it is meant to be run from a clone; a clone of the needed files is
+what this makes.  Files are copied byte for byte, never edited, and never enter this repository's history.
 
-    python oracle/stage_reference.py            # no-op when /root/reference is absent (GPU box) or already staged
+    python oracle/stage_reference.py            # no-op when the original is absent or unreadable, or already staged
 """
 from __future__ import annotations
 
@@ -21,7 +18,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
 SRC = Path("/root/reference")
-DST = ROOT / "baseline" / "_ref"
+DST = ROOT / "oracle" / "_ref"
 # what the hot path's callers import: the model/graph code, the utils they pull in, the three loop scripts, YAMLs, the two
 # sample images of BASELINE config 1 and the hyper-parameter files ComputeLoss reads
 TOP_FILES = ["detect.py", "val.py", "train.py", "hubconf.py", "export.py", "LICENSE"]
@@ -29,12 +26,21 @@ TREES = ["models", "utils", "data/hyps", "data/images"]
 DATA_FILES = ["data/coco128.yaml", "data/coco.yaml"]
 
 
+def readable(p: Path) -> bool:
+    """exists and may be read by this user (who may lack the permission to look inside the directory that holds it)"""
+    try:
+        with open(p, "rb"):
+            return True
+    except OSError:
+        return False
+
+
 def staged() -> bool:
-    return (DST / "models" / "yolo.py").exists()
+    return readable(DST / "models" / "yolo.py")
 
 
 def stage(force: bool = False) -> Path | None:
-    if not (SRC / "models" / "yolo.py").exists():
+    if not readable(SRC / "models" / "yolo.py"):
         return DST if staged() else None
     if staged() and not force:
         return DST

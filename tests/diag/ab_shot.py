@@ -1,16 +1,18 @@
 """On-device A/B of the kernel variant behind the run-time switch y3_set_bn_async: the SAME inputs go through both kernels,
 the outputs are compared bit for bit (the variants are meant to be bit-identical) and both are timed as CUDA-graph replays
 over buffer sets larger than L2; then the whole training step with the switch off / on.  Every result is appended to
-gpurun_out/ab_shot.jsonl as soon as it exists (the GPU call this runs in may be cut short).
-    python tests/diag/ab_shot.py [--budget SECONDS] [--skip-train]
+the --out file (default: ab_shot.jsonl in the system temp directory) as soon as it exists, so a run cut short keeps what it
+measured.
+    python tests/diag/ab_shot.py [--budget SECONDS] [--skip-train] [--out FILE.jsonl]
 The version of this script at commit 5fd94b1 also compared a staged Detect-decode kernel and ring variants of bn_stats /
-bn_act_fwd (profiles/r02_ab_shot_kernel_variants.jsonl): bit-identical, not faster, removed (profiles/r02_experiments.md).
+bn_act_fwd: bit-identical, not faster, removed.
 Diagnostics only — not collected by pytest, not part of the product."""
 import argparse
 import json
 import math
 import os
 import sys
+import tempfile
 import time
 from pathlib import Path
 
@@ -20,10 +22,9 @@ sys.path.insert(0, str(ROOT))
 ap = argparse.ArgumentParser()
 ap.add_argument("--budget", type=float, default=120.0, help="stop starting new sections after this many seconds")
 ap.add_argument("--skip-train", action="store_true")
+ap.add_argument("--out", type=Path, default=Path(tempfile.gettempdir()) / "ab_shot.jsonl")
 args = ap.parse_args()
-OUT = ROOT / "gpurun_out"
-OUT.mkdir(exist_ok=True)
-LOG = open(OUT / "ab_shot.jsonl", "a")
+LOG = open(args.out, "a")
 
 
 def emit(**kw):

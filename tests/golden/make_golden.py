@@ -11,6 +11,10 @@ What is pinned (SURVEY.md Appendix D):
   iou_cases.npz         box_iou, bbox_iou(CIoU) values                                    (ultralytics, via shim)
   val_cases.npz         val.process_batch correct[N,10] on seeded detections / labels     (val.py:147-188)
   tta_cases.npz         Model.forward(x, augment=True) rows (scale / flip views merged)    (models/yolo.py:239-280)
+  seam_*.npz            what tests/test_zz_reference_seam_gpu.py and the optimizer-group test compare against: the
+                        reference's smart_optimizer groups, its val.py loop pieces (NMS, scale_boxes, process_batch) and,
+                        per sample image, its letterboxed input, Model forward, NMS and scale_boxes  (detect.py, val.py,
+                        utils/torch_utils.py:207-237)
 """
 from __future__ import annotations
 
@@ -33,7 +37,7 @@ CFG = ROOT / "yolov3_b200" / "cfg"
 def ref_model(name, params):
     from models.yolo import Model  # reference
 
-    m = Model(str(ref_shim.REFERENCE_ROOT / "models" / f"{name}.yaml"))
+    m = Model(str(ref_shim.reference_root() / "models" / f"{name}.yaml"))
     missing, unexpected = m.load_state_dict(params, strict=False)
     assert not unexpected, unexpected
     assert all("num_batches_tracked" in k for k in missing), missing
@@ -319,11 +323,88 @@ def gen_val():
     np.savez_compressed(OUT / "val_cases.npz", **store)
 
 
+SEAM_ROWS = 512  # anchor rows of z kept per sample image
+
+
+def gen_seam():
+    """What the seam tests compare against, taken from the reference: (1) smart_optimizer's three parameter groups on the
+    nn.Module facade (names in order + each group's SGD settings), (2) the val.py loop pieces on seeded predictions,
+    (3) per sample image of data/images at 640: the letterboxed input, a seeded sample of the reference Model's z, its NMS and
+    scale_boxes."""
+    import val as ref_val
+    from models.yolo import Model as RefModel
+    from utils.dataloaders import LoadImages
+    from utils.general import non_max_suppression as ref_nms
+    from utils.general import scale_boxes as ref_scale
+    from utils.general import xywh2xyxy
+    from utils.torch_utils import smart_optimizer
+
+    sys.path.insert(0, str(ROOT))
+    from yolov3_b200.module import DetectionModel
+
+    out = {}
+    for name in ("yolov3-tiny", "yolov3"):
+        dm = DetectionModel(CFG / f"{name}.yaml", device="cpu")
+        names = {p.data_ptr(): n for n, p in dm.named_parameters()}
+        opt = smart_optimizer(dm, "SGD", lr=0.01, momentum=0.937, decay=5e-4)
+        for gi, g in enumerate(opt.param_groups):
+            out[f"opt_{name}_g{gi}_names"] = np.array([names[p.data_ptr()] for p in g["params"]])
+            out[f"opt_{name}_g{gi}_hyp"] = np.array([g["lr"], g["momentum"], g["dampening"], g["weight_decay"], float(g["nesterov"])])
+    # val.py:355-390 pieces on seeded predictions / labels
+    pred = O.synth_predictions(2, n_rows=3000, nc=80, seed=5)
+    targets = O.synth_targets(2, seed=4)
+    h = w = 640
+    shape0, ratio_pad = (480, 600), ((1.0667, 1.0667), (0.0, 64.0))
+    targets_px = targets.clone()
+    targets_px[:, 2:] *= torch.tensor((w, h, w, h))
+    iouv = torch.linspace(0.5, 0.95, 10)
+    import utils.general as G
+
+    real_time = G.time.time
+    G.time.time = lambda: 0.0  # the reference's wall-clock break (utils/general.py:675,746-748) would drop slow images
+    try:
+        ref_out = ref_nms(pred.clone(), 0.001, 0.6, multi_label=True, max_det=300)
+    finally:
+        G.time.time = real_time
+    for si in range(2):
+        labels = targets_px[targets_px[:, 0] == si, 1:]
+        predn = ref_out[si].clone()
+        ref_scale((h, w), predn[:, :4], shape0, ratio_pad)
+        tbox = xywh2xyxy(labels[:, 1:5])
+        ref_scale((h, w), tbox, shape0, ratio_pad)
+        correct = ref_val.process_batch(predn, torch.cat((labels[:, 0:1], tbox), 1), iouv)
+        out[f"val_nms_{si}"] = ref_out[si].numpy()
+        out[f"val_predn_{si}"] = predn.numpy()
+        out[f"val_correct_{si}"] = correct.numpy()
+    np.savez_compressed(OUT / "seam_cases.npz", **out)
+    # detect.py on the reference's sample images at 640 (tiny model with raised objectness / class biases): the letterboxed
+    # input, z at a fixed seeded sample of SEAM_ROWS anchor rows (the whole z would not fit the fixture), the reference's NMS
+    # of those rows and scale_boxes of its detections
+    cfg = CFG / "yolov3-tiny.yaml"
+    params = O.confident_params(cfg)
+    rm = RefModel(str(ref_shim.reference_root() / "models" / "yolov3-tiny.yaml"))
+    rm.load_state_dict(params, strict=False)
+    rm = rm.eval()
+    for path, im, im0s, _, _ in LoadImages(str(ref_shim.reference_root() / "data" / "images"), img_size=(640, 640), stride=32, auto=True):
+        x = torch.from_numpy(im).float()[None] / 255
+        with torch.no_grad():
+            z = rm(x)[0]
+        rows = torch.randperm(z.shape[1], generator=torch.Generator().manual_seed(0))[:SEAM_ROWS].sort().values
+        zs = z[:, rows].contiguous()
+        det = ref_nms(zs.clone(), 0.25, 0.45, max_det=50)[0]
+        sb = ref_scale(x.shape[2:], det[:, :4].clone(), im0s.shape)
+        np.savez_compressed(OUT / f"seam_detect_{Path(path).stem}.npz", im=im, im0_shape=np.array(im0s.shape), rows=rows.numpy(),
+                            z=zs.numpy(), det=det.numpy(), scaled=sb.numpy())
+        print(f"seam_detect_{Path(path).stem}: im {im.shape}, z rows {len(rows)} of {z.shape[1]}, {det.shape[0]} detections")
+
+
 if __name__ == "__main__":
     assert ref_shim.reference_available(), "run in the build container: /root/reference is required"
     ref_shim.install()
     torch.set_num_threads(8)
-    which = sys.argv[1:] or ["iou", "nms", "loss", "forward", "scale", "val", "tta"]
+    which = sys.argv[1:] or ["iou", "nms", "loss", "forward", "scale", "val", "tta", "seam"]
+    if "seam" in which:
+        gen_seam()
     if "tta" in which:
         gen_tta()
     if "val" in which:

@@ -1,6 +1,6 @@
 """Parity of the BENCHMARKED graph instances (VERDICT r1 weak #1/#2): the 640x640 engines bench.py times — yolov3.yaml
 bs 32 (BASELINE config 2) and yolov3-spp.yaml bs 8 (config 3, per-GPU shard) — against the CPU oracle (== the reference
-forward, models/yolo.py:135-147), including the CUDA-graph replay bench.py uses.  At 640^2 every CTA-pair tile is full,
+forward, models/yolo.py:135-147), including the CUDA-graph replay bench.py uses.  At 640^2
 the deep layers run several waves and the SPP pools see a 20x20 map (models/common.py:281-290) — none of which the 64..160
 pixel goldens exercise.
 

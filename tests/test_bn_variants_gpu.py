@@ -3,7 +3,7 @@ kernels it replaces: same inputs through both, results compared BIT FOR BIT (sam
 dy, the reduced sums and every per-block partial row.  Shapes cover rows shorter than a work unit, row tails, fewer units
 than blocks, c = 16 ... 1024, the SyncBatchNorm phase split and the 2x-upsample layers (which stay on the staged kernel).
 The staged kernels themselves are pinned against torch autograd in tests/test_train_layers_gpu.py.  Same code as the on-device
-A/B of the round (tests/diag/ab_shot.py, profiles/r02_ab_shot_kernel_variants.jsonl)."""
+A/B script tests/diag/ab_shot.py."""
 import pytest
 import torch
 
@@ -23,7 +23,7 @@ def _rnd_act(n, h, w, c, gen, scale=1.0):
     (3, 13, 13, 512, False),     # 832 items per row: one full + one partial unit
     (2, 2, 2, 1024, False),      # the 64x64 test images' deepest layer
     (2, 32, 32, 16, False),      # yolov3-tiny's 16-channel layer
-    (4, 80, 80, 256, False),     # several units per block (one wave of 444 blocks)
+    (4, 80, 80, 256, False),     # several units per block (one wave of 396 blocks)
     (2, 160, 160, 64, False),
     (2, 20, 20, 256, True),      # 2x-upsample layer: both settings run the staged kernel
 ])

@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM conv (y3_conv_bn_act_fwd) and the layer-0 conv against torch fp32 conv2d on identical
+"""wgmma implicit-GEMM conv (y3_conv_bn_act_fwd) and the layer-0 conv against torch fp32 conv2d on identical
 bf16-rounded operands.  Tolerance: the output is stored as bf16 (rel 2^-9) after fp32 accumulation:
 |err| <= 2e-2 + 1e-2*|ref|."""
 import sys

@@ -256,8 +256,8 @@ def _plan(c_in, c_out, k, s, hw, n=32, res=False, head=False, layout=0):
 
 def test_conv_kernel_selection_for_the_yolov3_layers():
     """The variant conv_tc_prepare picks for the distinct conv shapes of yolov3 @640 bs 32 (SURVEY App. A): tile N = c_out
-    bucket, CTA pairs for N >= 128, halo reuse for stride-1 3x3 (N = 256 only as a pair), TMA-store epilogue for stride 1
-    except halo + N = 256, resident weights when one N tile's weights fit in 96 KB, two epilogue groups for N <= 128."""
+    bucket, halo reuse for stride-1 3x3 with N <= 128, resident weights when one N tile's weights fit in 96 KB, one CTA per
+    SM of the H100 (132) at most."""
     from yolov3_b200 import _lib
 
     shapes = [(32, 64, 3, 2, 640, False), (64, 32, 1, 1, 320, False), (32, 64, 3, 1, 320, True), (64, 128, 3, 2, 320, False),
@@ -269,21 +269,19 @@ def test_conv_kernel_selection_for_the_yolov3_layers():
         p = _plan(c_in, c_out, k, s, hw, res=res)
         bn = 32 if c_out <= 32 else 64 if c_out <= 64 else 128 if c_out <= 128 else 256
         assert p["block_n"] == bn and p["block_k"] == (64 if c_in % 64 == 0 else 32), (c_in, c_out, p)
-        assert p["pair"] == int(bn >= 128) and p["epilogue_groups"] == (2 if bn <= 128 else 1), (c_in, c_out, p)
-        assert p["halo"] == int(k == 3 and s == 1), (c_in, c_out, p)
-        assert p["staged"] == int(s == 1 and not (p["halo"] and bn == 256)), (c_in, c_out, p)
+        assert p["halo"] == int(k == 3 and s == 1 and bn <= 128), (c_in, c_out, p)
         n_tiles = -(-c_out // bn)
-        w_bytes = k * k * c_in * (bn // 2 if p["pair"] else bn) * 2
+        w_bytes = k * k * c_in * bn * 2
         assert p["n_tiles"] == n_tiles and p["resident_weights"] == int(n_tiles == 1 and w_bytes <= 96 * 1024), (c_in, c_out, p)
         if s == 1:
             assert p["m_tiles"] == -(-(32 * (hw + 2) * (hw + 2)) // 128)
-        assert 1 <= p["grid"] <= 148 and (p["grid"] % 2 == 0 or not p["pair"])
+        assert 1 <= p["grid"] <= 132 and p["grid"] == min(132, p["m_tiles"] * p["n_tiles"]), (c_in, c_out, p)
     # the first stride-2 layer with x-paired weights: 6 taps of 64 channels, one k-block
     d = _plan(32, 64, 3, 2, 640, layout=_lib.W_XPAIR)
     assert d["xpair"] == 1 and d["block_k"] == 64 and d["k_blocks"] == 1 and d["resident_weights"] == 1
-    # Detect head: fp32 pixel-major output, never staged
+    # Detect head: fp32 pixel-major output
     h = _plan(256, 255, 1, 1, 80, head=True)
-    assert h["block_n"] == 256 and h["staged"] == 0 and h["pair"] == 1
+    assert h["block_n"] == 256 and h["halo"] == 0 and h["n_tiles"] == 1
 
 
 def test_reference_arm_json_contract():
@@ -309,7 +307,7 @@ def test_reference_arm_json_contract():
     assert d["higher_is_better"] is True and d["steps"] == 1 and d["value"] > 0 and d["n_gpus"] == 2
     assert d["config"]["global_batch"] == 64
     assert d["e2e"]["value"] == d["value"] and d["e2e"]["h2d_bytes_per_step"] == 0 and d["e2e"]["d2h_bytes_per_step"] == 0
-    # the reference's own Model from the staged copy (baseline/_ref) when it is there, else the oracle port — and it says which
+    # the reference's own Model from the staged copy (oracle/_ref) when it is there, else the oracle port — and it says which
     sys.path.insert(0, str(root / "oracle"))
     import ref_shim
 

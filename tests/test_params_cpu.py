@@ -82,27 +82,23 @@ def test_flat_store_layout_and_groups(name):
 
 
 def test_reference_smart_optimizer_groups_agree():
-    """The same three groups from the REFERENCE's smart_optimizer run on the nn.Module facade (when the reference is around)."""
-    import ref_shim
-
-    if not ref_shim.reference_available():
-        pytest.skip("reference not staged")
-    ref_shim.install()
-    from utils.torch_utils import smart_optimizer
+    """The same three groups as the REFERENCE's smart_optimizer built on the nn.Module facade (its groups and their settings
+    are recorded in tests/golden/seam_cases.npz by make_golden.py)."""
+    import numpy as np
 
     from yolov3_b200 import params as P
     from yolov3_b200.module import DetectionModel
 
+    g = np.load(Path(__file__).resolve().parent / "golden" / "seam_cases.npz")
     dm = DetectionModel(CFG / "yolov3-tiny.yaml", device="cpu")
     st = dm.core.store()
-    opt = smart_optimizer(dm, "SGD", lr=0.01, momentum=0.937, decay=5e-4)
-    by_ptr = {st.views[n].data_ptr(): n for n in st.order if st.slots[n].group != P.G_FROZEN}
+    names = {n for n in st.order if st.slots[n].group != P.G_FROZEN}
     got = {}
-    for grp, tag in zip(opt.param_groups, (P.G_BIAS, P.G_DECAY, P.G_BN)):  # smart_optimizer: g2 first, then g0 (decay), g1
-        for p in grp["params"]:
-            got[by_ptr[p.data_ptr()]] = tag
-        assert (grp["weight_decay"] > 0) == (tag == P.G_DECAY)
-    assert got == {n: st.slots[n].group for n in by_ptr.values()}
+    for gi, tag in enumerate((P.G_BIAS, P.G_DECAY, P.G_BN)):  # smart_optimizer: g2 first, then g0 (decay), g1
+        for n in g[f"opt_yolov3-tiny_g{gi}_names"]:
+            got[str(n)] = tag
+        assert (g[f"opt_yolov3-tiny_g{gi}_hyp"][3] > 0) == (tag == P.G_DECAY)
+    assert got == {n: st.slots[n].group for n in names}
 
 
 @pytest.mark.parametrize("name,n_buckets", [("yolov3", 4), ("yolov3", 1), ("yolov3", 7), ("yolov3-tiny", 4)])

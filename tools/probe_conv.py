@@ -1,9 +1,10 @@
-"""GPU probe: run the tcgen05 conv kernel over a battery of shapes and compare with torch fp32 conv2d on the same
+"""GPU probe: run the wgmma conv kernel over a battery of shapes and compare with torch fp32 conv2d on the same
 bf16-rounded operands.  Each case runs in its own subprocess under a timeout so that a trap in one case cannot take
-the others down.  Usage: python tools/probe_conv.py [--out gpurun_out/probe_conv.jsonl] [case_index]"""
+the others down.  Usage: python tools/probe_conv.py [--out FILE.jsonl] [case_index]  (default: probe_conv.jsonl in the system temp directory)"""
 import json
 import subprocess
 import sys
+import tempfile
 from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
@@ -129,7 +130,7 @@ def run_case(c):
 
 
 def main():
-    out = Path("gpurun_out/probe_conv.jsonl")
+    out = Path(tempfile.gettempdir()) / "probe_conv.jsonl"
     args = sys.argv[1:]
     if "--out" in args:
         out = Path(args[args.index("--out") + 1])

@@ -3,7 +3,7 @@
   python tools/probe_layer.py --cin 32 --cout 64 --k 3 --s 2 --hw 640 --n 32 [--res] [--iters 5] [--time]
 
 With --time prints the CUDA-event average over the iterations (inputs of the big early layers exceed L2 on their own).
-Environment toggles of the library (Y3_CONV_PAIR / _STAGED / _HALO / _BRES) apply."""
+Environment toggles of the library (Y3_CONV_HALO / _BRES) apply."""
 import argparse
 import sys
 from pathlib import Path

@@ -1,10 +1,10 @@
-"""Per-kernel SASS mnemonic histogram of the built library (profiles/r02_sass_histogram.txt).
+"""Per-kernel SASS mnemonic histogram of the built library.
 
-    python tools/sass_histogram.py > profiles/r02_sass_histogram.txt
+    python tools/sass_histogram.py
 
 Runs `cuobjdump -sass` on yolov3_b200/libyolov3_b200.so (no GPU needed) and counts, for every kernel, the instructions that
-prove which hardware path it takes: UTCHMMA (tcgen05.mma; .2CTA = cta_group::2), LDTM (tcgen05.ld), UTMALDG / UTMASTG (TMA load /
-store), UTCBAR (tcgen05.commit), SYNCS (mbarrier), ACQBULK / PREEXIT (griddepcontrol.wait / launch_dependents: programmatic
+prove which hardware path it takes: HGMMA (wgmma), WARPGROUP (wgmma fences / waits), UTMALDG / UTMASTG (TMA load / store),
+SYNCS (mbarrier), ACQBULK / PREEXIT (griddepcontrol.wait / launch_dependents: programmatic
 dependent launch), HMMA / IMMA (legacy mma.sync: only the 3-channel stem conv and the fallback wgrad), MUFU, REDUX, ATOM/ATOMS/RED,
 LDGSTS (cp.async: the shared-memory ring of the BatchNorm backward passes).
 """
@@ -16,7 +16,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parents[1]
 LIB = ROOT / "yolov3_b200" / "libyolov3_b200.so"
-KEYS = ["UTCHMMA", "UTCHMMA.2CTA", "LDTM", "UTMALDG", "UTMASTG", "UTCBAR", "SYNCS", "ACQBULK", "PREEXIT", "HMMA", "IMMA", "MUFU", "REDUX", "ATOM", "ATOMS", "RED", "LDG", "STG", "LDGSTS"]
+KEYS = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "SYNCS", "ACQBULK", "PREEXIT", "HMMA", "IMMA", "MUFU", "REDUX", "ATOM", "ATOMS", "RED", "LDG", "STG", "LDGSTS"]
 
 
 def demangle(names):
@@ -43,10 +43,8 @@ def main():
         base = op.split(".")[0]
         if base in KEYS:
             per[cur][base] += 1
-        if base == "UTCHMMA" and ".2CTA" in op:
-            per[cur]["UTCHMMA.2CTA"] += 1
     names = demangle(list(per))
-    print(f"# cuobjdump -sass {LIB.relative_to(ROOT)}  ({len(per)} kernels; sm_100a)")
+    print(f"# cuobjdump -sass {LIB.relative_to(ROOT)}  ({len(per)} kernels; sm_90a)")
     print("# columns: " + " ".join(KEYS) + " | total instructions | kernel")
     for k, c in per.items():
         total.update(c)

@@ -1,4 +1,4 @@
-"""yolov3_b200 — Blackwell-native (sm_100a) YOLOv3 detection hot path behind the ultralytics/yolov3 Python seams.
+"""yolov3_b200 — Hopper-native (sm_90a, H100) YOLOv3 detection hot path behind the ultralytics/yolov3 Python seams.
 
 Public surface mirrors the reference's (SURVEY.md §8b); every name below resolves lazily to its module (importing the package
 costs nothing and never touches the GPU).  All compute runs in the hand-written CUDA library ``libyolov3_b200.so`` through

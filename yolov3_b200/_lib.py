@@ -36,8 +36,8 @@ class ConvDesc(C.Structure):
 class ConvPlanInfo(C.Structure):
     """struct y3_conv_plan_info."""
 
-    _fields_ = [(k, C.c_int32) for k in ("block_n", "block_k", "pair", "staged", "halo", "resident_weights", "epilogue_groups",
-                                         "xpair", "m_tiles", "n_tiles", "k_blocks", "grid")]
+    _fields_ = [(k, C.c_int32) for k in ("block_n", "block_k", "halo", "resident_weights", "xpair", "m_tiles", "n_tiles",
+                                         "k_blocks", "grid")]
 
 
 W_TAPS, W_XPAIR = 0, 1

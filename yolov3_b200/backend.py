@@ -1,5 +1,5 @@
 """``DetectMultiBackend`` — the reference's own backend-plugin point (models/common.py:435-476, ``pt`` branch; callers
-detect.py:166,183,196, val.py:293,324,364, hubconf.py:63) with the B200 ``Model`` behind it: same constructor arguments,
+detect.py:166,183,196, val.py:293,324,364, hubconf.py:63) with the GPU ``Model`` behind it: same constructor arguments,
 same attributes (``stride names pt jit engine fp16 device triton model nhwc``), ``forward(im, augment, visualize)``,
 ``warmup(imgsz)`` and ``from_numpy``.  Only the PyTorch (``pt``) role exists here; there is no CPU device."""
 from __future__ import annotations
@@ -59,7 +59,7 @@ class DetectMultiBackend:
     def __init__(self, weights="yolov3.pt", device=torch.device("cuda"), dnn=False, data=None, fp16=False, fuse=True):  # noqa: B008
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("yolov3_b200 has no CPU path: DetectMultiBackend needs a CUDA (B200) device")
+            raise RuntimeError("yolov3_b200 has no CPU path: DetectMultiBackend needs a CUDA (H100) device")
         if dnn:
             raise NotImplementedError("only the PyTorch ('pt') role of DetectMultiBackend is accelerated")
         if isinstance(weights, (list, tuple)) and len(weights) > 1:  # models/common.py:471: attempt_load(weights list) -> Ensemble

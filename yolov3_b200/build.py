@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI shared library (nvcc, sm_100a only).  The .so lands next to this file so that it
+"""In-tree build of the C-ABI shared library (nvcc, sm_90a only).  The .so lands next to this file so that it
 travels with the repo snapshot to the GPU box; it is git-ignored."""
 from __future__ import annotations
 
@@ -10,7 +10,8 @@ from pathlib import Path
 PKG = Path(__file__).resolve().parent
 CSRC = PKG / "csrc"
 LIB = PKG / "libyolov3_b200.so"
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-diag-suppress", "177",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-diag-suppress", "177",
               "--use_fast_math", "-shared"]
 # kernels whose arithmetic must match the reference bit for bit are compiled without fast-math / FMA contraction
 EXACT_SOURCES = {"y3_nms.cu", "y3_detect.cu", "y3_loss.cu", "y3_iou.cu", "y3_val.cu", "y3_pre.cu", "y3_tta.cu"}
@@ -60,7 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         if verbose and out.strip():
             print(out)
     tmp = LIB.with_suffix(".so.tmp")
-    link = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", str(tmp), *objs]
+    link = [nvcc, *ARCH, "-shared", "-o", str(tmp), *objs]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}")

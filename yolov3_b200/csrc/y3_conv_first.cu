@@ -1,7 +1,6 @@
 // yolov3_b200 — layer-0 convolution (c_in = 3): 3x3 stride-1 pad-1 on the NCHW image (fp32, or uint8 with the /255 of
 // detect.py:190 fused) with folded BN + SiLU, fused with the NCHW -> padded-NHWC-bf16 conversion.  Bandwidth-bound
-// (24.7 FLOP/B, SURVEY App. A).  v1 was one thread per pixel with fp32 FMAs (970 us @bs32, LDS/FMA-bound, see
-// profiles/r01_per_op_v1_baseline.json); this version feeds warp-level bf16 MMAs from a shared-memory patch.
+// (24.7 FLOP/B, SURVEY App. A).  v1 was one thread per pixel with fp32 FMAs (LDS/FMA-bound); this version feeds warp-level bf16 MMAs from a shared-memory patch.
 // Also the test-only layout converters.
 // Replaces Conv.forward_fuse for model.0 (reference models/common.py:77-81, models/yolov3.yaml:18).
 #include "y3_common.cuh"
@@ -40,7 +39,7 @@ __device__ __forceinline__ float4 load_px4<uint8_t>(const uint8_t* p, float div)
   return v;
 }
 
-// Tensor-core version (legacy warp-level mma.sync m16n8k16: K = 27 padded to 32 is far too thin for a tcgen05 tile and
+// Tensor-core version (legacy warp-level mma.sync m16n8k16: K = 27 padded to 32 is far too thin for a wgmma tile and
 // the layer is bandwidth-bound anyway).  One block = 128 consecutive pixels of one image row; the 3x3x(128+2) input
 // patch is staged in shared memory with coalesced loads, each warp then builds the im2col A fragments for its 32 pixels
 // straight from smem, multiplies by the [32 x COUT] bf16 weight fragments held in registers, and stores bf16 NHWC.
@@ -56,7 +55,7 @@ constexpr int kFirstTW = 128;   // output columns per block
 
 // VEC: W % 4 == 0 and the image base is 16-byte (fp32) / 4-byte (uint8) aligned: the patch rows are staged with one
 // vector load per lane, all 8 rows a warp owns in flight at once.  The scalar staging loop kept ~5 dependent 4-byte loads
-// per thread in flight and 46 % of the kernel's stall samples sat on its STS (profiles/r01_ncu_conv_first_summary.txt).
+// per thread in flight and most of the kernel's stall samples sat on its STS.
 template <int COUT, typename TIN, bool VEC>
 __global__ void __launch_bounds__(128) conv_first_kernel(const TIN* __restrict__ in, float in_div, int H, int W,
                                                          const float* __restrict__ wgt, const float* __restrict__ bias,

@@ -1,6 +1,6 @@
-// yolov3_b200 — implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM),
-// operands staged by TMA, folded-BN bias + SiLU (+ residual, + nearest-2x upsample, + concat-offset / Detect store)
-// fused into the epilogue.  Replaces Conv.forward_fuse (reference models/common.py:77-81) and the adds/copies around it.
+// yolov3_b200 — implicit-GEMM convolution on the Hopper tensor cores (wgmma, fp32 accumulators in registers), operands
+// staged by TMA, folded-BN bias + SiLU (+ residual, + nearest-2x upsample, + concat-offset / Detect store) fused into the
+// epilogue.  Replaces Conv.forward_fuse (reference models/common.py:77-81) and the adds/copies around it.
 //
 // GEMM view:  D[pixel, cout] = sum_{tap, c} A[pixel shifted by tap, c] * W[cout, tap, c]
 //   * activations are bf16 "padded NHWC" [n, h+2, w+2, ld] with an all-zero halo, so for a stride-1 conv the A tile
@@ -10,13 +10,11 @@
 //   * a stride-2 conv reads the same buffer through a 5-D view (2*ld, (w+2)/2, 2, (h+2)/2, n) that splits rows and
 //     columns by parity; the A tile of tap (r,s) for a TH x TW patch of output pixels is one 5-D TMA box ("patch").
 //   * weights are bf16 [cout_pad, taps*cin] (K-major); B tile = [BLOCK_N x BLOCK_K] box.
-// Warp roles (320 or 576 threads, 1 CTA/SM, persistent over tiles): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer
-// (both run warp-uniform loops and elect one lane per issue), warps 2.. = epilogue, 8 warps per group (TMEM -> registers ->
-// global / swizzled smem + TMA store; two warps per TMEM lane quarter, each taking half of the tile's columns); tiles with
-// N <= 128 run two groups, group g converting the tiles of TMEM accumulator buffer g.  smem ring of STAGES {A,B} tiles; two
-// accumulator buffers in TMEM so the epilogue of tile i overlaps the main loop of tile i+1.  What bounded what, measured on
-// B200: profiles/r01_ncu_*.txt (epilogue MUFU/issue -> 8 warps + one-MUFU SiLU; SM operand ingress -> CTA pairs; TMA row
-// rate -> halo reuse; single-lane issue loops -> elect.sync; lock-step epilogue -> per-warp TMA + private bias slices).
+// Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warp 8 = TMA producer (the whole warp runs the loop, one elected
+// lane issues); warpgroups 0 and 1 (warps 0-7) = consumers, each owning 64 of the tile's 128 rows: it issues the
+// m64 x BLOCK_N wgmma of its rows for every stage of the smem ring, releases a stage as soon as the MMAs that read it have
+// completed, and after the last k-block converts its accumulators straight from the registers (bias, SiLU, residual,
+// bf16 / fp32 stores).  While the consumers run the epilogue the producer already fills the ring for their next tile.
 #include <cuda_bf16.h>
 
 #include <cstdlib>
@@ -30,82 +28,50 @@ namespace y3 {
 namespace {
 
 constexpr int kBlockM = 128;
-constexpr int kEpilogueWarps = 8;
-constexpr int kSmemBudget = 221 * 1024;  // ring + epilogue staging; alignment slack, barriers and bias slices come on top (227 KB max)
+// two consumer warpgroups + one producer warp: no idle warps, up to 224 registers per thread (the N = 256 tiles keep 128
+// accumulators each)
+constexpr int kThreads = 288;
+constexpr int kProducerWarp = 8;
+constexpr int kSmemBudget = 221 * 1024;  // ring (+ resident weights); alignment slack and barriers come on top (227 KB max)
 
-// STAGED = true (stride 1, bf16 output): each epilogue warp converts its 32 tile rows into a swizzled shared-memory
-// staging tile and stores them with its own TMA box (and pre-loads its residual rows into the same place with TMA),
-// instead of every thread issuing 16-byte global stores to 32 different cache lines per instruction.
 // HALO = true (stride-1 3x3, BLOCK_K = 64 or 32): one pipeline stage covers a whole filter ROW (3 taps): the A operand is
-// ONE TMA box of 128+2 consecutive pixels and the three taps read it at row offsets 0/1/2 through UMMA descriptors whose
-// start address is not aligned to the 1 KB swizzle pattern (the swizzle is a function of the absolute address, so the
-// descriptor's base_offset stays 0 — verified on hardware, see halo_enabled()).  A rows fetched per k-block drop from
-// 9*128 to 3*130 and the producer / MMA warps run a third of the pipeline stages.
-template <int BLOCK_N, int BLOCK_K, bool PAIR, bool STAGED, bool HALO>
+// ONE TMA box of 128+2 consecutive pixels and the three taps read it at row offsets 0/1/2 through wgmma descriptors whose
+// start address is not aligned to the swizzle pattern (the swizzle is a function of the absolute shared-memory address,
+// so the descriptor's base offset stays 0).  A rows fetched per k-block drop from 9*128 to 3*130 and the producer runs a
+// third of the pipeline stages.
+template <int BLOCK_N, int BLOCK_K, bool HALO>
 struct Cfg {
   static constexpr uint32_t kARows = HALO ? kBlockM + 2 : kBlockM;
   static constexpr uint32_t kATxBytes = kARows * BLOCK_K * 2;                         // bytes one A box delivers (flat mode)
   static constexpr uint32_t kABytes = (kATxBytes + 1023u) / 1024u * 1024u;            // slot size, 1 KB aligned
   static constexpr uint32_t kTaps = HALO ? 3 : 1;                                     // filter taps per stage
-  static constexpr uint32_t kBRows = PAIR ? BLOCK_N / 2 : BLOCK_N;  // a CTA pair splits the B tile between its two CTAs
-  static constexpr uint32_t kBBytes = kBRows * BLOCK_K * 2;
+  static constexpr uint32_t kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr uint32_t kStageBytes = kABytes + kTaps * kBBytes;
-  static constexpr uint32_t kSlabCols = BLOCK_N >= 64 ? 64 : 32;          // staging slab = [128 rows][kSlabCols bf16]
-  static constexpr uint32_t kSlabRowBytes = kSlabCols * 2;                // 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B)
-  static constexpr uint32_t kSlabBytes = kBlockM * kSlabRowBytes;
-  static constexpr uint32_t kSlabs = BLOCK_N / kSlabCols;
-  // two staging tiles per group for N <= 64: the residual of tile i+1 is TMA-loaded while tile i is converted and stored,
-  // so the epilogue of the thin layers does not expose one L2/HBM round trip per tile (their k-loop is ~600 clk long);
-  // N = 128 has one buffer per group (shared-memory budget) and relies on the other group to cover that latency
-  static constexpr uint32_t kStgTile = kBlockM * BLOCK_N * 2;
-  static constexpr uint32_t kStgBufs = BLOCK_N <= 64 ? 2 : 1;   // per epilogue group (two: residual prefetch one tile ahead)
-  // Thin tiles (N <= 64) can run TWO epilogue groups of 8 warps, group g converting the tiles of TMEM buffer g: their
-  // epilogue is issue-latency-bound (IPC ~1.5 with 2 warps per scheduler), more resident warps fill the issue slots.
-  static constexpr int kMaxGroups = BLOCK_N <= 128 ? 2 : 1;  // N = 256 kernels need > 112 registers per thread
-  static constexpr int kMaxThreads = 64 + 32 * kEpilogueWarps * kMaxGroups;
-  static constexpr uint32_t kStagingBytes = STAGED ? kMaxGroups * kStgBufs * kStgTile : 0;
   static constexpr int kMaxStages = 8;
-  static constexpr int kStagesRaw = (kSmemBudget - kStagingBytes) / kStageBytes;
+  static constexpr int kStagesRaw = kSmemBudget / kStageBytes;
   static constexpr int kStages = kStagesRaw > kMaxStages ? kMaxStages : kStagesRaw;
   // B-resident mode: `steps` weight boxes of kBBytes stay in shared memory for the whole kernel; the ring carries A only
   __host__ __device__ static constexpr uint32_t bres_bytes(int steps) { return (uint32_t(steps) * kBBytes + 1023u) / 1024u * 1024u; }
   __host__ __device__ static constexpr int bres_stages(int steps) {
-    const int s = (int(kSmemBudget) - int(kStagingBytes) - int(bres_bytes(steps))) / int(kABytes);
+    const int s = (int(kSmemBudget) - int(bres_bytes(steps))) / int(kABytes);
     return s > kMaxStages ? kMaxStages : s;
   }
-  static constexpr uint32_t kTmemCols = 2 * BLOCK_N < 32 ? 32 : 2 * BLOCK_N;  // power of two for N in {32,64,128,256}
-  static constexpr uint32_t kSwizzleBytes = BLOCK_K * 2;                       // 32 / 64 / 128
-  static constexpr uint32_t kLayout = BLOCK_K == 64 ? 2u : (BLOCK_K == 32 ? 4u : 6u);
+  static constexpr uint32_t kSwizzleBytes = BLOCK_K * 2;  // 32 / 64 / 128: one smem row of an operand tile
   static constexpr uint32_t kSbo = 8 * kSwizzleBytes;
-  static constexpr uint32_t kColsPerWarp = BLOCK_N >= 64 ? BLOCK_N / 2 : BLOCK_N;  // columns one epilogue warp converts
-  static constexpr uint32_t kBarBytes = 512;                                       // mbarriers + TMEM slot
-  static constexpr uint32_t kBiasBytes = kMaxGroups * kEpilogueWarps * kColsPerWarp * 4;  // one private bias slice per warp
-  static constexpr size_t kSmemBytes = size_t(kSmemBudget) + 1024 /*align*/ + kBarBytes + kBiasBytes;
+  static constexpr uint32_t kBarBytes = 256;              // mbarriers
+  static constexpr size_t kSmemBytes = size_t(kSmemBudget) + 1024 /*align*/ + kBarBytes;
   static_assert(kStages >= 2, "pipeline needs at least two stages");
   static_assert(!HALO || BLOCK_K >= 32, "halo reuse: rows of 64 or 128 bytes");
 };
 
-// accumulator chunk + bias (+ SiLU).  SiLU(x) = h + h*tanh(h) with h = x/2 = fma(acc, 0.5, b/2): the bias slice holds
-// b/2 for SiLU layers, so bias add and halving are one FFMA (bit-identical: scaling by 0.5 is exact) — 3 instructions
-// per element; the thin layers' epilogue is issue-bound (profiles/r01_ncu_issue_loop.txt).
-__device__ __forceinline__ void bias_act(const uint32_t (&v)[32], const float* __restrict__ sb, float (&x)[32], bool silu) {
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {
-    const float4 b = *reinterpret_cast<const float4*>(sb + j);
-    const float bb[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float a = __uint_as_float(v[j + e]);
-      if (silu) {
-        const float h = fmaf(a, 0.5f, bb[e]);
-        float t;
-        asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
-        x[j + e] = fmaf(h, t, h);
-      } else {
-        x[j + e] = a + bb[e];
-      }
-    }
-  }
+// bias (+ SiLU) of one accumulator.  SiLU(x) = h + h*tanh(h) with h = x/2 = fma(acc, 0.5, b/2): `b` holds b/2 for SiLU
+// layers, so bias add and halving are one FFMA (bit-identical: scaling by 0.5 is exact) — one MUFU op per element.
+__device__ __forceinline__ float bias_act(float a, float b, bool silu) {
+  if (!silu) return a + b;
+  const float h = fmaf(a, 0.5f, b);
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
+  return fmaf(h, t, h);
 }
 
 // exact n / d for any 32-bit n with a precomputed (multiplier, shift) pair (host: fast_div_for)
@@ -114,582 +80,275 @@ __device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t mul, uint32_t 
   return (t + ((n - t) >> (shr ? 1 : 0))) >> (shr ? shr - 1 : 0);
 }
 
-// PAIR = true: two CTAs of a cluster (one SM pair) cooperate on a 256-row tile with tcgen05 cta_group::2: each CTA
-// stages its own 128 A rows and HALF of the B tile, the leader CTA's single MMA thread issues M=256 MMAs that read both
-// CTAs' shared memory and write both CTAs' TMEM.  Per-SM operand ingress drops from (128+N)*K to (128+N/2)*K bytes per
-// k-block — the 1-CTA kernel measured ~0.67 of the MMA rate on the big 3x3 layers because (128+256)*64*2 B per 512 MMA
-// cycles exceeds the ~64 B/clk an SM can pull from L2 (profiles/r01_per_op_v2_epilogue.json).
-template <int BLOCK_N, int BLOCK_K, bool PAIR, bool STAGED, bool HALO>
-__global__ void __launch_bounds__((Cfg<BLOCK_N, BLOCK_K, PAIR, STAGED, HALO>::kMaxThreads), 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res,
-               const ConvTcArgs p) {
-  using C = Cfg<BLOCK_N, BLOCK_K, PAIR, STAGED, HALO>;
+// where accumulator row m of tile (mt, n0) goes: null pointers for halo / out-of-range rows
+struct RowOut {
+  __nv_bfloat16* out;       // bf16 output (first of the 4 upsampled copies)
+  float* f32;               // fp32 pixel-major output (Detect heads)
+  const __nv_bfloat16* res; // residual
+};
+
+__device__ __forceinline__ RowOut row_out(const ConvTcArgs& p, int mt, int n0, int m) {
+  RowOut o{nullptr, nullptr, nullptr};
+  bool valid;
+  int img, oy, ox;  // image, UNPADDED output coordinates
+  if (p.mode == 0) {
+    const int row = mt * kBlockM + m;
+    const int plane = p.hp * p.wp;
+    img = static_cast<int>(fast_div(static_cast<uint32_t>(row), p.plane_mul, p.plane_shr));
+    const int rem = row - img * plane;
+    const int yp = static_cast<int>(fast_div(static_cast<uint32_t>(rem), p.wp_mul, p.wp_shr)), xp = rem - yp * p.wp;
+    valid = row < p.rows_total && yp >= 1 && yp <= p.hp - 2 && xp >= 1 && xp <= p.wp - 2;
+    oy = yp - 1;
+    ox = xp - 1;
+  } else {
+    const int per_img = p.tiles_w * p.tiles_h;
+    img = mt / per_img;
+    const int t = mt - img * per_img;
+    const int ty = m / p.tw, tx = m - ty * p.tw;
+    oy = (t / p.tiles_w) * p.th + ty;
+    ox = (t % p.tiles_w) * p.tw + tx;
+    valid = ty < p.th && oy < p.ho && ox < p.wo;
+  }
+  if (!valid) return o;
+  const int oh = p.mode == 0 ? p.hp - 2 : p.ho;  // conv-output height/width (unpadded)
+  const int ow = p.mode == 0 ? p.wp - 2 : p.wo;
+  long long conv_row = (static_cast<long long>(img) * (oh + 2) + oy + 1) * (ow + 2) + ox + 1;
+  if (p.phase)  // one parity class of a transposed stride-2 conv: (oy, ox) -> (2 oy + a, 2 ox + b) of the 2x grid
+    conv_row = (static_cast<long long>(img) * (2 * oh + 2) + 2 * oy + p.ph_a + 1) * (2 * ow + 2) + 2 * ox + p.ph_b + 1;
+  if (p.res) o.res = p.res + conv_row * p.res_ld + p.res_coff + n0;
+  if (p.out_f32) {
+    o.f32 = p.out_f32 + ((static_cast<long long>(img) * oh + oy) * ow + ox) * p.out_f32_ld + n0;
+  } else if (p.upsample) {
+    const long long r00 = (static_cast<long long>(img) * (2 * oh + 2) + 2 * oy + 1) * (2 * ow + 2) + 2 * ox + 1;
+    o.out = p.out + r00 * p.out_ld + p.out_coff + n0;
+  } else {
+    o.out = p.out + conv_row * p.out_ld + p.out_coff + n0;
+  }
+  return o;
+}
+
+template <int BLOCK_N, int BLOCK_K, bool HALO>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const ConvTcArgs p) {
+  using C = Cfg<BLOCK_N, BLOCK_K, HALO>;
   const int STAGES = p.stages;
   const bool bres = p.bres != 0;
   constexpr uint32_t kBStage = C::kTaps * C::kBBytes;  // B bytes per stage (ring mode)
   const int b_steps = p.taps * p.kblocks;             // weight boxes of one N tile (resident mode keeps them all)
-  constexpr uint32_t IDESC = umma_idesc_bf16(PAIR ? 256 : 128, BLOCK_N);
-  constexpr uint32_t kEpiThreads = 32 * kEpilogueWarps;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
-  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);  // swizzled TMA/UMMA tiles need 1 KB alignment
+  uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);  // swizzled TMA / wgmma tiles need 1 KB alignment
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * C::kABytes;  // ring of B stages, or the resident weight tile
-  uint8_t* smem_stg = smem_b + (bres ? C::bres_bytes(b_steps) : uint32_t(STAGES) * kBStage);  // 1 KB aligned
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_stg + C::kStagingBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + (bres ? C::bres_bytes(b_steps) : uint32_t(STAGES) * kBStage));
   uint64_t* empty_bar = full_bar + C::kMaxStages;
-  uint64_t* tfull_bar = empty_bar + C::kMaxStages;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* res_bar = tempty_bar + 2;  // [16 epilogue warps / row-group owners][2 staging buffers]
-  uint64_t* bres_bar = res_bar + 32;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bres_bar + 1);
-  // bias of the current N tile.  Read through __ldg it missed the (almost entirely shared-memory) L1 and exposed an L2
-  // round trip per 32-column chunk: 29 % of all warp stall samples of the epilogue (profiles/r01_ncu_conv_tc_full_summary.txt).
-  float* s_bias = reinterpret_cast<float*>(smem_stg + C::kStagingBytes + C::kBarBytes);
+  uint64_t* bres_bar = empty_bar + C::kMaxStages;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;  // 0 = leader
-  const int n_workers = PAIR ? gridDim.x / 2 : gridDim.x;
-  const int worker = PAIR ? blockIdx.x / 2 : blockIdx.x;
 
-  if (PAIR) cluster_sync_all();  // both CTAs are resident before the pair-wide TMEM allocation
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
     for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], PAIR ? 2 : 1);  // pair: leader's expect_tx arrive + peer's remote arrive
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], PAIR ? 2 * kEpiThreads : kEpiThreads);  // pair: both CTAs' epilogues release the buffer
-    }
-    for (int i = 0; i < 32; ++i) mbar_init(&res_bar[i], 1);
-    mbar_init(bres_bar, PAIR ? 2 : 1);
-    if (STAGED) {
-      tma_prefetch_desc(&map_out);
-      if (p.res) tma_prefetch_desc(&map_res);
-    }
+    mbar_init(bres_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if (PAIR) {
-      tmem_alloc_pair(tmem_slot, C::kTmemCols);
-      tmem_relinquish_pair();
-    } else {
-      tmem_alloc(tmem_slot, C::kTmemCols);
-      tmem_relinquish();
-    }
-  }
-  tc_fence_before();
-  if (PAIR) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // everything above touched only shared memory, TMEM and the kernel parameters: it may run while the previous kernel of the
+  __syncthreads();
+  // everything above touched only shared memory and the kernel parameters: it may run while the previous kernel of the
   // stream drains.  From here on global memory is read and written.
   pdl_wait();
   pdl_trigger();
 
-  const int m_units = PAIR ? (p.m_tiles + 1) / 2 : p.m_tiles;  // a pair owns two consecutive M tiles
-  const int total_tiles = m_units * p.n_tiles;
+  const int total_tiles = p.m_tiles * p.n_tiles;
   const int k_iters = HALO ? 3 * p.kblocks : p.taps * p.kblocks;  // HALO: one iteration = one filter row of one k-block
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ------------------------------------------------------------------ TMA producer
-    // The WHOLE warp runs the loop in warp-uniform control flow and one elected lane issues the copies.  With a single
-    // active thread (if (lane == 0)) the compiler cannot prove that the operands of UTMALDG / UTCHMMA are uniform and
-    // wraps every one of them in ELECT + R2UR.BROADCAST: ~110 dependent instructions (~790 clk) per pipeline stage,
-    // which — not the tensor pipe — paced every layer with short k-loops (profiles/r01_ncu_issue_loop.txt).
-    {
-      uint32_t stage = 0, phase = 0;
-      if (bres && worker < total_tiles && elect_one()) {
-        // resident weights (single N tile): every (k-block, tap) box once, all credited to one barrier
-        const int n0 = static_cast<int>(rank) * C::kBRows;
-        const uint32_t bytes = uint32_t(b_steps) * C::kBBytes;
-        if (PAIR) {
-          const uint32_t bar_addr = mapa_u32(smem_u32(bres_bar), 0);
-          if (rank == 0)
-            mbar_expect_tx(bres_bar, 2 * bytes);
-          else
-            mbar_arrive_cluster(bar_addr);
-          for (int st = 0; st < b_steps; ++st) {
-            const int kb = st / p.taps, tap = st - kb * p.taps;
-            tma_load_2d_pair(smem_b + st * C::kBBytes, &map_b, bar_addr, (p.custom_taps ? p.tap_wcol[tap] : tap) * p.cin + kb * BLOCK_K, n0);
-          }
-        } else {
-          mbar_expect_tx(bres_bar, bytes);
-          for (int st = 0; st < b_steps; ++st) {
-            const int kb = st / p.taps, tap = st - kb * p.taps;
-            tma_load_2d(smem_b + st * C::kBBytes, &map_b, bres_bar, (p.custom_taps ? p.tap_wcol[tap] : tap) * p.cin + kb * BLOCK_K, n0);
-          }
-        }
+    // The WHOLE warp runs the loop in warp-uniform control flow and one elected lane issues the copies: with a single
+    // active thread (if (lane == 0)) the compiler cannot prove that the TMA operands are uniform.
+    uint32_t stage = 0, phase = 0;
+    if (bres && int(blockIdx.x) < total_tiles && elect_one()) {
+      // resident weights (single N tile): every (k-block, tap) box once, all credited to one barrier
+      mbar_expect_tx(bres_bar, uint32_t(b_steps) * C::kBBytes);
+      for (int st = 0; st < b_steps; ++st) {
+        const int kb = st / p.taps, tap = st - kb * p.taps;
+        tma_load_2d(smem_b + st * C::kBBytes, &map_b, bres_bar, (p.custom_taps ? p.tap_wcol[tap] : tap) * p.cin + kb * BLOCK_K, 0);
       }
-      // loop-invariant parameters in registers, and one copy of the tile loop per addressing mode: this loop runs on a
-      // single lane's issue slots (~5 clk per dependent instruction), every instruction in it is paid per pipeline stage
-      const int n_tiles = p.n_tiles, kblocks = p.kblocks, wp = p.wp, cin = p.cin, a_coff = p.a_coff, a_ld = p.a_ld;
-      const int taps_it = HALO ? 3 : p.taps;  // HALO: tap = filter row r
-      const bool xpair = p.xpair != 0, nine = p.taps == 9, custom = p.custom_taps != 0;
-      const int taps_w = xpair ? 2 : 3;       // taps per filter row
-      const uint32_t stage_tx = p.a_tx_bytes + (bres ? 0u : kBStage);
-      auto run = [&](auto mode_tag) {
-        constexpr int MODE = decltype(mode_tag)::value;
-        for (int tile = worker; tile < total_tiles; tile += n_workers) {
-          const int nt = tile % n_tiles;
-          const int mt = PAIR ? (tile / n_tiles) * 2 + static_cast<int>(rank) : tile / n_tiles;
-          const int n0 = nt * BLOCK_N + static_cast<int>(rank) * C::kBRows;  // this CTA's slice of the weight tile
-          int row0 = 0, img = 0, oh0 = 0, ow0 = 0;
-          if (MODE == 0) {
-            row0 = mt * kBlockM;
-          } else {
-            const int per_img = p.tiles_w * p.tiles_h;
-            img = mt / per_img;
-            const int t = mt - img * per_img;
-            oh0 = (t / p.tiles_w) * p.th;
-            ow0 = (t % p.tiles_w) * p.tw;
-          }
-          // (k-block kb, tap) advance incrementally: a runtime division per stage was a quarter of the loop
-          int kb = 0, tap = 0, r = 0, s = 0;  // tap = r * taps_w + s  (1x1: always 0)
-          for (int it = 0; it < k_iters; ++it) {
-            mbar_wait(&empty_bar[stage], phase ^ 1u, p.err, 1);
-            if (elect_one()) {
-              uint8_t* a_dst = smem_a + stage * C::kABytes;
-              uint8_t* b_dst = smem_b + stage * kBStage;
-              const int kcol = kb * BLOCK_K;
-              // flat mode: the tap's A box is the tile's pixel rows shifted by (r-1)*wp + (s-1) (HALO: a whole filter row)
-              const int shift = HALO ? (tap - 1) * wp - 1 : (custom ? p.tap_shift[tap] : (nine ? (r - 1) * wp + (s - 1) : 0));
-              // patch mode: filter row r, column s.  x-paired weights (stride 2, in_ld == c_in): one box covers the two
-              // horizontally adjacent taps (r, 2s) and (r, 2s+1), which are contiguous channels of the parity view
-              const int c0 = xpair ? a_coff : (s & 1) * a_ld + a_coff + kcol;
-              const int c1 = xpair ? s : (s >> 1);
-              const int bcol = (HALO ? tap * 3 : (custom ? p.tap_wcol[tap] : tap)) * cin + kcol;
-              if (PAIR) {
-                // all bytes of both CTAs are credited to the LEADER's full barrier; the peer only contributes an arrival
-                const uint32_t bar_addr = mapa_u32(smem_u32(&full_bar[stage]), 0);
-                if (rank == 0)
-                  mbar_expect_tx(&full_bar[stage], 2 * stage_tx);
-                else
-                  mbar_arrive_cluster(bar_addr);
-                if (MODE == 0)
-                  tma_load_2d_pair(a_dst, &map_a, bar_addr, a_coff + kcol, row0 + shift);
-                else
-                  tma_load_5d_pair(a_dst, &map_a, bar_addr, c0, ow0 + c1, r & 1, oh0 + (r >> 1), img);
-                if (!bres) {
-#pragma unroll
-                  for (uint32_t t = 0; t < C::kTaps; ++t)
-                    tma_load_2d_pair(b_dst + t * C::kBBytes, &map_b, bar_addr, bcol + int(t) * cin, n0);
-                }
-              } else {
-                mbar_expect_tx(&full_bar[stage], stage_tx);
-                if (MODE == 0)
-                  tma_load_2d(a_dst, &map_a, &full_bar[stage], a_coff + kcol, row0 + shift);
-                else
-                  tma_load_5d(a_dst, &map_a, &full_bar[stage], c0, ow0 + c1, r & 1, oh0 + (r >> 1), img);
-                if (!bres) {
-#pragma unroll
-                  for (uint32_t t = 0; t < C::kTaps; ++t)
-                    tma_load_2d(b_dst + t * C::kBBytes, &map_b, &full_bar[stage], bcol + int(t) * cin, n0);
-                }
-              }
-            }
-            __syncwarp();
-            if (++stage == uint32_t(STAGES)) {
-              stage = 0;
-              phase ^= 1u;
-            }
-            if (++s == taps_w) {
-              s = 0;
-              ++r;
-            }
-            if (++tap == taps_it) {
-              tap = 0;
-              r = 0;
-              s = 0;
-              ++kb;
-            }
-          }
-        }
-      };
-      if (p.mode == 0)
-        run(std::integral_constant<int, 0>{});
-      else
-        run(std::integral_constant<int, 1>{});
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (leader CTA; whole warp, elected lane)
-    if (rank == 0) {
-      uint32_t stage = 0, phase = 0;
-      int iter = 0;
-      // shared-memory matrix descriptors: only the 14-bit start-address field (16-byte units) changes between MMAs
-      constexpr uint32_t kDescHi = ((C::kSbo >> 4) & 0x3FFFu) | (1u << 14) | (C::kLayout << 29);
-      const uint32_t a_base = (smem_u32(smem_a) >> 4) & 0x3FFFu, b_base = (smem_u32(smem_b) >> 4) & 0x3FFFu;
-      if (bres && worker < total_tiles) mbar_wait(bres_bar, 0, p.err, 6);  // resident weights have landed
-      for (int tile = worker; tile < total_tiles; tile += n_workers, ++iter) {
-        const uint32_t as = iter & 1, aphase = (iter >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1u, p.err, 2);  // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + as * BLOCK_N;
+    __syncwarp();
+    // loop-invariant parameters in registers, and one copy of the tile loop per addressing mode
+    const int n_tiles = p.n_tiles, wp = p.wp, cin = p.cin, a_coff = p.a_coff, a_ld = p.a_ld;
+    const int taps_it = HALO ? 3 : p.taps;  // HALO: tap = filter row r
+    const bool xpair = p.xpair != 0, nine = p.taps == 9, custom = p.custom_taps != 0;
+    const int taps_w = xpair ? 2 : 3;       // taps per filter row
+    const uint32_t stage_tx = p.a_tx_bytes + (bres ? 0u : kBStage);
+    auto run = [&](auto mode_tag) {
+      constexpr int MODE = decltype(mode_tag)::value;
+      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const int nt = tile % n_tiles;
+        const int mt = tile / n_tiles;
+        const int n0 = nt * BLOCK_N;
+        int row0 = 0, img = 0, oh0 = 0, ow0 = 0;
+        if (MODE == 0) {
+          row0 = mt * kBlockM;
+        } else {
+          const int per_img = p.tiles_w * p.tiles_h;
+          img = mt / per_img;
+          const int t = mt - img * per_img;
+          oh0 = (t / p.tiles_w) * p.th;
+          ow0 = (t % p.tiles_w) * p.tw;
+        }
+        // (k-block kb, tap) advance incrementally: a runtime division per stage was a quarter of the loop
+        int kb = 0, tap = 0, r = 0, s = 0;  // tap = r * taps_w + s  (1x1: always 0)
         for (int it = 0; it < k_iters; ++it) {
-          mbar_wait(&full_bar[stage], phase, p.err, 3);  // TMA bytes have landed
-          tc_fence_after();
-          const uint32_t a_lo = a_base + stage * (C::kABytes >> 4);
-          const uint32_t b_lo = b_base + (bres ? uint32_t(it) : stage) * (kBStage >> 4);
+          mbar_wait(&empty_bar[stage], phase ^ 1u, p.err, 1);
           if (elect_one()) {
+            uint8_t* a_dst = smem_a + stage * C::kABytes;
+            uint8_t* b_dst = smem_b + stage * kBStage;
+            const int kcol = kb * BLOCK_K;
+            // flat mode: the tap's A box is the tile's pixel rows shifted by (r-1)*wp + (s-1) (HALO: a whole filter row)
+            const int shift = HALO ? (tap - 1) * wp - 1 : (custom ? p.tap_shift[tap] : (nine ? (r - 1) * wp + (s - 1) : 0));
+            // patch mode: filter row r, column s.  x-paired weights (stride 2, in_ld == c_in): one box covers the two
+            // horizontally adjacent taps (r, 2s) and (r, 2s+1), which are contiguous channels of the parity view
+            const int c0 = xpair ? a_coff : (s & 1) * a_ld + a_coff + kcol;
+            const int c1 = xpair ? s : (s >> 1);
+            const int bcol = (HALO ? tap * 3 : (custom ? p.tap_wcol[tap] : tap)) * cin + kcol;
+            mbar_expect_tx(&full_bar[stage], stage_tx);
+            if (MODE == 0)
+              tma_load_2d(a_dst, &map_a, &full_bar[stage], a_coff + kcol, row0 + shift);
+            else
+              tma_load_5d(a_dst, &map_a, &full_bar[stage], c0, ow0 + c1, r & 1, oh0 + (r >> 1), img);
+            if (!bres) {
 #pragma unroll
-            for (uint32_t t = 0; t < C::kTaps; ++t) {
-#pragma unroll
-              for (int k = 0; k < BLOCK_K / 16; ++k) {
-                // HALO: tap t reads the A box shifted by t pixel rows: start address off the 1 KB swizzle pattern
-                // (legal with base_offset 0: the XOR pattern is taken from the absolute address)
-                const uint64_t adesc = (uint64_t(kDescHi) << 32) | (a_lo + ((t * (BLOCK_K * 2) + k * 32) >> 4));
-                const uint64_t bdesc = (uint64_t(kDescHi) << 32) | (b_lo + ((t * C::kBBytes + k * 32) >> 4));
-                const uint32_t acc = (t | uint32_t(k)) != 0 ? 1u : (it != 0 ? 1u : 0u);
-                if (PAIR)
-                  umma_bf16_ss_pair(d_tmem, adesc, bdesc, IDESC, acc);
-                else
-                  umma_bf16_ss(d_tmem, adesc, bdesc, IDESC, acc);
-              }
-            }
-            // the smem slot (in BOTH CTAs of a pair) is free once these MMAs have read it
-            if (PAIR) {
-              umma_commit_pair(&empty_bar[stage], 0x3);
-              if (it == k_iters - 1) umma_commit_pair(&tfull_bar[as], 0x3);
-            } else {
-              umma_commit(&empty_bar[stage]);
-              if (it == k_iters - 1) umma_commit(&tfull_bar[as]);
+              for (uint32_t t = 0; t < C::kTaps; ++t)
+                tma_load_2d(b_dst + t * C::kBBytes, &map_b, &full_bar[stage], bcol + int(t) * cin, n0);
             }
           }
           __syncwarp();
-          if (++stage == STAGES) {
+          if (++stage == uint32_t(STAGES)) {
             stage = 0;
             phase ^= 1u;
           }
+          if (++s == taps_w) {
+            s = 0;
+            ++r;
+          }
+          if (++tap == taps_it) {
+            tap = 0;
+            r = 0;
+            s = 0;
+            ++kb;
+          }
         }
       }
-    }
+    };
+    if (p.mode == 0)
+      run(std::integral_constant<int, 0>{});
+    else
+      run(std::integral_constant<int, 1>{});
   } else {
-    // ------------------------------------------------------------------ epilogue (warps 2..9 = 256 threads)
-    // Every warp runs on its own: it owns TMEM lane quarter `quarter` (32 tile rows) and column half `half`, keeps a
-    // private copy of its bias slice, and (STAGED) loads the residual of / stores exactly its 32 rows with its own TMA
-    // boxes and mbarriers.  No block-wide barrier is left in the tile loop, so a warp that is done starts on the next tile
-    // (other TMEM buffer) while slower ones finish.  The first version walked all 8 warps through every tile in lock-step
-    // (two 256-thread named barriers, one elected TMA thread) and the thin layers were bound by that serial chain:
-    // the MMA warp waited on tmem_empty for 430 k polls per launch (profiles/r01_ncu_issue_loop.txt).
-    const int groups = (static_cast<int>(blockDim.x) - 64) >> 8;  // 1, or 2 for thin tiles (launch_cfg)
-    const int ew = warp - 2;                  // epilogue warp index
-    const int group = ew >> 3;                // group g converts the tiles whose accumulator is TMEM buffer g
-    const int quarter = warp & 3;             // a warp may only touch TMEM lanes [32*(warp%4), +32)
-    const int half = (ew & 7) >> 2;           // which half of the tile's columns this warp converts
-    constexpr int kColsPerWarp = C::kColsPerWarp;
-    const int c_begin = BLOCK_N >= 64 ? half * kColsPerWarp : 0;
-    const bool active = BLOCK_N >= 64 || half == 0;
-    const int m = quarter * 32 + lane;
-    float* s_bias_w = s_bias + ew * kColsPerWarp;
-    const uint32_t lead_tempty[2] = {PAIR ? mapa_u32(smem_u32(&tempty_bar[0]), 0) : 0u,
-                                     PAIR ? mapa_u32(smem_u32(&tempty_bar[1]), 0) : 0u};
-    // STAGED: N = 64 has ONE 64-column slab, shared by the two warps of a lane quarter (pair barrier 1 + quarter, 64
-    // threads; the half-0 warp issues the TMA traffic); otherwise each warp owns whole slabs
-    constexpr bool kPairSync = STAGED && BLOCK_N == 64;
-    constexpr uint32_t kMySlabs = kPairSync ? 1u : (C::kColsPerWarp + C::kSlabCols - 1) / C::kSlabCols;
-    const uint32_t slab0 = kPairSync ? 0u : uint32_t(c_begin) / C::kSlabCols;
-    const bool issuer = STAGED && active && lane == 0 && (!kPairSync || half == 0);
-    uint64_t* my_res_bar = res_bar + (kPairSync ? group * 4 + quarter : ew) * 2;
-    const int pair_bar = 1 + quarter + 4 * group;  // named barrier of the two warps sharing a lane quarter (N = 64)
-    constexpr uint32_t kMyResBytes = kMySlabs * 32u * C::kSlabRowBytes;
-    int iter = 0;
-    int bias_nt = -1;  // N tile whose bias currently sits in s_bias_w
-    const bool silu = p.act == Y3_ACT_SILU;
-    const float bscale = silu ? 0.5f : 1.0f;
-    for (int tile = worker; tile < total_tiles; tile += n_workers, ++iter) {
-      if (groups == 2 && (iter & 1) != group) continue;
-      const uint32_t as = iter & 1, aphase = (iter >> 1) & 1;
-      const int li = groups == 2 ? iter >> 1 : iter;  // tiles this group has converted so far
-      const int nt = tile % p.n_tiles;
-      const int mt = PAIR ? (tile / p.n_tiles) * 2 + static_cast<int>(rank) : tile / p.n_tiles;
+    // ------------------------------------------------------------------ consumers: wgmma + epilogue (warpgroups 0, 1)
+    const int wg = warp >> 2;                             // tile rows [64 wg, 64 wg + 64)
+    const int m0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);  // this thread's accumulator rows: m0 and m0 + 8
+    const int cq = 2 * (lane & 3);                        // ... and columns 8 j + cq, 8 j + cq + 1
+    constexpr uint32_t kDescHi = wgmma_desc_hi(C::kSbo, C::kSwizzleBytes);
+    const uint32_t a_base = smem_u32(smem_a) + uint32_t(wg) * 64u * C::kSwizzleBytes;
+    const uint32_t b_base = smem_u32(smem_b);
+    uint32_t stage = 0, phase = 0;
+    if (bres && int(blockIdx.x) < total_tiles) mbar_wait(bres_bar, 0, p.err, 6);  // resident weights have landed
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      float acc[BLOCK_N / 2];
+      uint32_t prev = 0;
+      for (int it = 0; it < k_iters; ++it) {
+        mbar_wait(&full_bar[stage], phase, p.err, 3);  // TMA bytes have landed
+        const uint32_t a_st = a_base + stage * C::kABytes;
+        const uint32_t b_st = b_base + (bres ? uint32_t(it) : stage) * kBStage;
+        wgmma_fence();
+#pragma unroll
+        for (uint32_t t = 0; t < C::kTaps; ++t) {
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / 16; ++k) {
+            // HALO: tap t reads the A box shifted by t pixel rows (start address off the swizzle pattern)
+            const uint64_t adesc = wgmma_desc(kDescHi, a_st + t * C::kSwizzleBytes + k * 32);
+            const uint64_t bdesc = wgmma_desc(kDescHi, b_st + t * C::kBBytes + k * 32);
+            Wgmma<BLOCK_N>::template mma<0, 0>(acc, adesc, bdesc, (it != 0 || t != 0 || k != 0) ? 1u : 0u);
+          }
+        }
+        wgmma_commit();
+        // the previous stage's MMAs have completed: its slot may be refilled
+        wgmma_wait<1>();
+        if (it > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == uint32_t(STAGES)) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      // ---- epilogue straight from the accumulator registers
+      const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
       const int n0 = nt * BLOCK_N;
-
-      // ---- which output pixel does accumulator row m belong to?
-      bool valid;
-      int img, oy, ox;  // image, UNPADDED output coordinates
-      if (p.mode == 0) {
-        const int row = mt * kBlockM + m;
-        const int plane = p.hp * p.wp;
-        img = static_cast<int>(fast_div(static_cast<uint32_t>(row), p.plane_mul, p.plane_shr));
-        const int rem = row - img * plane;
-        const int yp = static_cast<int>(fast_div(static_cast<uint32_t>(rem), p.wp_mul, p.wp_shr)), xp = rem - yp * p.wp;
-        valid = row < p.rows_total && yp >= 1 && yp <= p.hp - 2 && xp >= 1 && xp <= p.wp - 2;
-        oy = yp - 1;
-        ox = xp - 1;
-      } else {
-        const int per_img = p.tiles_w * p.tiles_h;
-        img = mt / per_img;
-        const int t = mt - img * per_img;
-        const int ty = m / p.tw, tx = m - ty * p.tw;
-        oy = (t / p.tiles_w) * p.th + ty;
-        ox = (t % p.tiles_w) * p.tw + tx;
-        valid = ty < p.th && oy < p.ho && ox < p.wo;
-      }
-      valid = valid && active && mt < p.m_tiles;  // a pair's second CTA may own a tile past the end
-      if (nt != bias_nt) {  // a layer with a single N tile loads its bias once
-        if (active)
-          for (int c = lane; c < kColsPerWarp; c += 32) s_bias_w[c] = bscale * __ldg(p.bias + n0 + c_begin + c);
-        bias_nt = nt;
-        __syncwarp();
-      }
-      if constexpr (STAGED) {
-        // ---------------- staged epilogue (flat mode, bf16 output): TMEM -> registers -> swizzled smem tile -> TMA store
-        const int row0 = mt * kBlockM + quarter * 32;  // first tile row of this warp
-        constexpr bool kTwo = C::kStgBufs == 2;
-        const uint32_t sb = kTwo ? uint32_t(li & 1) : 0u;              // this group's staging buffer for this tile
-        const uint32_t rphase = kTwo ? uint32_t(li >> 1) & 1u : uint32_t(li) & 1u;
-        uint8_t* stg_g = smem_stg + uint32_t(group) * C::kStgBufs * C::kStgTile;  // this group's buffers
-        // this warp's 32 rows of its first slab, in buffer sb
-        const uint32_t reg_off = slab0 * C::kSlabBytes + uint32_t(quarter) * 32u * C::kSlabRowBytes;
-        uint8_t* reg = stg_g + sb * C::kStgTile + reg_off;
-        if (issuer) {
-          if (kTwo) {
-            // residual prefetch distance 1: tile i+1's residual goes into the OTHER buffer, which this thread's store of
-            // tile i-1 must have finished reading; without a residual only its store of tile i-2 (this buffer)
-            if (p.res) bulk_wait_read_all(); else bulk_wait_read_1();
-            if (p.res) {
-              if (li == 0) {
-                mbar_expect_tx(&my_res_bar[0], kMyResBytes);
+      const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
+      // read from the kernel parameters here rather than kept live through the main loop
+      const bool silu = p.act == Y3_ACT_SILU;
+      const float bscale = silu ? 0.5f : 1.0f;
+      const int reps = p.upsample ? 4 : 1;
+      // one row at a time: only that row's three output pointers are live beside the accumulators (N = 256 keeps 128)
 #pragma unroll
-                for (uint32_t sl = 0; sl < kMySlabs; ++sl)
-                  tma_load_2d(reg + sl * C::kSlabBytes, &map_res, &my_res_bar[0],
-                              p.res_coff + n0 + (slab0 + sl) * C::kSlabCols, row0);
-              }
-              const int tnext = tile + groups * n_workers;  // this group's next tile
-              if (tnext < total_tiles) {
-                const int nt2 = tnext % p.n_tiles;
-                const int mt2 = PAIR ? (tnext / p.n_tiles) * 2 + static_cast<int>(rank) : tnext / p.n_tiles;
-                uint8_t* reg2 = stg_g + (sb ^ 1u) * C::kStgTile + reg_off;
-                mbar_expect_tx(&my_res_bar[sb ^ 1u], kMyResBytes);
+      for (int h = 0; h < 2; ++h) {
+        const RowOut ro = row_out(p, mt, n0, m0 + 8 * h);
+        if (!ro.f32 && !ro.out) continue;
 #pragma unroll
-                for (uint32_t sl = 0; sl < kMySlabs; ++sl)
-                  tma_load_2d(reg2 + sl * C::kSlabBytes, &map_res, &my_res_bar[sb ^ 1u],
-                              p.res_coff + nt2 * BLOCK_N + (slab0 + sl) * C::kSlabCols, mt2 * kBlockM + quarter * 32);
-              }
-            }
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int c = 8 * j + cq;
+          if (!p.out_f32 && n0 + c >= p.cout) continue;  // c_out % 32 == 0: a column pair is either inside or outside
+          const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c));
+          float x0 = bias_act(acc[4 * j + 2 * h], bscale * b.x, silu);
+          float x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b.y, silu);
+          if (ro.f32) {
+            *reinterpret_cast<float2*>(ro.f32 + c) = make_float2(x0, x1);
           } else {
-            bulk_wait_read_all();  // the previous tile's store has finished reading this warp's staging rows
-            if (p.res) {
-              mbar_expect_tx(&my_res_bar[0], kMyResBytes);
-#pragma unroll
-              for (uint32_t sl = 0; sl < kMySlabs; ++sl)
-                tma_load_2d(reg + sl * C::kSlabBytes, &map_res, &my_res_bar[0], p.res_coff + n0 + (slab0 + sl) * C::kSlabCols,
-                            row0);
+            if (ro.res) {
+              const float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(ro.res + c));
+              x0 += f.x;
+              x1 += f.y;
             }
-          }
-        }
-        // the staging rows are free (the issuer has waited for the store that last read them)
-        if (kPairSync) named_bar_sync(pair_bar, 64); else __syncwarp();
-        mbar_wait(&tfull_bar[as], aphase, p.err, 4, p.poll_ns);
-        tc_fence_after();
-        if (p.res && active) mbar_wait(&my_res_bar[sb], rphase, p.err, 5);  // residual rows landed (idle warps own none)
-        const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * BLOCK_N;
-        const uint32_t swz = C::kSlabRowBytes == 128 ? (m & 7) : ((m >> 1) & 3);
-        if (active) {
-#pragma unroll 1
-          for (int c = c_begin; c < c_begin + kColsPerWarp; c += 32) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(t_addr + c, v);
-            tmem_ld_wait();
-            float x[32];
-            bias_act(v, s_bias_w + (c - c_begin), x, silu);
-            const uint32_t slab = c / C::kSlabCols, j0 = (c % C::kSlabCols) / 8;
-            const uint32_t row_addr = smem_u32(stg_g) + sb * C::kStgTile + slab * C::kSlabBytes + m * C::kSlabRowBytes;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const uint32_t addr = row_addr + (((j0 + q) ^ swz) << 4);
-              uint4 o = make_uint4(0u, 0u, 0u, 0u);  // halo / out-of-range rows store zeros (keeps the halo invariant)
-              if (valid) {
-                if (p.res) {
-                  const uint4 r = lds128(addr);
-                  const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const float2 f = unpack_bf16x2(rr[e]);
-                    x[q * 8 + e * 2 + 0] += f.x;
-                    x[q * 8 + e * 2 + 1] += f.y;
-                  }
-                }
-                o.x = pack_bf16x2(x[q * 8 + 0], x[q * 8 + 1]);
-                o.y = pack_bf16x2(x[q * 8 + 2], x[q * 8 + 3]);
-                o.z = pack_bf16x2(x[q * 8 + 4], x[q * 8 + 5]);
-                o.w = pack_bf16x2(x[q * 8 + 6], x[q * 8 + 7]);
-              }
-              sts128(addr, o);
-            }
-          }
-        }
-        fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the TMA (async proxy)
-        tc_fence_before();
-        if (PAIR)
-          mbar_arrive_cluster(lead_tempty[as]);
-        else
-          mbar_arrive(&tempty_bar[as]);
-        if (kPairSync) named_bar_sync(pair_bar, 64); else __syncwarp();
-        if (issuer) {
-#pragma unroll
-          for (uint32_t sl = 0; sl < kMySlabs; ++sl)
-            tma_store_2d(&map_out, reg + sl * C::kSlabBytes, p.out_coff + n0 + (slab0 + sl) * C::kSlabCols, row0);
-          bulk_commit_group();
-        }
-        continue;
-      }
-      const int oh = p.mode == 0 ? p.hp - 2 : p.ho;  // conv-output height/width (unpadded)
-      const int ow = p.mode == 0 ? p.wp - 2 : p.wo;
-      long long conv_row = (static_cast<long long>(img) * (oh + 2) + oy + 1) * (ow + 2) + ox + 1;
-      if (p.phase)  // one parity class of a transposed stride-2 conv: (oy, ox) -> (2 oy + a, 2 ox + b) of the 2x grid
-        conv_row = (static_cast<long long>(img) * (2 * oh + 2) + 2 * oy + p.ph_a + 1) * (2 * ow + 2) + 2 * ox + p.ph_b + 1;
-      const __nv_bfloat16* res_ptr = (p.res && valid) ? p.res + conv_row * p.res_ld + p.res_coff + n0 : nullptr;
-      __nv_bfloat16* out_ptr = nullptr;
-      float* f32_ptr = nullptr;
-      long long up_row_stride = 0;
-      if (p.out_f32) {
-        f32_ptr = p.out_f32 + ((static_cast<long long>(img) * oh + oy) * ow + ox) * p.out_f32_ld + n0;
-      } else if (p.upsample) {
-        const int w2 = 2 * ow + 2;
-        const long long r00 = (static_cast<long long>(img) * (2 * oh + 2) + 2 * oy + 1) * w2 + 2 * ox + 1;
-        out_ptr = p.out + r00 * p.out_ld + p.out_coff + n0;
-        up_row_stride = static_cast<long long>(w2) * p.out_ld;
-      } else {
-        out_ptr = p.out + conv_row * p.out_ld + p.out_coff + n0;
-      }
-      // residual of the first chunk is requested before waiting for the accumulator: its latency hides behind the MMAs
-      uint4 rcur[4];
-      if (res_ptr) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) rcur[q] = __ldg(reinterpret_cast<const uint4*>(res_ptr + c_begin) + q);
-      }
-
-      mbar_wait(&tfull_bar[as], aphase, p.err, 4, p.poll_ns);  // accumulator complete
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + as * BLOCK_N;
-      if (active) {
-#pragma unroll 1
-        for (int c = c_begin; c < c_begin + kColsPerWarp; c += 32) {
-          uint32_t v[32];
-          tmem_ld_32x32b_x32(t_addr + c, v);
-          uint4 rnext[4];
-          const bool more = c + 32 < c_begin + kColsPerWarp;
-          if (res_ptr && more) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) rnext[q] = __ldg(reinterpret_cast<const uint4*>(res_ptr + c + 32) + q);
-          }
-          tmem_ld_wait();
-          if (valid && (f32_ptr || n0 + c < p.cout)) {
-            float x[32];
-            bias_act(v, s_bias_w + (c - c_begin), x, silu);
-            if (f32_ptr) {
-              // fp32 pixel-major store (Detect heads): 128 contiguous bytes per thread and chunk
-#pragma unroll
-              for (int q = 0; q < 8; ++q)
-                reinterpret_cast<float4*>(f32_ptr + c)[q] = make_float4(x[q * 4], x[q * 4 + 1], x[q * 4 + 2], x[q * 4 + 3]);
-            } else {
-              if (res_ptr) {
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                  const uint32_t rr[4] = {rcur[q].x, rcur[q].y, rcur[q].z, rcur[q].w};
-#pragma unroll
-                  for (int e = 0; e < 4; ++e) {
-                    const float2 f = unpack_bf16x2(rr[e]);
-                    x[q * 8 + e * 2 + 0] += f.x;
-                    x[q * 8 + e * 2 + 1] += f.y;
-                  }
-                }
-              }
-              uint4 o[4];
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                o[q].x = pack_bf16x2(x[q * 8 + 0], x[q * 8 + 1]);
-                o[q].y = pack_bf16x2(x[q * 8 + 2], x[q * 8 + 3]);
-                o[q].z = pack_bf16x2(x[q * 8 + 4], x[q * 8 + 5]);
-                o[q].w = pack_bf16x2(x[q * 8 + 6], x[q * 8 + 7]);
-              }
-              const int reps = p.upsample ? 4 : 1;
-              for (int rep = 0; rep < reps; ++rep) {
-                uint4* dst = reinterpret_cast<uint4*>(out_ptr + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + c);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) dst[q] = o[q];
-              }
-            }
-          }
-          if (res_ptr && more) {
-#pragma unroll
-            for (int q = 0; q < 4; ++q) rcur[q] = rnext[q];
+            const uint32_t v = pack_bf16x2(x0, x1);
+            for (int rep = 0; rep < reps; ++rep)
+              *reinterpret_cast<uint32_t*>(ro.out + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + c) = v;
           }
         }
       }
-      tc_fence_before();
-      if (PAIR)
-        mbar_arrive_cluster(lead_tempty[as]);  // the leader's MMA thread waits for BOTH CTAs' epilogues
-      else
-        mbar_arrive(&tempty_bar[as]);
     }
-    if (issuer) bulk_wait_all();  // this thread's last TMA store has completed
-  }
-
-  __syncwarp();
-  tc_fence_before();
-  if (PAIR) cluster_sync_all(); else __syncthreads();  // pair: nobody leaves while the peer may still signal its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem_base, C::kTmemCols); else tmem_dealloc(tmem_base, C::kTmemCols);
   }
 }
 
-template <int BLOCK_N, int BLOCK_K, bool PAIR, bool STAGED, bool HALO = false>
+template <int BLOCK_N, int BLOCK_K, bool HALO = false>
 int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
-  using C = Cfg<BLOCK_N, BLOCK_K, PAIR, STAGED, HALO>;
-  auto kern = conv_tc_kernel<BLOCK_N, BLOCK_K, PAIR, STAGED, HALO>;
+  using C = Cfg<BLOCK_N, BLOCK_K, HALO>;
+  auto kern = conv_tc_kernel<BLOCK_N, BLOCK_K, HALO>;
   static bool attr_set = false;  // benign race: idempotent attribute
   if (!attr_set) {
     Y3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(C::kSmemBytes)));
     attr_set = true;
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(plan.grid);
-  const int groups = plan.groups == 2 && C::kMaxGroups == 2 ? 2 : 1;
-  cfg.blockDim = dim3(64 + 32 * kEpilogueWarps * groups);
-  cfg.dynamicSmemBytes = C::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int n_attr = 0;
-  if (PAIR) {
-    attr[n_attr].id = cudaLaunchAttributeClusterDimension;
-    attr[n_attr].val.clusterDim.x = 2;
-    attr[n_attr].val.clusterDim.y = 1;
-    attr[n_attr].val.clusterDim.z = 1;
-    ++n_attr;
-  }
-  if (pdl_enabled()) {  // the kernel parks at pdl_wait() after its prologue (y3_common.cuh)
-    attr[n_attr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n_attr].val.programmaticStreamSerializationAllowed = 1;
-    ++n_attr;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n_attr;
   ConvTcArgs args = plan.args;
   args.bres = plan.bres;
-  {
-    static int poll = -1;  // Y3_CONV_POLL_NS: nanosleep between polls of the epilogue's accumulator wait (default 0 = spin)
-    if (poll < 0) {
-      const char* e = getenv("Y3_CONV_POLL_NS");
-      poll = e ? atoi(e) : 0;
-      if (poll < 0) poll = 0;
-    }
-    args.poll_ns = static_cast<unsigned>(poll);
-  }
   args.stages = plan.bres ? C::bres_stages(args.taps * args.kblocks) : C::kStages;
   if (args.stages < 3) {  // not enough ring left beside the resident weights: fall back to streaming them
     args.bres = 0;
     args.stages = C::kStages;
   }
-  Y3_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, plan.map_a, plan.map_b, plan.map_out, plan.map_res, args));
+  // the kernel parks at pdl_wait() after its prologue (y3_common.cuh)
+  Y3_CHECK_CUDA(launch_pdl(kern, dim3(plan.grid), dim3(kThreads), C::kSmemBytes, stream, plan.map_a, plan.map_b, args));
   return Y3_OK;
 }
 
@@ -698,68 +357,35 @@ int pick_block_n(int cout) { return cout <= 32 ? 32 : (cout <= 64 ? 64 : (cout <
 }  // namespace
 
 int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream) {
-#define Y3_DISPATCH_K(BN, PR)                                                                                   \
-  switch (plan.block_k) {                                                                                       \
-    case 64: return plan.staged ? launch_cfg<BN, 64, PR, true>(plan, stream) : launch_cfg<BN, 64, PR, false>(plan, stream); \
-    case 32: return plan.staged ? launch_cfg<BN, 32, PR, true>(plan, stream) : launch_cfg<BN, 32, PR, false>(plan, stream); \
-    case 16: return plan.staged ? launch_cfg<BN, 16, PR, true>(plan, stream) : launch_cfg<BN, 16, PR, false>(plan, stream); \
-  }                                                                                                             \
+#define Y3_DISPATCH_K(BN)                                              \
+  switch (plan.block_k) {                                              \
+    case 64: return launch_cfg<BN, 64>(plan, stream);                  \
+    case 32: return launch_cfg<BN, 32>(plan, stream);                  \
+    case 16: return launch_cfg<BN, 16>(plan, stream);                  \
+  }                                                                    \
   break;
-  if (plan.halo && plan.block_k == 32) {  // c_in = 32 layers (64-byte rows, SWIZZLE_64B)
-    if (plan.block_n == 64)
-      return plan.staged ? launch_cfg<64, 32, false, true, true>(plan, stream) : launch_cfg<64, 32, false, false, true>(plan, stream);
-    if (plan.block_n == 32)
-      return plan.staged ? launch_cfg<32, 32, false, true, true>(plan, stream) : launch_cfg<32, 32, false, false, true>(plan, stream);
-    return set_error(Y3_ERR_BAD_ARG, "conv_tc: no K=32 halo kernel for tile N=%d", plan.block_n);
+  if (plan.halo) {  // stride-1 3x3: K = 64 with N <= 128, K = 32 (c_in = 32 layers, 64-byte rows) with N <= 64
+    if (plan.block_k == 64) {
+      if (plan.block_n == 128) return launch_cfg<128, 64, true>(plan, stream);
+      if (plan.block_n == 64) return launch_cfg<64, 64, true>(plan, stream);
+      if (plan.block_n == 32) return launch_cfg<32, 64, true>(plan, stream);
+    } else if (plan.block_k == 32) {
+      if (plan.block_n == 64) return launch_cfg<64, 32, true>(plan, stream);
+      if (plan.block_n == 32) return launch_cfg<32, 32, true>(plan, stream);
+    }
+    return set_error(Y3_ERR_BAD_ARG, "conv_tc: no halo kernel for tile N=%d K=%d", plan.block_n, plan.block_k);
   }
-  if (plan.halo) {  // block_k == 64, stride-1 3x3; N = 256 only as a CTA pair and never staged (smem)
-    if (plan.pair) {
-      if (plan.block_n == 256) return launch_cfg<256, 64, true, false, true>(plan, stream);
-      if (plan.block_n == 128)
-        return plan.staged ? launch_cfg<128, 64, true, true, true>(plan, stream) : launch_cfg<128, 64, true, false, true>(plan, stream);
-    } else {
-      if (plan.block_n == 128)
-        return plan.staged ? launch_cfg<128, 64, false, true, true>(plan, stream) : launch_cfg<128, 64, false, false, true>(plan, stream);
-      if (plan.block_n == 64)
-        return plan.staged ? launch_cfg<64, 64, false, true, true>(plan, stream) : launch_cfg<64, 64, false, false, true>(plan, stream);
-      if (plan.block_n == 32)
-        return plan.staged ? launch_cfg<32, 64, false, true, true>(plan, stream) : launch_cfg<32, 64, false, false, true>(plan, stream);
-    }
-    return set_error(Y3_ERR_BAD_ARG, "conv_tc: no halo kernel for tile N=%d pair=%d", plan.block_n, plan.pair);
-  }
-  if (plan.pair) {
-    switch (plan.block_n) {
-      case 128: Y3_DISPATCH_K(128, true)
-      case 256: Y3_DISPATCH_K(256, true)
-    }
-  } else {
-    switch (plan.block_n) {
-      case 32: Y3_DISPATCH_K(32, false)
-      case 64: Y3_DISPATCH_K(64, false)
-      case 128: Y3_DISPATCH_K(128, false)
-      case 256: Y3_DISPATCH_K(256, false)
-    }
+  switch (plan.block_n) {
+    case 32: Y3_DISPATCH_K(32)
+    case 64: Y3_DISPATCH_K(64)
+    case 128: Y3_DISPATCH_K(128)
+    case 256: Y3_DISPATCH_K(256)
   }
 #undef Y3_DISPATCH_K
-  return set_error(Y3_ERR_BAD_ARG, "conv_tc: no kernel for tile N=%d K=%d pair=%d", plan.block_n, plan.block_k, plan.pair);
+  return set_error(Y3_ERR_BAD_ARG, "conv_tc: no kernel for tile N=%d K=%d", plan.block_n, plan.block_k);
 }
 
-// Y3_CONV_PAIR=0 forces the 1-CTA kernel everywhere (A/B measurements); default: CTA pairs for tile N >= 128.
-// Y3_CONV_STAGED=0 forces the direct-store epilogue everywhere (A/B measurements).
-static bool staged_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("Y3_CONV_STAGED");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
-
-// Y3_CONV_HALO=0 disables the halo-reuse A path.  Descriptors of the row-shifted taps carry base_offset = 0: measured on
-// B200 (tools/probe_conv.py, profiles/r01_probe_conv_halo_baseoffset0.jsonl) all conv cases are exact that way, i.e. the
-// tensor core applies the 128B-swizzle XOR to the ABSOLUTE shared-memory address bits [7,10) exactly as the TMA unit did
-// when it wrote the box; with base_offset = (addr >> 7) & 7 — the other reading of the ISA text — the shifted taps read
-// wrong rows (that probe variant has been removed again).
+// Y3_CONV_HALO=0 disables the halo-reuse A path (A/B measurements).
 static bool halo_enabled() {
   static int v = -1;
   if (v < 0) {
@@ -774,25 +400,6 @@ static bool bres_enabled() {
   static int v = -1;
   if (v < 0) {
     const char* e = getenv("Y3_CONV_BRES");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
-
-// Y3_CONV_GROUPS=1 keeps a single epilogue group for the thin tiles (A/B measurements).
-static bool groups_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("Y3_CONV_GROUPS");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v != 0;
-}
-
-static bool pair_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("Y3_CONV_PAIR");
     v = (e && e[0] == '0') ? 0 : 1;
   }
   return v != 0;
@@ -897,9 +504,8 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     Y3_REQUIRE(rows < (1ll << 31) - 4096, "conv: too many pixels");
     a.rows_total = static_cast<int>(rows);
     a.m_tiles = static_cast<int>((rows + kBlockM - 1) / kBlockM);
-    // halo reuse needs >= 2 stages of (17 KB + 3 B tiles): any N <= 128, N = 256 only as a CTA pair
-    const bool pair_ok = bn >= 128 && pair_enabled() && a.m_tiles >= 2;
-    plan->halo = (!extra && taps == 9 && (bk == 64 || (bk == 32 && bn <= 64)) && halo_enabled() && (bn <= 128 || pair_ok)) ? 1 : 0;
+    // halo reuse needs >= 2 stages of (17 KB + 3 B tiles): N <= 128 (N = 256 would leave room for one stage)
+    plan->halo = (!extra && taps == 9 && ((bk == 64 && bn <= 128) || (bk == 32 && bn <= 64)) && halo_enabled()) ? 1 : 0;
     if (extra) {
       a.custom_taps = 1;
       for (int t = 0; t < extra->ntaps; ++t) {
@@ -955,47 +561,19 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     const uint64_t ktot = static_cast<uint64_t>(extra ? d.ksize * d.ksize : taps) * gemm_cin;  // the whole weight matrix
     const uint64_t dims[2] = {ktot, static_cast<uint64_t>(cout_pad)};
     const uint64_t strides[2] = {0, ktot * 2};
-    plan->pair = (bn >= 128 && pair_enabled() && a.m_tiles >= 2) ? 1 : 0;
-    const uint32_t box[2] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(plan->pair ? bn / 2 : bn)};
+    const uint32_t box[2] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(bn)};
     rc = select_only ? Y3_OK : encode_tensor_map_bf16(&plan->map_b, d.weight, 2, dims, strides, box, bk * 2);
     if (rc) return rc;
   }
   {
     // resident weights: one N tile whose (taps x k-blocks) boxes fit beside a useful A ring.  The TMA unit's row rate
     // (not bytes) bounds the thin layers, and re-fetching the same <= 96 KB of weights for every M tile was most of it.
-    const long long b_bytes = static_cast<long long>(taps) * a.kblocks * (plan->pair ? bn / 2 : bn) * bk * 2;
+    const long long b_bytes = static_cast<long long>(taps) * a.kblocks * bn * bk * 2;
     plan->bres = (a.n_tiles == 1 && b_bytes <= 96 * 1024 && bres_enabled()) ? 1 : 0;
   }
-  // staged (TMA-store) epilogue: flat mode, bf16 output, no upsample
-  plan->staged = (a.mode == 0 && !head && !d.upsample && !(extra && extra->phase) && staged_enabled() && !(plan->halo && bn == 256)) ? 1 : 0;
-  plan->map_out = plan->map_a;
-  plan->map_res = plan->map_a;
-  if (plan->staged) {
-    const uint32_t slab_cols = bn >= 64 ? 64 : 32;
-    // dim0 ends at the last channel this conv owns, so a partial last N tile is clipped by the TMA unit
-    const uint64_t dims[2] = {static_cast<uint64_t>(d.out_coff + d.c_out), static_cast<uint64_t>(a.rows_total)};
-    const uint64_t strides[2] = {0, static_cast<uint64_t>(d.out_ld) * 2};
-    const uint32_t box[2] = {slab_cols, 32};  // one epilogue warp's rows
-    rc = select_only ? Y3_OK : encode_tensor_map_bf16(&plan->map_out, d.out, 2, dims, strides, box, slab_cols * 2);
-    if (rc) return rc;
-    if (d.res) {
-      const uint64_t rdims[2] = {static_cast<uint64_t>(d.res_ld), static_cast<uint64_t>(a.rows_total)};
-      const uint64_t rstrides[2] = {0, static_cast<uint64_t>(d.res_ld) * 2};
-      rc = select_only ? Y3_OK : encode_tensor_map_bf16(&plan->map_res, d.res, 2, rdims, rstrides, box, slab_cols * 2);
-      if (rc) return rc;
-    }
-  }
   const int sms = num_sms();
-  if (plan->pair) {
-    const long long total = static_cast<long long>((a.m_tiles + 1) / 2) * a.n_tiles;  // 256-row pair tiles
-    const long long clusters = total < sms / 2 ? total : sms / 2;
-    plan->grid = static_cast<int>(clusters * 2);
-  } else {
-    const long long total = static_cast<long long>(a.m_tiles) * a.n_tiles;
-    plan->grid = static_cast<int>(total < sms ? total : sms);
-  }
-  plan->groups = (bn <= 128 && groups_enabled()) ? 2 : 1;
-  plan->smem_bytes = 0;
+  const long long total = static_cast<long long>(a.m_tiles) * a.n_tiles;
+  plan->grid = static_cast<int>(total < sms ? total : sms);
   return Y3_OK;
 }
 
@@ -1008,11 +586,8 @@ extern "C" int y3_conv_plan(const y3_conv_desc* d, y3_conv_plan_info* out) {
   if (rc) return rc;
   out->block_n = plan.block_n;
   out->block_k = plan.block_k;
-  out->pair = plan.pair;
-  out->staged = plan.staged;
   out->halo = plan.halo;
   out->resident_weights = plan.bres;
-  out->epilogue_groups = plan.groups;
   out->xpair = plan.args.xpair;
   out->m_tiles = plan.args.m_tiles;
   out->n_tiles = plan.args.n_tiles;

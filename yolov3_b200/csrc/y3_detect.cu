@@ -79,8 +79,7 @@ __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.0f,
 // cells, so the source of group-local element e = q*no + k is base + q*head_ld + k and its destination is z_base + e:
 // both offsets are per-lane constants computed once before the loop; per element the kernel then does one load, one
 // sigmoid, one store, and only the 4 box fields of each row take the grid/anchor branch.  The first version recomputed the
-// (q, k) split and moved seven shuffle words per element: 96 warp instructions per 32 outputs, issue-bound at 1.9 TB/s
-// (profiles/r01_ncu_decode_summary.txt).
+// (q, k) split and moved seven shuffle words per element: 96 warp instructions per 32 outputs, issue-bound.
 template <int NITER>
 __global__ void __launch_bounds__(256, NITER <= 3 ? 3 : 1) head_decode_kernel(const HeadDecodeArgs p) {
   pdl_entry();

@@ -38,14 +38,13 @@ void pdl_set(int on);
 #define Y3_BN_ASYNC_DEFAULT 1
 #endif
 
-// ---- tcgen05 conv: kernel arguments (device view) and a prepared launch
+// ---- tensor-core conv: kernel arguments (device view) and a prepared launch
 struct ConvTcArgs {
   int mode;  // 0: "flat" stride-1 (1x1 / 3x3) on the padded pixel list; 1: "patch" stride-2 3x3
   int taps, kblocks, cin;
   int a_coff, a_ld;
   uint32_t a_tx_bytes;   // bytes one A box delivers
   int xpair;             // patch mode with x-paired weights: 6 taps of 2*c_in channels
-  unsigned poll_ns;      // back-off between mbarrier polls of the epilogue warps (0 = spin)
   int stages;            // depth of the shared-memory ring (set by the launcher from the tile configuration)
   int bres;              // 1: the whole weight tile stays resident in shared memory (loaded once per CTA)
   int m_tiles, n_tiles;
@@ -80,16 +79,12 @@ struct ConvTcExtra {  // host side of the above (conv_tc_prepare)
 };
 
 struct ConvTcPlan {
-  CUtensorMap map_a, map_b, map_out, map_res;
-  int staged;  // 1: epilogue stages the tile in shared memory and stores it with TMA
+  CUtensorMap map_a, map_b;
   int halo;    // 1: stride-1 3x3 with one A box per filter row (halo reuse)
   int bres;    // 1: weights resident in shared memory (single N tile, small K)
-  int groups;  // epilogue groups of 8 warps (2 for tile N <= 64)
   ConvTcArgs args;
   int block_n, block_k;
-  int pair;  // 1: CTA-pair (cta_group::2) kernel, launched as clusters of 2
   int grid;
-  size_t smem_bytes;
 };
 int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only = false, const ConvTcExtra* extra = nullptr);
 int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream);

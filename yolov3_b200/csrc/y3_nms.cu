@@ -68,7 +68,7 @@ __device__ __forceinline__ int next_pow2(int v) { return v <= 1 ? 1 : 1 << (32 -
 // One warp per 32 consecutive prediction rows: the lanes test obj of 32 rows with one strided load, then the warp visits
 // only the rows that passed (85 contiguous floats each), and one atomic per warp reserves the key slots.  The first
 // version spent a warp, two block barriers and a share of a block atomic on EVERY row and was bound by those serial
-// latencies (64 rows in flight per SM): 282 us for 806 k rows at conf 0.25 (profiles/r01_nms_launches_*.txt).
+// latencies (64 rows in flight per SM).
 constexpr int kCandWarps = 8;
 
 __global__ void __launch_bounds__(32 * kCandWarps) nms_candidates_kernel(const NmsArgs p) {
@@ -111,8 +111,7 @@ __global__ void __launch_bounds__(32 * kCandWarps) nms_candidates_kernel(const N
     }
   } else {
     // single label: FOUR passing rows per iteration — their class loads are issued back to back before any of the shuffle
-    // reductions starts.  One row at a time left a warp with a single 340-byte row in flight and the kernel latency-bound
-    // (122 us for 274 MB at conf 0.001, gpurun r2j3).
+    // reductions starts.  One row at a time left a warp with a single 340-byte row in flight and the kernel latency-bound.
     constexpr int kRows = 4;
     for (unsigned rem = todo; rem;) {
       int rr[kRows];
@@ -405,8 +404,7 @@ __device__ __forceinline__ bool box_suppresses(const float4& bi, float ai, const
 
 // One WARP per (image, class) segment of up to 512 members: boxes live in registers (member j -> lane j % 32, slot j / 32),
 // the box of the current keeper is broadcast by shuffle, no block barrier in the greedy loop.  The block-per-segment
-// kernel below spent 8 warps and a __syncthreads per keeper and was issue-bound (5 blocks per SM in lock-step):
-// 138 us / 1.07 ms for 65 / 375 members per class (profiles/r01_nms_launches_summary.txt).
+// kernel below spent 8 warps and a __syncthreads per keeper and was issue-bound (5 blocks per SM in lock-step).
 constexpr int kWarpSlots = 16;
 constexpr int kWarpSegMax = 32 * kWarpSlots;
 
@@ -596,7 +594,7 @@ __global__ void __launch_bounds__(1024) nms_compact_kernel(const NmsArgs p) {
 
 // ================================================================================================ v2 pipeline
 // The first version sorted every candidate twice with global bitonic networks (conf, then (class, rank)): ~25 launches, the
-// two sorts 60 % of the 0.37 ms at conf 0.25 (profiles/r01_nms_launches_summary.txt).  Nothing needs a GLOBAL order except
+// two sorts most of the time.  Nothing needs a GLOBAL order except
 // the <= max_det rows that are returned, so v2 is:
 //   K1 candidates (unchanged)           keys (conf bits | ~id), unordered, per image
 //   K2 nms_bucket_kernel   1 CTA/image  max_nms cut (exact radix select, only when count > max_nms), xywh -> xyxy, counting
@@ -808,8 +806,8 @@ constexpr int kMaskLarge = 512;  // ... up to this size: nms_seg_mask_kernel<512
 // (2) boxes to shared memory in confidence order, (3) ALL pair tests in parallel — thread (i, w) builds the 32-bit word "which of
 // members 32w..32w+31 does member i suppress" with no dependency between pairs — (4) one warp resolves the greedy order with
 // bit operations only: walk i upward, skip removed members, OR row i into the removed set.  The per-keeper formulations (a warp
-// with boxes in registers, or a block with a barrier per keeper) serialise m dependent rounds: 228 us + 107 us for ~215 members
-// per class and 782 us for ~375 (multi-label) against ~65 us of pair-test work (gpurun r2j5).
+// with boxes in registers, or a block with a barrier per keeper) serialise m dependent rounds, several times
+// the pair-test work at a few hundred members per class.
 template <int MAXM, int THREADS>
 __global__ void __launch_bounds__(THREADS) nms_seg_mask_kernel(const NmsArgs p, int m_lo) {
   pdl_entry();
@@ -1120,7 +1118,7 @@ __global__ void __launch_bounds__(1024) nms_output_kernel(const NmsArgs p) {
     const bool select_first = S > kOutSortMax || (S > 1024 && S >= 2 * D);
     if (select_first) {
       // only the top D rows are returned: an exact radix select (8 passes over S keys) followed by a sort of D keys beats
-      // sorting everything — a 8192-key shared-memory bitonic network alone took 98 us for 4.4 k survivors (gpurun r2j5)
+      // sorting everything with an 8192-key shared-memory bitonic network
       thr = block_select_kth(sk, S, D, s_sel, &s_prefix, &s_k_);  // exactly D survivors have key >= thr
       cnt = D;
     }
@@ -1303,10 +1301,8 @@ extern "C" int y3_nms_batched(const float* pred, const y3_nms_params* q, void* w
   }
   if (!v1) {
     Y3_CHECK_CUDA(::y3::launch_pdl(nms_bucket_kernel, dim3(a.bs), dim3(kBucketThreads), 0, stream, a));
-    // measured (gpurun r2j5 / r2j6, 32 x 25200 rows) with the first matrix kernel (one thread per mask word, full test on all 32
-    // pairs): <= 128 members per class (conf 0.25: ~65) 37 us vs 50 us for a warp-per-segment kernel with the boxes in registers;
-    // ~215 per class (conf 0.001) 448 us (768-wide) vs 228 us; ~375 (multi-label) 1178 us vs 782 us for the per-keeper block
-    // kernel.  The two-phase pair test (ballot of intersections, exact test on those) is what made the matrix form win there too.
+    // the first matrix kernel (one thread per mask word, full test on all 32 pairs) beat a warp-per-segment kernel only at
+    // <= 128 members per class and lost at a few hundred.  The two-phase pair test (ballot of intersections, exact test on those) is what made the matrix form win there too.
     if (int rc = launch_seg_mask<kMaskSmall, 128>(a, 0, stream)) return rc;
     if (int rc = launch_seg_mask<kMaskLarge, 256>(a, kMaskSmall, stream)) return rc;
     Y3_CHECK_CUDA(::y3::launch_pdl(nms_seg_block_kernel, dim3(a.nc, a.bs), dim3(256), 0, stream, a));

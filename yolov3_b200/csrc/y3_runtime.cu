@@ -45,7 +45,7 @@ int num_sms() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-      sms = 148;
+      sms = 132;
   }
   return sms;
 }
@@ -108,10 +108,12 @@ extern "C" int y3_last_error(char* buf, size_t n) {
 }
 
 extern "C" int y3_device_check(void) {
-  int dev = 0, major = 0;
+  int dev = 0, major = 0, minor = 0;
   Y3_CHECK_CUDA(cudaGetDevice(&dev));
   Y3_CHECK_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 10) return y3::set_error(Y3_ERR_UNSUPPORTED, "device compute capability %d.x is not sm_100", major);
+  Y3_CHECK_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
+  if (major != 9 || minor != 0)
+    return y3::set_error(Y3_ERR_UNSUPPORTED, "device compute capability %d.%d is not sm_90", major, minor);
   return Y3_OK;
 }
 

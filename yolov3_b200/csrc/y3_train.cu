@@ -35,14 +35,13 @@ struct SliceW {
 // Every elementwise / reduction kernel below walks INTERIOR image rows: row r of n*h -> (image, y) with one 32-bit division
 // per row, then 16-byte items e = x*c8 + cg inside the row (c8 = channels/8 is a power of two for every BatchNorm of the
 // YOLOv3 graphs, so x = e >> log2(c8)).  The first version derived (n, y, x) from a 64-bit flat index with two 64-bit
-// divisions per 16 bytes and ran 4-8x above its HBM floor (profiles/r01_train_launches_summary.txt).
+// divisions per 16 bytes and ran several times above its HBM floor.
 struct Rows {
   int n, h, w, c8, c8_shift;  // c8_shift = log2(c8), or -1 when c8 is not a power of two (generic division)
   int upr;                    // work units per image row: a unit = kUnitIters x 256 consecutive 16-byte items of one row
 };
 // Every thread of a unit issues all of its (kUnitIters x loads-per-item) 16-byte loads before it consumes any: with one whole
-// row per block (10 dependent iterations per thread) the small layers ran at a fifth of HBM speed on latency alone
-// (gpurun r2j2 launch list: 21 us for 26 MB).
+// row per block (10 dependent iterations per thread) the small layers ran far below HBM speed on latency alone.
 constexpr int kUnitIters = 2;
 __device__ __forceinline__ void split_item(const Rows& g, int e, int& x, int& cg) {
   if (g.c8_shift >= 0) {
@@ -122,12 +121,11 @@ __global__ void __launch_bounds__(256, 4) bn_stats_kernel(Slice y, Rows g, float
 
 // Second stage of every two-stage reduction here: column sums of the nblk partial rows in a FIXED order (bit-reproducible).
 // Block = 32 columns x 32 row lanes: lane ty adds rows ty, ty+32, ... (coalesced 128-byte reads across tx), then the 32 lane
-// sums are added in index order.  The first version gave each column to one thread that walked all ~300 rows serially:
-// 37 us per BatchNorm layer, 2.7 ms of a 17 ms step (gpurun r2j2 launch list).
+// sums are added in index order.  The first version gave each column to one thread that walked all ~300 rows serially.
 __device__ __forceinline__ float colsum_32x32(const float* __restrict__ partial, int nblk, long long pitch, int col, bool valid,
                                               float (*sh)[33]) {
   // all of this lane's rows are requested before the first add (kMaxPartialBlocks / 32 <= 14 independent loads in flight): as a
-  // load-add loop the 14 L2 round trips serialised and every BatchNorm finalize cost ~4 us per column sum (gpurun r2j4)
+  // load-add loop the 14 L2 round trips serialised
   constexpr int kMaxRowsPerLane = 14;
   float v[kMaxRowsPerLane];
 #pragma unroll
@@ -380,16 +378,14 @@ __global__ void __launch_bounds__(256, UPS ? 2 : 3) bn_act_bwd_kernel(const BnBw
 
 // ---------------------------------------------------------------------------------------------- cp.async ring variant
 // bn_act_bwd_kernel keeps a unit's 16-byte vectors in registers between issue and use: 4 loads per thread in flight, three
-// blocks per SM, a bubble at every unit boundary, long-scoreboard stalls on top (profiles/r02_ncu_bn_bwd_summary.txt); a
-// register look-ahead halved the resident blocks and gained nothing (profiles/r02_experiments.md).  The variant below stages
+// blocks per SM, a bubble at every unit boundary, long-scoreboard stalls on top; a
+// register look-ahead halved the resident blocks and gained nothing.  The variant below stages
 // the SAME units through a per-thread shared-memory ring with cp.async: a thread copies its own 16-byte items kRingDepth-1
 // units ahead into its own slots and reads them back itself, so there is no barrier and no mbarrier anywhere
 // (cp.async.wait_group cannot dead-lock) and 144 KB per SM are in flight without costing registers.  Unit order, item order
-// and operations are exactly those of bn_act_bwd_kernel: results are bit-identical.  Measured on the B200
-// (tests/diag/ab_shot.py, profiles/r02_ab_shot_kernel_variants.jsonl): reduce + apply passes 3-8 % faster on every layer
-// shape of the 640x640 step (e.g. 45.5 -> 43.4 us at 8x80x80x256, 136.0 -> 126.9 us at 8x320x320x64).  The same ring under
-// bn_stats gained +-5 % and under bn_act_fwd LOST 10-30 % (three 64 KB blocks per SM instead of five or six register-only
-// ones): those two were removed again — the passes are bound by resident warps x issue, not by bytes in flight.
+// and operations are exactly those of bn_act_bwd_kernel: results are bit-identical (A/B script: tests/diag/ab_shot.py).
+// The same ring under bn_stats gained nothing and under bn_act_fwd lost (three 64 KB blocks per SM instead of five or six
+// register-only ones): those two were removed again — the passes are bound by resident warps x issue, not by bytes in flight.
 // Switch: y3_set_bn_async / Y3_BN_ASYNC (default on).
 __device__ __forceinline__ void cp_async16(uint32_t saddr, const void* gptr) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(gptr) : "memory");
@@ -772,7 +768,7 @@ __global__ void __launch_bounds__(256) im2col_first_kernel(const TIN* __restrict
 // strides of the [co,ci,k,k] parameter) — which IS the forward pack's order.  Per optimizer step the whole buffer is
 // converted to bf16 by one elementwise kernel (the forward packs are views of that copy) and ONE launch of the kernel
 // below transposes every layer into its dgrad pack [ci_pad][(k-1-kh)*k + (k-1-kw)][co].  71 per-layer launches with
-// scattered 2-byte stores (0.96 ms / step, profiles/r01_train_launches_summary.txt) become two bandwidth-bound ones.
+// scattered 2-byte stores become two bandwidth-bound ones.
 __global__ void __launch_bounds__(256) f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ dst, long long n8) {
   pdl_entry();
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n8;
@@ -897,8 +893,8 @@ cudaError_t allow_smem(int bytes) {
   done = e == cudaSuccess;
   return e;
 }
-constexpr int kMaxPartialBlocks = 444;  // = 3 resident 256-thread blocks per SM x 148 SMs: exactly one wave of the reduction kernels
-                                        // (592 ran 1.33 waves: the tail block set doubled the small layers' time); fixed: sizes stay device-independent
+constexpr int kMaxPartialBlocks = 396;  // = 3 resident 256-thread blocks per SM x 132 SMs (H100): exactly one wave of the reduction
+                                        // kernels (a partial second wave doubles the small layers' time); fixed: sizes stay device-independent
 
 __global__ void __launch_bounds__(1024) bn_bwd_finalize_kernel(const float* __restrict__ partial, int nblk, int c,
                                                                float* __restrict__ sums, float* __restrict__ dbeta_acc,
@@ -1079,7 +1075,7 @@ extern "C" int y3_conv_wgrad(const y3_wgrad_desc* d, y3_stream_t stream) {
   Y3_REQUIRE(d->dy_ld % 8 == 0 && d->dy_coff % 8 == 0 && d->x_ld % 8 == 0 && d->x_coff % 8 == 0, "wgrad: bad slices");
   Y3_REQUIRE(d->stride == 0 || d->stride == 1 || (d->stride == 2 && y3::wgrad_tc_enabled() && d->ci % 32 == 0),
              "wgrad: stride must be 1, or 2 with the tensor-core kernel (c_in % 32 == 0)");
-  // tcgen05 kernel (csrc/y3_wgrad_tc.cu) whenever its tiling fits; the warp-level MMA kernel below otherwise
+  // wgmma kernel (csrc/y3_wgrad_tc.cu) whenever its tiling fits; the warp-level MMA kernel below otherwise
   if (y3::wgrad_tc_enabled() && d->ci % 32 == 0 && (reinterpret_cast<uintptr_t>(d->dy) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(d->x) & 15) == 0)
     return y3::wgrad_tc(*d, static_cast<cudaStream_t>(stream));

@@ -1,14 +1,14 @@
-// yolov3_b200 — weight gradient of a conv on the 5th-gen tensor cores.
+// yolov3_b200 — weight gradient of a conv on the Hopper tensor cores (wgmma).
 //   dW[co, ci, tap] += sum over padded pixels p of dy[p, co] * x[p + shift(tap), ci]
 // is a GEMM whose K dimension is the PIXEL index: both operands sit in memory pixel-major with channels contiguous, i.e.
-// "MN-major" in tcgen05 terms (a_major = b_major = 1 in the instruction descriptor; shared-memory descriptors of the
-// canonical MN-major SWIZZLE_128B layout: 64 channels (128 B) contiguous, 8 pixel rows per swizzle atom, SBO = 1024 B
-// between 8-row groups, LBO = bytes between 64-channel blocks).  The same TMA boxes as the forward conv ([64 pixels x 64
-// channels], the x box shifted by the tap) land in exactly that layout — no transposition anywhere.
-// One CTA = one (128-co block, N-ci block, tap) output tile over a range of pixels (split-K), accumulator in TMEM, fp32
-// atomics into PyTorch-layout dW.  Replaces the mma.sync kernel of y3_train.cu (41 % of a training step,
-// profiles/r01_train_launches_summary.txt) behind the same y3_conv_wgrad entry point (reference: autograd of
-// Conv.forward, models/common.py:71-75).
+// "MN-major" (transposed) wgmma operands: shared-memory descriptors of the canonical MN-major swizzled layout — 64
+// channels (128 B) contiguous, 8 pixel rows per swizzle atom, SBO = bytes between 8-row groups, LBO = bytes between
+// 64-channel blocks.  The same TMA boxes as the forward conv ([64 pixels x 64 channels], the x box shifted by the tap)
+// land in exactly that layout — no transposition anywhere.
+// One CTA = one (128-co block, N-ci block, tap) output tile over a range of pixels (split-K): warp 8 streams the boxes,
+// warpgroups 0 and 1 accumulate co rows [0, 64) and [64, 128) in registers and finish with fp32 atomics into
+// PyTorch-layout dW.  Replaces the mma.sync kernel of y3_train.cu behind the same y3_conv_wgrad entry point
+// (reference: autograd of Conv.forward, models/common.py:71-75).
 #include <cuda_bf16.h>
 
 #include <cstdlib>
@@ -19,9 +19,10 @@
 namespace y3 {
 namespace {
 
-constexpr int kWgM = 128;     // co per tile (TMEM lanes)
+constexpr int kWgM = 128;     // co per tile
 constexpr int kWgK = 64;      // pixels per pipeline stage (flat mode); the stride-2 patch mode uses 80 = tw x th
-constexpr int kWgThreads = 192;  // warp 0 producer, warp 1 MMA issuer + TMEM owner, warps 2-5 epilogue
+constexpr int kWgThreads = 288;  // warpgroups 0-1 wgmma + epilogue, warp 8 producer (no idle warps)
+constexpr int kWgProducerWarp = 8;
 
 struct WgTcArgs {
   int co, ci, taps, wp;
@@ -33,36 +34,38 @@ struct WgTcArgs {
   int layout;           // Y3_DW_OIHW [co][ci][taps] | Y3_DW_TAP_MAJOR [taps][co][ci] | Y3_DW_OHWI [co][taps][ci] (vector reductions)
   int single;           // 1: this CTA is the only contributor to its dW tile AND dw need not be accumulated into (plain stores)
   int* err;
-  uint32_t lbo_a, lbo_b, sbo_a, sbo_b;  // descriptor strides in bytes (probe-able, see Y3_WGRAD_VARIANT)
+  uint32_t lbo_a, lbo_b, sbo_a, sbo_b;  // descriptor strides in bytes
   // stride-2 "patch" mode (KB = 80): a K block is a tw x th patch of OUTPUT pixels; dy comes through a 4-D map of its padded
   // grid, x through the 5-D parity view the forward stride-2 conv uses (one box per tap)
   int s2, tw, th, tiles_w, tiles_per_img, x_ld;
 };
 
-// N = ci tile width (32 .. 256); SWZ = bytes of one smem row = min(N, 64) * 2 for B, 128 for A; KB = pixels per K block
 template <int N, int KB>
-__global__ void __launch_bounds__(kWgThreads, 2)
+struct WgCfg {
+  static constexpr int kBCols = N >= 64 ? 64 : N;            // channels per B box
+  static constexpr uint32_t kStage = 2 * KB * 128 + (N / kBCols) * KB * kBCols * 2;
+  static constexpr int kStages = (200 * 1024) / kStage > 6 ? 6 : (200 * 1024) / kStage;
+  static constexpr size_t kSmemBytes = size_t(kStages) * kStage + 1024 + 256;
+  static_assert(kStages >= 2, "wgrad: the ring needs two stages");
+};
+
+// N = ci tile width (32 .. 256); KB = pixels per K block
+template <int N, int KB>
+__global__ void __launch_bounds__(kWgThreads, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const WgTcArgs p) {
-  constexpr int kBCols = N >= 64 ? 64 : N;            // channels per B box
+  constexpr int kBCols = WgCfg<N, KB>::kBCols;
   constexpr int kBBoxes = N / kBCols;
   constexpr uint32_t kABox = KB * 128;                // one A box: KB pixel rows x 64 channels
   constexpr uint32_t kABytes = 2 * kABox;             // co 0-63 | co 64-127
   constexpr uint32_t kBBox = KB * kBCols * 2;
-  constexpr uint32_t kBBytes = kBBoxes * kBBox;
-  constexpr uint32_t kStage = kABytes + kBBytes;
-  // <= ~100 KB of ring: two CTAs per SM, so one CTA's prologue / atomic epilogue overlaps the other's main loop
-  constexpr int STAGES = N >= 256 ? 3 : ((100 * 1024) / kStage > 4 ? 4 : (100 * 1024) / kStage);
-  constexpr uint32_t kLayoutA = 2u, kLayoutB = kBCols == 64 ? 2u : 4u;  // SWIZZLE_128B / SWIZZLE_64B
-  constexpr uint32_t IDESC = umma_idesc_bf16(kWgM, N) | (1u << 15) | (1u << 16);  // A and B MN-major
-  constexpr uint32_t kTmemCols = N < 32 ? 32 : N;
+  constexpr uint32_t kStage = WgCfg<N, KB>::kStage;
+  constexpr int STAGES = WgCfg<N, KB>::kStages;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (raw_addr & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * kStage);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* done_bar = empty_bar + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done_bar + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.y;  // co tile * n_ci_tiles + ci tile
@@ -78,136 +81,111 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constan
     tma_prefetch_desc(&map_x);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
-    mbar_init(done_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();  // prologue above overlaps the previous kernel's tail (y3_common.cuh)
   pdl_trigger();
+  if (k_iters <= 0) return;
 
-  if (k_iters > 0) {
-    if (warp == 0) {
-      uint32_t stage = 0, phase = 0;
-      for (int it = 0; it < k_iters; ++it) {
-        mbar_wait(&empty_bar[stage], phase ^ 1u, p.err, 11);
-        if (elect_one()) {
-          uint8_t* a_dst = smem + stage * kStage;
-          uint8_t* b_dst = a_dst + kABytes;
-          mbar_expect_tx(&full_bar[stage], kStage);
-          if (KB == 80) {  // stride-2 patch mode
-            const int kb = kb0 + it;
-            const int img = kb / p.tiles_per_img, t = kb - img * p.tiles_per_img;
-            const int oy0 = (t / p.tiles_w) * p.th, ox0 = (t % p.tiles_w) * p.tw;
-            const int r = tap / 3, sx = tap - r * 3;
-            tma_load_4d(a_dst, &map_dy, &full_bar[stage], p.dy_coff + co0, 1 + ox0, 1 + oy0, img);
-            tma_load_4d(a_dst + kABox, &map_dy, &full_bar[stage], p.dy_coff + co0 + 64, 1 + ox0, 1 + oy0, img);
+  if (warp == kWgProducerWarp) {
+    uint32_t stage = 0, phase = 0;
+    for (int it = 0; it < k_iters; ++it) {
+      mbar_wait(&empty_bar[stage], phase ^ 1u, p.err, 11);
+      if (elect_one()) {
+        uint8_t* a_dst = smem + stage * kStage;
+        uint8_t* b_dst = a_dst + kABytes;
+        mbar_expect_tx(&full_bar[stage], kStage);
+        if (KB == 80) {  // stride-2 patch mode
+          const int kb = kb0 + it;
+          const int img = kb / p.tiles_per_img, t = kb - img * p.tiles_per_img;
+          const int oy0 = (t / p.tiles_w) * p.th, ox0 = (t % p.tiles_w) * p.tw;
+          const int r = tap / 3, sx = tap - r * 3;
+          tma_load_4d(a_dst, &map_dy, &full_bar[stage], p.dy_coff + co0, 1 + ox0, 1 + oy0, img);
+          tma_load_4d(a_dst + kABox, &map_dy, &full_bar[stage], p.dy_coff + co0 + 64, 1 + ox0, 1 + oy0, img);
 #pragma unroll
-            for (int b = 0; b < kBBoxes; ++b)  // input pixel of output (oy, ox), tap (r, sx): padded (2 oy + r, 2 ox + sx)
-              tma_load_5d(b_dst + b * kBBox, &map_x, &full_bar[stage], (sx & 1) * p.x_ld + p.x_coff + ci0 + b * kBCols,
-                          ox0 + (sx >> 1), r & 1, oy0 + (r >> 1), img);
-          } else {
-            const int row = (kb0 + it) * KB;
-            tma_load_2d(a_dst, &map_dy, &full_bar[stage], p.dy_coff + co0, row);
-            tma_load_2d(a_dst + kABox, &map_dy, &full_bar[stage], p.dy_coff + co0 + 64, row);
+          for (int b = 0; b < kBBoxes; ++b)  // input pixel of output (oy, ox), tap (r, sx): padded (2 oy + r, 2 ox + sx)
+            tma_load_5d(b_dst + b * kBBox, &map_x, &full_bar[stage], (sx & 1) * p.x_ld + p.x_coff + ci0 + b * kBCols,
+                        ox0 + (sx >> 1), r & 1, oy0 + (r >> 1), img);
+        } else {
+          const int row = (kb0 + it) * KB;
+          tma_load_2d(a_dst, &map_dy, &full_bar[stage], p.dy_coff + co0, row);
+          tma_load_2d(a_dst + kABox, &map_dy, &full_bar[stage], p.dy_coff + co0 + 64, row);
 #pragma unroll
-            for (int b = 0; b < kBBoxes; ++b)
-              tma_load_2d(b_dst + b * kBBox, &map_x, &full_bar[stage], p.x_coff + ci0 + b * kBCols, row + shift);
-          }
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
+          for (int b = 0; b < kBBoxes; ++b)
+            tma_load_2d(b_dst + b * kBBox, &map_x, &full_bar[stage], p.x_coff + ci0 + b * kBCols, row + shift);
         }
       }
-    } else if (warp == 1) {
-      uint32_t stage = 0, phase = 0;
-      const uint32_t hi_a = ((p.sbo_a >> 4) & 0x3FFFu) | (1u << 14) | (kLayoutA << 29);
-      const uint32_t hi_b = ((p.sbo_b >> 4) & 0x3FFFu) | (1u << 14) | (kLayoutB << 29);
-      const uint32_t lo_a0 = ((smem_u32(smem) >> 4) & 0x3FFFu) | (((p.lbo_a >> 4) & 0x3FFFu) << 16);
-      const uint32_t lo_b0 = (((smem_u32(smem) + kABytes) >> 4) & 0x3FFFu) | (((p.lbo_b >> 4) & 0x3FFFu) << 16);
-      constexpr uint32_t kRowA = 128, kRowB = kBCols * 2;  // bytes per pixel row inside a box
-      for (int it = 0; it < k_iters; ++it) {
-        mbar_wait(&full_bar[stage], phase, p.err, 12);
-        tc_fence_after();
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < KB / 16; ++ks) {
-            const uint64_t adesc = (uint64_t(hi_a) << 32) | (lo_a0 + ((stage * kStage + ks * 16 * kRowA) >> 4));
-            const uint64_t bdesc = (uint64_t(hi_b) << 32) | (lo_b0 + ((stage * kStage + ks * 16 * kRowB) >> 4));
-            umma_bf16_ss(tmem_base, adesc, bdesc, IDESC, (it | ks) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (it == k_iters - 1) umma_commit(done_bar);
-        }
-        __syncwarp();
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
+      __syncwarp();
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
       }
-    } else {
-      // epilogue: TMEM lane = co row, columns = ci; fp32 atomics into dW[co][ci][tap]
-      const int quarter = warp & 3;
-      const int co = co0 + quarter * 32 + lane;
-      mbar_wait(done_bar, 0, p.err, 13);
-      tc_fence_after();
-      const bool rows_contig = p.layout != Y3_DW_OIHW || p.taps == 1;  // this thread's ci run is contiguous in memory
+    }
+  } else {
+    const int wg = warp >> 2;  // co rows [64 wg, 64 wg + 64) of the tile
+    const uint32_t hi_a = wgmma_desc_hi(p.sbo_a, 128);
+    const uint32_t hi_b = wgmma_desc_hi(p.sbo_b, kBCols * 2);
+    const uint32_t a0 = smem_u32(smem) + uint32_t(wg) * kABox, b0 = smem_u32(smem) + kABytes;
+    constexpr uint32_t kRowA = 128, kRowB = kBCols * 2;  // bytes per pixel row inside a box
+    float acc[N / 2];
+    uint32_t stage = 0, phase = 0, prev = 0;
+    for (int it = 0; it < k_iters; ++it) {
+      mbar_wait(&full_bar[stage], phase, p.err, 12);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < KB / 16; ++ks) {
+        const uint64_t adesc = wgmma_desc(hi_a, a0 + stage * kStage + ks * 16 * kRowA, p.lbo_a);
+        const uint64_t bdesc = wgmma_desc(hi_b, b0 + stage * kStage + ks * 16 * kRowB, p.lbo_b);
+        Wgmma<N>::template mma<1, 1>(acc, adesc, bdesc, (it | ks) != 0 ? 1u : 0u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();  // the previous stage's MMAs have completed: its slot may be refilled
+      if (it > 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+
+    // epilogue: accumulator row = co, column = ci; fp32 atomics (or plain stores) into dW
+    const bool rows_contig = p.layout != Y3_DW_OIHW || p.taps == 1;  // this thread's ci run is contiguous in memory
+    const int cq = 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int co = co0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+      if (co >= p.co) continue;
       float* dst = p.layout == Y3_DW_OHWI ? p.dw + (static_cast<long long>(co) * p.taps + tap) * p.ci + ci0
                    : rows_contig          ? p.dw + (static_cast<long long>(tap) * p.co + co) * p.ci + ci0
                                           : p.dw + (static_cast<long long>(co) * p.ci + ci0) * p.taps + tap;
-#pragma unroll 1
-      for (int c = 0; c < N; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + c, v);
-        tmem_ld_wait();
-        if (co >= p.co) continue;
-        if (rows_contig && ci0 + c + 32 <= p.ci) {
-          // 128 contiguous bytes per thread: 16-byte vector reductions (or plain stores when nobody else adds to this tile)
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            float* q = dst + c + j;
-            if (p.single)
-              *reinterpret_cast<float4*>(q) = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]),
-                                                          __uint_as_float(v[j + 2]), __uint_as_float(v[j + 3]));
-            else
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(q), "f"(__uint_as_float(v[j])),
-                           "f"(__uint_as_float(v[j + 1])), "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
-                           : "memory");
-          }
+      for (int j = 0; j < N / 8; ++j) {
+        const int c = 8 * j + cq;
+        const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+        if (rows_contig && ci0 + c + 2 <= p.ci) {
+          float* q = dst + c;  // two contiguous floats: 8-byte vector reduction (or a plain store when nobody else adds)
+          if (p.single)
+            *reinterpret_cast<float2*>(q) = make_float2(v0, v1);
+          else
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(q), "f"(v0), "f"(v1) : "memory");
         } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (ci0 + c + j < p.ci)
-              atomicAdd(dst + static_cast<long long>(c + j) * (rows_contig ? 1 : p.taps), __uint_as_float(v[j]));
+          const long long step = rows_contig ? 1 : p.taps;
+          if (ci0 + c < p.ci) atomicAdd(dst + c * step, v0);
+          if (ci0 + c + 1 < p.ci) atomicAdd(dst + (c + 1) * step, v1);
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
 template <int N, int KB>
 int wgrad_tc_launch(const CUtensorMap& mdy, const CUtensorMap& mx, const WgTcArgs& a, dim3 grid, cudaStream_t stream) {
-  constexpr int kBCols = N >= 64 ? 64 : N;
-  constexpr uint32_t kStage = 2 * KB * 128 + (N / kBCols) * KB * kBCols * 2;
-  constexpr int STAGES = N >= 256 ? 3 : ((100 * 1024) / kStage > 4 ? 4 : (100 * 1024) / kStage);
-  static_assert(STAGES >= 2, "wgrad: the ring needs two stages");
-  constexpr size_t smem = size_t(STAGES) * kStage + 1024 + 256;
+  constexpr size_t smem = WgCfg<N, KB>::kSmemBytes;
   auto kern = wgrad_tc_kernel<N, KB>;
   static bool attr_set = false;
   if (!attr_set) {
@@ -220,8 +198,7 @@ int wgrad_tc_launch(const CUtensorMap& mdy, const CUtensorMap& mx, const WgTcArg
 
 }  // namespace
 
-// Y3_WGRAD_TC=0 keeps the warp-level MMA kernel.  Y3_WGRAD_VARIANT (probe of the MN-major descriptor strides, round 1):
-//   0 (default) LBO = bytes between 64-channel boxes, SBO = 1024;  1: LBO and SBO swapped;  2: LBO = 0 / SBO = 1024
+// Y3_WGRAD_TC=0 keeps the warp-level MMA kernel.
 int wgrad_tc_enabled() {
   static int v = -1;
   if (v < 0) {
@@ -302,9 +279,9 @@ static int wgrad_tc_s2(const y3_wgrad_desc& d, cudaStream_t stream) {
   a.sbo_a = 1024;
   a.sbo_b = 8 * bcols * 2;
   const int tiles = ((d.co + kWgM - 1) / kWgM) * a.n_ci_tiles;
-  // split the pixel dimension so that the grid is ONE wave of the 2 CTAs an SM holds (floor, not ceil: 33 splits x 9 taps = 297
-  // CTAs on 296 slots ran a second wave for a single CTA — 196 us instead of ~110, gpurun r2j6)
-  long long want = (2ll * num_sms()) / (static_cast<long long>(tiles) * 9);
+  // split the pixel dimension so that the grid is ONE wave of CTAs, one per SM (floor, not ceil: a grid a few CTAs over a
+  // wave costs a whole extra wave)
+  long long want = static_cast<long long>(num_sms()) / (static_cast<long long>(tiles) * 9);
   long long max_split = (a.kblocks_total + 7) / 8;
   if (want > max_split) want = max_split;
   if (want < 1 || d.deterministic) want = 1;
@@ -325,7 +302,7 @@ int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream) {
   const int taps = d.ksize * d.ksize;
   const long long rows = static_cast<long long>(d.n) * (d.h + 2) * (d.w + 2);
   Y3_REQUIRE(rows < (1ll << 31) - 4096, "wgrad: too many pixels");
-  static int n_max = -1;  // Y3_WGRAD_NMAX=256 allows 256-wide ci tiles (one CTA per SM); default 128 (two CTAs per SM)
+  static int n_max = -1;  // Y3_WGRAD_NMAX=256 allows 256-wide ci tiles; default 128
   if (n_max < 0) {
     const char* e = getenv("Y3_WGRAD_NMAX");
     n_max = (e && atoi(e) == 256) ? 256 : 128;
@@ -359,29 +336,14 @@ int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream) {
   a.x_coff = d.x_coff;
   a.dw = d.dw;
   a.err = nullptr;
-  static int variant = -1;
-  if (variant < 0) {
-    const char* e = getenv("Y3_WGRAD_VARIANT");
-    variant = e ? atoi(e) : 0;
-  }
-  const uint32_t box_a = kWgK * 128, box_b = kWgK * bcols * 2;
-  a.lbo_a = box_a;
-  a.lbo_b = box_b;
-  a.sbo_a = 1024;            // 8 pixel rows of 128 B
-  a.sbo_b = 8 * bcols * 2;   // 8 pixel rows of a B box
-  if (variant == 1) {
-    a.lbo_a = a.sbo_a;
-    a.lbo_b = a.sbo_b;
-    a.sbo_a = box_a;
-    a.sbo_b = box_b;
-  } else if (variant == 2) {
-    a.lbo_a = 0;
-    a.lbo_b = 0;
-  }
+  a.lbo_a = kWgK * 128;          // bytes between 64-channel boxes
+  a.lbo_b = kWgK * bcols * 2;
+  a.sbo_a = 1024;                 // 8 pixel rows of 128 B
+  a.sbo_b = 8 * bcols * 2;        // 8 pixel rows of a B box
   const int tiles = ((d.co + kWgM - 1) / kWgM) * a.n_ci_tiles;
-  // split the pixel dimension so that ~2 CTAs per SM exist; at least 8 pixel blocks per CTA
-  // one wave of the 2 resident CTAs per SM (floor: a grid a few CTAs over a wave costs a whole extra wave)
-  long long want = (2ll * num_sms()) / (static_cast<long long>(tiles) * taps);
+  // split the pixel dimension into one wave of CTAs, one per SM (floor: a grid a few CTAs over a wave costs a whole extra
+  // wave); at least 8 pixel blocks per CTA
+  long long want = static_cast<long long>(num_sms()) / (static_cast<long long>(tiles) * taps);
   long long max_split = (a.kblocks_total + 7) / 8;
   if (want > max_split) want = max_split;
   if (want < 1) want = 1;

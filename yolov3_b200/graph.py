@@ -63,7 +63,7 @@ def parse(cfg: dict, ch: int = 3):
     for i, (f, n, m, args) in enumerate(cfg["backbone"] + cfg["head"]):
         m = m.replace("nn.", "") if isinstance(m, str) else m.__name__
         if m not in SUPPORTED:
-            raise NotImplementedError(f"layer type {m!r} is not used by the YOLOv3 YAMLs and has no sm_100a kernel here")
+            raise NotImplementedError(f"layer type {m!r} is not used by the YOLOv3 YAMLs and has no sm_90a kernel here")
         args = [nc if a == "nc" else anchors if a == "anchors" else (None if a == "None" else a) for a in args]
         n = max(round(n * gd), 1) if n > 1 else n
         if m in ("Conv", "Bottleneck", "SPP"):

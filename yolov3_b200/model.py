@@ -1,5 +1,5 @@
 """``Model`` — host-side mirror of the reference's ``DetectionModel`` (models/yolo.py:193-295) whose forward runs
-entirely in the sm_100a library: the YAML graph is lowered once per input shape into a flat list of prepared kernel
+entirely in the sm_90a library: the YAML graph is lowered once per input shape into a flat list of prepared kernel
 launches (``Engine``), executed by ``y3_model_forward`` and optionally replayed as a CUDA graph.
 
 What is kept from the reference surface (SURVEY.md §8b): ``Model(cfg, ch, nc, anchors)``, ``.forward(x)`` returning
@@ -269,7 +269,7 @@ class Model:
         if profile or visualize:
             raise NotImplementedError("profile/visualize are outside the accelerated path (SURVEY §8a)")
         if not x.is_cuda:
-            raise RuntimeError("yolov3_b200 has no CPU path: move the input to the B200 (x.cuda())")
+            raise RuntimeError("yolov3_b200 has no CPU path: move the input to the GPU (x.cuda())")
         if augment:  # models/yolo.py:235-236: augmented inference returns (z_aug, None)
             if self.training:
                 raise RuntimeError("augment=True is an inference option (models/yolo.py:233-237)")

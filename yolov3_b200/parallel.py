@@ -52,7 +52,7 @@ def allreduce_gradients(params, average: bool = True, flat: torch.Tensor | None 
 
 
 class DDP:
-    """``smart_DDP(model)`` (utils/torch_utils.py:60-72) for the B200 ``Model``: marks the model so that its training engine
+    """``smart_DDP(model)`` (utils/torch_utils.py:60-72) for the GPU ``Model``: marks the model so that its training engine
     overlaps the bucketed gradient all-reduce with the backward pass, and broadcasts rank 0's parameters like DDP's
     constructor does (train.py:323).  ``forward`` / attribute access go to the wrapped model (``de_parallel`` not needed).
 

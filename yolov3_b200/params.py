@@ -6,7 +6,7 @@ buffer), laid out for the training hot path:
   all-reduced while the rest of the backward runs (the reference gets the same overlap from DistributedDataParallel's
   buckets, utils/torch_utils.py:60-72);
 * every conv weight is stored ``[co][kh][kw][ci]`` — the channels_last strides of the ``[co, ci, k, k]`` parameter tensor the
-  reference names ``model.N.conv.weight`` — which is exactly the K-major order the tcgen05 conv kernel wants, so the bf16
+  reference names ``model.N.conv.weight`` — which is exactly the K-major order the wgmma conv kernel wants, so the bf16
   forward packs are views of one elementwise bf16 copy of this buffer and the wgrad kernel accumulates straight into the
   parameter's ``.grad`` view (no permute, no per-layer copies);
 * every slot is padded to a multiple of 256 elements and tagged with its optimizer group (smart_optimizer,
@@ -161,9 +161,9 @@ class ParamStore:
     def bucket_ranges(self, n_buckets=4, tail_fraction=0.012):
         """Contiguous element ranges of G (slot-aligned) in backward-completion order.  The LAST bucket — the only one whose
         all-reduce cannot hide behind remaining backward work — is kept small (``tail_fraction`` of the gradient bytes: in
-        YOLOv3 the layers back-propagated last, 0..5, hold ~1 % of the parameters (2.8 MB) but ~30 % of the backward time; with
-        an 18 MB tail — layers 0..7 — 0.53 ms of the exchange stayed exposed on 8 GPUs, gpurun r2j10); the rest is split
-        evenly."""
+        YOLOv3 the layers back-propagated last, 0..5, hold ~1 % of the parameters (2.8 MB), so their exchange after the
+        backward is short; a larger tail — layers 0..7, 18 MB — left a visible share of the exchange exposed); the rest is
+        split evenly."""
         names = [n for n in self.order if self.slots[n].group != G_FROZEN]
         total = self.n_train
         cuts = [total * (1 - tail_fraction) * (i + 1) / (n_buckets - 1) for i in range(n_buckets - 1)] if n_buckets > 1 else []

@@ -1,5 +1,5 @@
 """Per-launch timing of an Engine (CUDA events on the launching stream) with the algorithmic FLOPs / bytes of every
-launch, for the roofline numbers bench.py reports and the tables under profiles/."""
+launch, for the roofline numbers bench.py reports."""
 from __future__ import annotations
 
 import ctypes as C

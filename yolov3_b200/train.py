@@ -1,13 +1,13 @@
-"""Training-mode forward + backward of the YOLOv3 graph on the sm_100a kernels (SURVEY §8 rows a19/a20).
+"""Training-mode forward + backward of the YOLOv3 graph on the sm_90a kernels (SURVEY §8 rows a19/a20).
 
 Mirrors what the reference runs in ``train.py:401-411`` — ``pred = model(imgs)`` in train mode (BatchNorm with batch
 statistics, eps 1e-3 / momentum 0.03; ``Detect`` returning the raw ``[bs,na,ny,nx,no]`` maps, models/yolo.py:110), then
 ``loss.backward()`` through every Conv block — without autograd graphs or cuDNN:
 
-  forward  per Conv block:  conv (tcgen05 implicit GEMM, identity epilogue) -> bn_stats (per-block partial sums)
+  forward  per Conv block:  conv (wgmma implicit GEMM, identity epilogue) -> bn_stats (per-block partial sums)
                             -> bn_finalize (fixed-order second stage, running statistics) -> bn_act_fwd
   backward per Conv block:  bn_act_bwd (partial sums -> dgamma/dbeta accumulated into the flat gradient buffer -> dy)
-                            -> wgrad (tcgen05, accumulating straight into the parameter's .grad view)
+                            -> wgrad (wgmma, accumulating straight into the parameter's .grad view)
                             -> dgrad, which is the SAME conv kernel run on dy with the transposed, tap-flipped weight pack
                                (stride-2 layers: on the zero-stuffed dy), accumulating into the input's gradient through
                                the residual port (the Bottleneck shortcut's gradient rides on that port too).

@@ -114,7 +114,7 @@ def zero_stuff(src: PaddedNHWC, dst: PaddedNHWC):
 
 
 def wgrad_tap_major(ci: int) -> bool:
-    """True when y3_conv_wgrad takes the [k*k, co, ci] accumulation layout for this c_in (tcgen05 kernel in use)."""
+    """True when y3_conv_wgrad takes the [k*k, co, ci] accumulation layout for this c_in (wgmma kernel in use)."""
     return bool(_lib.lib().y3_conv_wgrad_tap_major(int(ci)))
 
 
