@@ -48,6 +48,15 @@ CASES = [
     dict(name="1x1_n32_res_many_tiles", n=4, h=80, w=80, cin=64, cout=32, k=1, s=1, res=True),
     dict(name="1x1_k512_n256_res", n=2, h=40, w=40, cin=512, cout=256, k=1, s=1, res=True),      # staged, one buffer
     dict(name="3x3_k64_n64_res_many_tiles", n=4, h=80, w=80, cin=64, cout=64, k=3, s=1, res=True),
+    # residual staged in shared memory (N = 256) over many tiles, and the residual aliasing the output (training dgrad)
+    # with CTAs running more than one tile
+    dict(name="3x3_k128_n256_res_many_tiles", n=4, h=80, w=80, cin=128, cout=256, k=3, s=1, res=True),
+    dict(name="3x3_k128_n256_res_is_out", n=4, h=80, w=80, cin=128, cout=256, k=3, s=1, res=True, res_alias=True),
+    dict(name="3x3_k64_n128_res_is_out", n=4, h=80, w=80, cin=64, cout=128, k=3, s=1, res=True, res_alias=True),
+    # a padded N tile (c_out 96 in a tile of 128) written at a channel offset of a wider buffer whose other channels hold
+    # poison: they must keep it
+    dict(name="3x3_n96_res_out_coff_poison", n=2, h=20, w=20, cin=64, cout=96, k=3, s=1, res=True, out_ld=256, out_coff=64,
+         out_poison=True),
 ]
 
 
@@ -97,7 +106,11 @@ def run_case(c):
         halo_ok = bool((head[:, cout:] == 0).all())
     else:
         out = PaddedNHWC.zeros(n, ho * u, wo * u, cout, ld=c.get("out_ld", cout))
+        poison = 7.0 if c.get("out_poison") else 0.0
+        out.buf[:, 1:-1, 1:-1, :] = poison
         out = out.slice(c.get("out_coff", 0), cout) if c.get("out_ld") else out
+        if c.get("res_alias"):
+            out = res
         ops.conv_bn_act(xin, wp, bp, cout, k, s, act, out=out, res=res, upsample=bool(c.get("upsample")), err=err,
                         weight_layout=layout)
         torch.cuda.synchronize()
@@ -108,8 +121,8 @@ def run_case(c):
         halo = bufc.clone()
         halo[:, 1:-1, 1:-1, :] = 0
         other = bufc[:, 1:-1, 1:-1, :].clone()
-        other[..., out.coff:out.coff + cout] = 0
-        halo_ok = bool((halo == 0).all()) and bool((other == 0).all())
+        other[..., out.coff:out.coff + cout] = poison
+        halo_ok = bool((halo == 0).all()) and bool((other == poison).all())
     diff = (got - ref).abs()
     tol = 2e-2 + 1e-2 * ref.abs()
     bad = diff > tol

@@ -59,6 +59,20 @@ struct Cfg {
   static constexpr uint32_t kSwizzleBytes = BLOCK_K * 2;  // 32 / 64 / 128: one smem row of an operand tile
   static constexpr uint32_t kSbo = 8 * kSwizzleBytes;
   static constexpr uint32_t kBarBytes = 256;              // mbarriers
+  // N = 256 keeps 128 accumulators per thread and has no registers left to batch residual loads in the epilogue: each
+  // consumer thread copies its own residual elements into shared memory (cp.async) when a tile starts, and the copies
+  // land during the main loop.  Launches with a residual give the ring the bytes of that buffer (launch_cfg).
+  static constexpr bool kResSmem = BLOCK_N == 256;
+  static constexpr uint32_t kResBytes = kResSmem ? kBlockM * BLOCK_N * 2 : 0;
+  // Shared-memory layout from the 1 KB-aligned base, as conv_tc_kernel lays it out: A ring, then B ring or resident
+  // weights, then the mbarriers (bar_offset), then the residual buffer (kResSmem launches with a residual).  launch_cfg
+  // checks smem_end() against the allocation before every launch.
+  __host__ __device__ static constexpr uint32_t bar_offset(int stages, bool bres, int b_steps) {
+    return uint32_t(stages) * kABytes + (bres ? bres_bytes(b_steps) : uint32_t(stages) * kTaps * kBBytes);
+  }
+  __host__ __device__ static constexpr uint32_t smem_end(int stages, bool bres, int b_steps, bool res) {
+    return bar_offset(stages, bres, b_steps) + kBarBytes + (res ? kResBytes : 0u);
+  }
   static constexpr size_t kSmemBytes = size_t(kSmemBudget) + 1024 /*align*/ + kBarBytes;
   static_assert(kStages >= 2, "pipeline needs at least two stages");
   static_assert(!HALO || BLOCK_K >= 32, "halo reuse: rows of 64 or 128 bytes");
@@ -72,6 +86,16 @@ __device__ __forceinline__ float bias_act(float a, float b, bool silu) {
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
   return fmaf(h, t, h);
+}
+
+__device__ __forceinline__ void cp_async4(uint32_t saddr, const void* gptr) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(saddr), "l"(gptr) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(saddr));
+  return v;
 }
 
 // exact n / d for any 32-bit n with a precomputed (multiplier, shift) pair (host: fast_div_for)
@@ -261,7 +285,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     const uint32_t b_base = smem_u32(smem_b);
     uint32_t stage = 0, phase = 0;
     if (bres && int(blockIdx.x) < total_tiles) mbar_wait(bres_bar, 0, p.err, 6);  // resident weights have landed
+    // kResSmem: word (h * BLOCK_N / 8 + j) * 256 + threadIdx.x holds this thread's residual pair j of row m0 + 8 h
+    // (recomputed where it is used: no register is left to keep it through the main loop)
+    auto res_slot = [&]() { return smem_u32(full_bar) + C::kBarBytes + threadIdx.x * 4u; };
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      if (C::kResSmem && p.res) {
+        const uint32_t res_s = res_slot();
+        // Only this thread reads these words back, after its own cp.async.wait_all: no barrier.  The previous tile's reads
+        // of them completed before its stores were issued.  With res == out the residual of a tile is read before that
+        // tile's stores, and tiles are disjoint.
+        const int n0 = (tile % p.n_tiles) * BLOCK_N;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const RowOut ro = row_out(p, tile / p.n_tiles, n0, m0 + 8 * h);
+          if (!ro.res) continue;
+#pragma unroll 4
+          for (int j = 0; j < BLOCK_N / 8; ++j)
+            if (n0 + 8 * j + cq < p.cout) cp_async4(res_s + uint32_t(h * BLOCK_N / 8 + j) * 1024u, ro.res + 8 * j + cq);
+        }
+      }
       float acc[BLOCK_N / 2];
       uint32_t prev = 0;
       for (int it = 0; it < k_iters; ++it) {
@@ -301,29 +343,51 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       const bool silu = p.act == Y3_ACT_SILU;
       const float bscale = silu ? 0.5f : 1.0f;
       const int reps = p.upsample ? 4 : 1;
-      // one row at a time: only that row's three output pointers are live beside the accumulators (N = 256 keeps 128)
+      // one row at a time: only that row's three output pointers are live beside the accumulators (N = 256 keeps 128).
+      // The residual may alias the output (training dgrad: res == out), so the compiler keeps every residual load behind
+      // the stores that precede it in program order.  Loading a whole chunk of column pairs (bias and residual) before
+      // the first store of that chunk makes it one trip to memory per chunk instead of one per column pair.  Correct with
+      // res == out: a thread reads exactly the elements it then overwrites, and tiles are disjoint.
+      constexpr int kChunk = C::kResSmem ? 1 : (BLOCK_N / 8 < 16 ? BLOCK_N / 8 : 16);  // column pairs per batch
+      if (C::kResSmem && p.res) cp_async_wait_all();
+      const uint32_t res_s = C::kResSmem ? res_slot() : 0u;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const RowOut ro = row_out(p, mt, n0, m0 + 8 * h);
         if (!ro.f32 && !ro.out) continue;
 #pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const int c = 8 * j + cq;
-          if (!p.out_f32 && n0 + c >= p.cout) continue;  // c_out % 32 == 0: a column pair is either inside or outside
-          const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c));
-          float x0 = bias_act(acc[4 * j + 2 * h], bscale * b.x, silu);
-          float x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b.y, silu);
-          if (ro.f32) {
-            *reinterpret_cast<float2*>(ro.f32 + c) = make_float2(x0, x1);
-          } else {
-            if (ro.res) {
-              const float2 f = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(ro.res + c));
-              x0 += f.x;
-              x1 += f.y;
+        for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
+          float2 b[kChunk];
+          uint32_t r[kChunk];
+#pragma unroll
+          for (int jj = 0; jj < kChunk; ++jj) {
+            const int c = 8 * (j0 + jj) + cq;
+            const bool in = p.out_f32 || n0 + c < p.cout;  // c_out % 32 == 0: a column pair is either inside or outside
+            b[jj] = in ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
+            if (C::kResSmem)
+              r[jj] = (in && ro.res) ? lds32(res_s + uint32_t(h * BLOCK_N / 8 + j0 + jj) * 1024u) : 0u;
+            else
+              r[jj] = (in && ro.res) ? __ldcg(reinterpret_cast<const unsigned int*>(ro.res + c)) : 0u;
+          }
+#pragma unroll
+          for (int jj = 0; jj < kChunk; ++jj) {
+            const int j = j0 + jj;
+            const int c = 8 * j + cq;
+            if (!p.out_f32 && n0 + c >= p.cout) continue;
+            float x0 = bias_act(acc[4 * j + 2 * h], bscale * b[jj].x, silu);
+            float x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b[jj].y, silu);
+            if (ro.f32) {
+              *reinterpret_cast<float2*>(ro.f32 + c) = make_float2(x0, x1);
+            } else {
+              if (ro.res) {
+                const float2 f = unpack_bf16x2(r[jj]);
+                x0 += f.x;
+                x1 += f.y;
+              }
+              const uint32_t v = pack_bf16x2(x0, x1);
+              for (int rep = 0; rep < reps; ++rep)
+                *reinterpret_cast<uint32_t*>(ro.out + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + c) = v;
             }
-            const uint32_t v = pack_bf16x2(x0, x1);
-            for (int rep = 0; rep < reps; ++rep)
-              *reinterpret_cast<uint32_t*>(ro.out + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + c) = v;
           }
         }
       }
@@ -347,6 +411,20 @@ int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
     args.bres = 0;
     args.stages = C::kStages;
   }
+  if (C::kResSmem && args.res) {  // the residual staging buffer takes its bytes from the ring
+    const int ring = int(kSmemBudget - C::kResBytes) - (args.bres ? int(C::bres_bytes(args.taps * args.kblocks)) : 0);
+    args.stages = ring / int(args.bres ? C::kABytes : C::kStageBytes);
+    if (args.stages > C::kMaxStages) args.stages = C::kMaxStages;
+    if (args.stages < 3) {
+      args.bres = 0;
+      args.stages = int(kSmemBudget - C::kResBytes) / int(C::kStageBytes);
+    }
+  }
+  // the 1 KB alignment of the base comes out of the allocation's slack
+  if (args.stages < 2 || args.stages > C::kMaxStages ||
+      C::smem_end(args.stages, args.bres != 0, args.taps * args.kblocks, C::kResSmem && args.res) + 1024u > C::kSmemBytes)
+    return set_error(Y3_ERR_BAD_ARG, "conv_tc: %d ring stages (resident weights %d, residual %d) do not fit %zu bytes of shared memory (N=%d K=%d)",
+                     args.stages, args.bres, args.res != nullptr, C::kSmemBytes, BLOCK_N, BLOCK_K);
   // the kernel parks at pdl_wait() after its prologue (y3_common.cuh)
   Y3_CHECK_CUDA(launch_pdl(kern, dim3(plan.grid), dim3(kThreads), C::kSmemBytes, stream, plan.map_a, plan.map_b, args));
   return Y3_OK;
