@@ -10,11 +10,19 @@
 //   * a stride-2 conv reads the same buffer through a 5-D view (2*ld, (w+2)/2, 2, (h+2)/2, n) that splits rows and
 //     columns by parity; the A tile of tap (r,s) for a TH x TW patch of output pixels is one 5-D TMA box ("patch").
 //   * weights are bf16 [cout_pad, taps*cin] (K-major); B tile = [BLOCK_N x BLOCK_K] box.
-// Warp roles (288 threads, 1 CTA/SM, persistent over tiles): warp 8 = TMA producer (the whole warp runs the loop, one elected
+// Warp roles (320 threads, 1 CTA/SM, persistent over tiles): warp 8 = TMA producer (the whole warp runs the loop, one elected
 // lane issues); warpgroups 0 and 1 (warps 0-7) = consumers, each owning 64 of the tile's 128 rows: it issues the
-// m64 x BLOCK_N wgmma of its rows for every stage of the smem ring, releases a stage as soon as the MMAs that read it have
-// completed, and after the last k-block converts its accumulators straight from the registers (bias, SiLU, residual,
-// bf16 / fp32 stores).  While the consumers run the epilogue the producer already fills the ring for their next tile.
+// m64 x BLOCK_N wgmma of its rows for every stage of the smem ring and releases a stage as soon as the MMAs that read it
+// have completed; warp 9 = store warp (N = 256 bf16-output launches).  Per tile of such a launch:
+//   1. stage: during the tile's main loop the store warp copies the tile's residual into a 128 x BLOCK_N bf16 shared-memory
+//      tile and the BLOCK_N bias floats beside it (cp.async), then arrives on `staged`;
+//   2. finish: after the last k-block the consumers wait on `staged`, apply bias, SiLU and residual from their registers,
+//      write the bf16 pairs back into the same words, arrive on `done` and go straight on to the next tile's MMAs;
+//   3. drain: the store warp waits on `done` and writes the tile out with 16-byte stores (halo and out-of-range rows
+//      skipped, concat offset, nearest-2x upsample), then stages the next tile into the same buffer.
+// The fp32 Detect-head launches (a 128 x 256 fp32 tile does not fit beside the ring) and the N <= 128 launches (Cfg::kStaged)
+// store straight from the consumers' registers.  While the consumers finish a tile the producer already fills the ring for
+// their next one.
 #include <cuda_bf16.h>
 
 #include <cstdlib>
@@ -28,10 +36,11 @@ namespace y3 {
 namespace {
 
 constexpr int kBlockM = 128;
-// two consumer warpgroups + one producer warp: no idle warps, up to 224 registers per thread (the N = 256 tiles keep 128
-// accumulators each)
-constexpr int kThreads = 288;
+// two consumer warpgroups + one producer warp + one store warp.  Ten warps put at most three on any of the SM's four
+// register partitions, as nine did: 168 registers per thread (the N = 256 tiles keep 128 accumulators each)
+constexpr int kThreads = 320;
 constexpr int kProducerWarp = 8;
+constexpr int kStoreWarp = 9;
 constexpr int kSmemBudget = 221 * 1024;  // ring (+ resident weights); alignment slack and barriers come on top (227 KB max)
 
 // HALO = true (stride-1 3x3, BLOCK_K = 64 or 32): one pipeline stage covers a whole filter ROW (3 taps): the A operand is
@@ -48,33 +57,37 @@ struct Cfg {
   static constexpr uint32_t kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr uint32_t kStageBytes = kABytes + kTaps * kBBytes;
   static constexpr int kMaxStages = 8;
-  static constexpr int kStagesRaw = kSmemBudget / kStageBytes;
-  static constexpr int kStages = kStagesRaw > kMaxStages ? kMaxStages : kStagesRaw;
+  // N = 256 bf16-output launches hand the finished tile to the store warp: they keep the output tile (128 x BLOCK_N bf16)
+  // and the tile's BLOCK_N bias floats beside the ring, and those bytes come out of the ring's budget (`reserve`).
+  // Thinner tiles run only a few microseconds each: one warp cannot drain and restage them in that time, and their
+  // epilogue from the registers (batched bias and residual loads) costs less than the store warp's turn-around.
+  static constexpr bool kStaged = BLOCK_N == 256;
+  static constexpr uint32_t kTileBytes = kBlockM * BLOCK_N * 2;
+  static constexpr uint32_t kOutBytes = kTileBytes + BLOCK_N * 4;
+  __host__ __device__ static constexpr int ring_stages(uint32_t reserve) {
+    const int s = int(kSmemBudget - reserve) / int(kStageBytes);
+    return s > kMaxStages ? kMaxStages : s;
+  }
   // B-resident mode: `steps` weight boxes of kBBytes stay in shared memory for the whole kernel; the ring carries A only
   __host__ __device__ static constexpr uint32_t bres_bytes(int steps) { return (uint32_t(steps) * kBBytes + 1023u) / 1024u * 1024u; }
-  __host__ __device__ static constexpr int bres_stages(int steps) {
-    const int s = (int(kSmemBudget) - int(bres_bytes(steps))) / int(kABytes);
+  __host__ __device__ static constexpr int bres_stages(int steps, uint32_t reserve) {
+    const int s = (int(kSmemBudget - reserve) - int(bres_bytes(steps))) / int(kABytes);
     return s > kMaxStages ? kMaxStages : s;
   }
   static constexpr uint32_t kSwizzleBytes = BLOCK_K * 2;  // 32 / 64 / 128: one smem row of an operand tile
   static constexpr uint32_t kSbo = 8 * kSwizzleBytes;
   static constexpr uint32_t kBarBytes = 256;              // mbarriers
-  // N = 256 keeps 128 accumulators per thread and has no registers left to batch residual loads in the epilogue: each
-  // consumer thread copies its own residual elements into shared memory (cp.async) when a tile starts, and the copies
-  // land during the main loop.  Launches with a residual give the ring the bytes of that buffer (launch_cfg).
-  static constexpr bool kResSmem = BLOCK_N == 256;
-  static constexpr uint32_t kResBytes = kResSmem ? kBlockM * BLOCK_N * 2 : 0;
   // Shared-memory layout from the 1 KB-aligned base, as conv_tc_kernel lays it out: A ring, then B ring or resident
-  // weights, then the mbarriers (bar_offset), then the residual buffer (kResSmem launches with a residual).  launch_cfg
+  // weights, then the mbarriers (bar_offset), then the output tile and the bias (kStaged bf16-output launches).  launch_cfg
   // checks smem_end() against the allocation before every launch.
   __host__ __device__ static constexpr uint32_t bar_offset(int stages, bool bres, int b_steps) {
     return uint32_t(stages) * kABytes + (bres ? bres_bytes(b_steps) : uint32_t(stages) * kTaps * kBBytes);
   }
-  __host__ __device__ static constexpr uint32_t smem_end(int stages, bool bres, int b_steps, bool res) {
-    return bar_offset(stages, bres, b_steps) + kBarBytes + (res ? kResBytes : 0u);
+  __host__ __device__ static constexpr uint32_t smem_end(int stages, bool bres, int b_steps, bool out_tile) {
+    return bar_offset(stages, bres, b_steps) + kBarBytes + (out_tile ? kOutBytes : 0u);
   }
   static constexpr size_t kSmemBytes = size_t(kSmemBudget) + 1024 /*align*/ + kBarBytes;
-  static_assert(kStages >= 2, "pipeline needs at least two stages");
+  static_assert(ring_stages(kStaged ? kOutBytes : 0u) >= 2, "pipeline needs at least two stages");
   static_assert(!HALO || BLOCK_K >= 32, "halo reuse: rows of 64 or 128 bytes");
 };
 
@@ -88,15 +101,10 @@ __device__ __forceinline__ float bias_act(float a, float b, bool silu) {
   return fmaf(h, t, h);
 }
 
-__device__ __forceinline__ void cp_async4(uint32_t saddr, const void* gptr) {
-  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(saddr), "l"(gptr) : "memory");
+__device__ __forceinline__ void cp_async16(uint32_t saddr, const void* gptr) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(gptr) : "memory");
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
-__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
-  uint32_t v;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(saddr));
-  return v;
-}
 
 // exact n / d for any 32-bit n with a precomputed (multiplier, shift) pair (host: fast_div_for)
 __device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t mul, uint32_t shr) {
@@ -168,6 +176,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + (bres ? C::bres_bytes(b_steps) : uint32_t(STAGES) * kBStage));
   uint64_t* empty_bar = full_bar + C::kMaxStages;
   uint64_t* bres_bar = empty_bar + C::kMaxStages;
+  uint64_t* staged_bar = bres_bar + 1;  // store warp -> consumers: the tile's residual and bias are in shared memory
+  uint64_t* done_bar = bres_bar + 2;    // consumers -> store warp: the finished tile is in shared memory
+  // output tile: word (h * BLOCK_N / 8 + j) * 256 + t holds consumer thread t's column pair j of its row m0 + 8 h (the
+  // residual pair before the consumers finish the tile, the output pair after).  Lanes 4 r .. 4 r + 3 of a consumer warp
+  // hold 8 consecutive columns of one row, so 16 bytes at word (h * BLOCK_N / 8 + j) * 256 + 32 w + 4 r are 8 channels of
+  // one row of warp w
+  uint32_t* stile = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(full_bar) + C::kBarBytes);
+  float* sbias = reinterpret_cast<float*>(stile + C::kTileBytes / 4);
+  const bool staged_out = C::kStaged && p.out_f32 == nullptr;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -180,6 +197,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
     mbar_init(bres_bar, 1);
+    mbar_init(staged_bar, 32);  // every store-warp lane, after its own copies have landed
+    mbar_init(done_bar, 8);     // one arrival per consumer warp
     fence_mbar_init();
   }
   __syncthreads();
@@ -275,6 +294,97 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       run(std::integral_constant<int, 0>{});
     else
       run(std::integral_constant<int, 1>{});
+  } else if (warp == kStoreWarp) {
+    // ------------------------------------------------------------------ store warp (N = 256 bf16-output launches)
+    if (!staged_out) return;
+    // lane = 8 c + r: row r of 8 rows of one consumer warp's block, chunk c of 4 consecutive 16-byte chunks.  Each quarter
+    // warp reads 128 contiguous bytes of the tile (no bank conflict) and each row gets a 64-byte global segment.
+    const int r = lane & 7, c = lane >> 3;
+    const uint32_t stile_s = smem_u32(stile);
+    // The destinations of a tile's 128 rows are computed once, four per lane (rows lane + 32 q), before the tile is
+    // finished; the drain and the staging fetch them by shuffle.  Row (w >> 2) * 64 + (w & 3) * 16 + 8 h + r of the
+    // (h, w) loops below sits in slot q = 2 (w >> 2) + ((w & 3) >> 1) of lane 16 (w & 1) + 8 h + r.
+    struct Rows {
+      __nv_bfloat16* out[4];
+      const __nv_bfloat16* res[4];
+    };
+    auto rows_of = [&](int tile, Rows& R) {
+      const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BLOCK_N;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const RowOut ro = row_out(p, mt, n0, 32 * q + lane);
+        R.out[q] = ro.out;
+        R.res[q] = ro.res;
+      }
+    };
+    auto chunk = [&](int h, int w, int j) { return uint32_t((h * BLOCK_N / 8 + j) * 64 + w * 8 + r); };  // 16-byte index
+    auto src_lane = [&](int h, int w) { return (w & 1) * 16 + 8 * h + r; };
+    auto stage_bias = [&](int tile) {
+      const int n0 = (tile % p.n_tiles) * BLOCK_N;
+      for (int i = lane; i < BLOCK_N / 4; i += 32)
+        if (n0 + 4 * i < p.cout) cp_async16(smem_u32(sbias + 4 * i), p.bias + n0 + 4 * i);
+    };
+    // With res == out (training dgrad) a tile's residual is read before that tile is written, and tiles are disjoint.
+    // c_out % 32 == 0: a group of 4 chunks is either inside c_out or outside.
+    auto stage_res = [&](int tile, const Rows& R) {
+      const int n0 = (tile % p.n_tiles) * BLOCK_N;
+      if (p.res) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int w = 0; w < 8; ++w) {
+            const auto* res = reinterpret_cast<const __nv_bfloat16*>(
+                __shfl_sync(~0u, reinterpret_cast<unsigned long long>(R.res[2 * (w >> 2) + ((w & 3) >> 1)]), src_lane(h, w)));
+            if (!res) continue;
+#pragma unroll 1
+            for (int jg = 0; jg < BLOCK_N / 32; ++jg)
+              if (n0 + 32 * jg < p.cout) cp_async16(stile_s + 16u * chunk(h, w, 4 * jg + c), res + 8 * (4 * jg + c));
+          }
+      }
+      cp_async_wait_all();
+      mbar_arrive(staged_bar);
+    };
+    auto drain = [&](int tile, const Rows& R) {
+      const int n0 = (tile % p.n_tiles) * BLOCK_N;
+      const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
+      const int reps = p.upsample ? 4 : 1;
+      const uint4* tile16 = reinterpret_cast<const uint4*>(stile);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+          auto* out = reinterpret_cast<__nv_bfloat16*>(
+              __shfl_sync(~0u, reinterpret_cast<unsigned long long>(R.out[2 * (w >> 2) + ((w & 3) >> 1)]), src_lane(h, w)));
+          if (!out) continue;
+#pragma unroll 2
+          for (int jg = 0; jg < BLOCK_N / 32; ++jg) {
+            if (n0 + 32 * jg >= p.cout) break;
+            const int j = 4 * jg + c;
+            const uint4 v = tile16[chunk(h, w, j)];
+            for (int rep = 0; rep < reps; ++rep)
+              *reinterpret_cast<uint4*>(out + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + 8 * j) = v;
+          }
+        }
+    };
+    uint32_t tphase = 0;
+    Rows cur, nxt;
+    if (int(blockIdx.x) < total_tiles) {
+      rows_of(blockIdx.x, cur);
+      stage_bias(blockIdx.x);
+      stage_res(blockIdx.x, cur);
+    }
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      const int next = tile + int(gridDim.x);
+      if (next < total_tiles) rows_of(next, nxt);  // while the consumers run the tile's main loop
+      mbar_wait(done_bar, tphase, p.err, 7);      // the consumers have finished the tile
+      tphase ^= 1u;
+      if (next < total_tiles) stage_bias(next);   // the consumers have read this tile's bias; lands during the drain
+      drain(tile, cur);
+      // each lane overwrites only chunks it has just read into registers, and the consumers wait on `staged` before
+      // they write the next tile
+      if (next < total_tiles) stage_res(next, nxt);
+      cur = nxt;
+    }
   } else {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue (warpgroups 0, 1)
     const int wg = warp >> 2;                             // tile rows [64 wg, 64 wg + 64)
@@ -283,27 +393,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     constexpr uint32_t kDescHi = wgmma_desc_hi(C::kSbo, C::kSwizzleBytes);
     const uint32_t a_base = smem_u32(smem_a) + uint32_t(wg) * 64u * C::kSwizzleBytes;
     const uint32_t b_base = smem_u32(smem_b);
-    uint32_t stage = 0, phase = 0;
+    uint32_t stage = 0, phase = 0, tphase = 0;
     if (bres && int(blockIdx.x) < total_tiles) mbar_wait(bres_bar, 0, p.err, 6);  // resident weights have landed
-    // kResSmem: word (h * BLOCK_N / 8 + j) * 256 + threadIdx.x holds this thread's residual pair j of row m0 + 8 h
-    // (recomputed where it is used: no register is left to keep it through the main loop)
-    auto res_slot = [&]() { return smem_u32(full_bar) + C::kBarBytes + threadIdx.x * 4u; };
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      if (C::kResSmem && p.res) {
-        const uint32_t res_s = res_slot();
-        // Only this thread reads these words back, after its own cp.async.wait_all: no barrier.  The previous tile's reads
-        // of them completed before its stores were issued.  With res == out the residual of a tile is read before that
-        // tile's stores, and tiles are disjoint.
-        const int n0 = (tile % p.n_tiles) * BLOCK_N;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const RowOut ro = row_out(p, tile / p.n_tiles, n0, m0 + 8 * h);
-          if (!ro.res) continue;
-#pragma unroll 4
-          for (int j = 0; j < BLOCK_N / 8; ++j)
-            if (n0 + 8 * j + cq < p.cout) cp_async4(res_s + uint32_t(h * BLOCK_N / 8 + j) * 1024u, ro.res + 8 * j + cq);
-        }
-      }
       float acc[BLOCK_N / 2];
       uint32_t prev = 0;
       for (int it = 0; it < k_iters; ++it) {
@@ -335,58 +427,80 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       wgmma_fence_regs(acc);
       if (lane == 0) mbar_arrive(&empty_bar[prev]);
 
-      // ---- epilogue straight from the accumulator registers
-      const int nt = tile % p.n_tiles, mt = tile / p.n_tiles;
-      const int n0 = nt * BLOCK_N;
-      const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
-      // read from the kernel parameters here rather than kept live through the main loop
+      // ---- epilogue from the accumulator registers (read from the kernel parameters here rather than kept live through
+      // the main loop)
       const bool silu = p.act == Y3_ACT_SILU;
       const float bscale = silu ? 0.5f : 1.0f;
-      const int reps = p.upsample ? 4 : 1;
-      // one row at a time: only that row's three output pointers are live beside the accumulators (N = 256 keeps 128).
-      // The residual may alias the output (training dgrad: res == out), so the compiler keeps every residual load behind
-      // the stores that precede it in program order.  Loading a whole chunk of column pairs (bias and residual) before
-      // the first store of that chunk makes it one trip to memory per chunk instead of one per column pair.  Correct with
-      // res == out: a thread reads exactly the elements it then overwrites, and tiles are disjoint.
-      constexpr int kChunk = C::kResSmem ? 1 : (BLOCK_N / 8 < 16 ? BLOCK_N / 8 : 16);  // column pairs per batch
-      if (C::kResSmem && p.res) cp_async_wait_all();
-      const uint32_t res_s = C::kResSmem ? res_slot() : 0u;
+      if (staged_out) {
+        // Every column pair of every row goes through the tile: the store warp drops halo rows and columns past c_out
+        // (their bias and residual words were never staged).
+        mbar_wait(staged_bar, tphase, p.err, 8);  // the tile's residual and bias have landed
+        tphase ^= 1u;
+        const bool has_res = p.res != nullptr;
+        uint32_t* words = stile + threadIdx.x;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const RowOut ro = row_out(p, mt, n0, m0 + 8 * h);
-        if (!ro.f32 && !ro.out) continue;
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const float2 b = *reinterpret_cast<const float2*>(sbias + 8 * j + cq);
 #pragma unroll
-        for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
-          float2 b[kChunk];
-          uint32_t r[kChunk];
-#pragma unroll
-          for (int jj = 0; jj < kChunk; ++jj) {
-            const int c = 8 * (j0 + jj) + cq;
-            const bool in = p.out_f32 || n0 + c < p.cout;  // c_out % 32 == 0: a column pair is either inside or outside
-            b[jj] = in ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
-            if (C::kResSmem)
-              r[jj] = (in && ro.res) ? lds32(res_s + uint32_t(h * BLOCK_N / 8 + j0 + jj) * 1024u) : 0u;
-            else
-              r[jj] = (in && ro.res) ? __ldcg(reinterpret_cast<const unsigned int*>(ro.res + c)) : 0u;
+          for (int h = 0; h < 2; ++h) {
+            uint32_t& word = words[(h * BLOCK_N / 8 + j) * 256];
+            float x0 = bias_act(acc[4 * j + 2 * h], bscale * b.x, silu);
+            float x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b.y, silu);
+            if (has_res) {
+              const float2 f = unpack_bf16x2(word);
+              x0 += f.x;
+              x1 += f.y;
+            }
+            word = pack_bf16x2(x0, x1);
           }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(done_bar);
+      } else {
+        // N <= 128 tiles and the fp32 Detect heads: straight from the registers, one row at a time, so only that row's
+        // three output pointers are live beside the accumulators.  The residual may alias the output (training dgrad:
+        // res == out), so the compiler keeps every residual load behind the stores that precede it in program order.
+        // Loading a whole chunk of column pairs (bias and residual) before the first store of that chunk makes it one trip
+        // to memory per chunk instead of one per column pair.  Correct with res == out: a thread reads exactly the
+        // elements it then overwrites, and tiles are disjoint.  (N = 256 only comes here for the heads, which have no
+        // residual, and has no registers left for a chunk.)
+        const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BLOCK_N;
+        const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
+        const int reps = p.upsample ? 4 : 1;
+        constexpr int kChunk = C::kStaged ? 1 : (BLOCK_N / 8 < 16 ? BLOCK_N / 8 : 16);  // column pairs per batch
 #pragma unroll
-          for (int jj = 0; jj < kChunk; ++jj) {
-            const int j = j0 + jj;
-            const int c = 8 * j + cq;
-            if (!p.out_f32 && n0 + c >= p.cout) continue;
-            float x0 = bias_act(acc[4 * j + 2 * h], bscale * b[jj].x, silu);
-            float x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b[jj].y, silu);
-            if (ro.f32) {
-              *reinterpret_cast<float2*>(ro.f32 + c) = make_float2(x0, x1);
-            } else {
-              if (ro.res) {
-                const float2 f = unpack_bf16x2(r[jj]);
-                x0 += f.x;
-                x1 += f.y;
+        for (int h = 0; h < 2; ++h) {
+          const RowOut ro = row_out(p, mt, n0, m0 + 8 * h);
+          if (!ro.f32 && !ro.out) continue;
+#pragma unroll
+          for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
+            float2 b[kChunk];
+            uint32_t r[kChunk];
+#pragma unroll
+            for (int jj = 0; jj < kChunk; ++jj) {
+              const int c = 8 * (j0 + jj) + cq;
+              const bool in = p.out_f32 || n0 + c < p.cout;  // c_out % 32 == 0: a column pair is either inside or outside
+              b[jj] = in ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
+              r[jj] = (in && ro.res) ? __ldcg(reinterpret_cast<const unsigned int*>(ro.res + c)) : 0u;
+            }
+#pragma unroll
+            for (int jj = 0; jj < kChunk; ++jj) {
+              const int c = 8 * (j0 + jj) + cq;
+              if (!p.out_f32 && n0 + c >= p.cout) continue;
+              float x0 = bias_act(acc[4 * (j0 + jj) + 2 * h], bscale * b[jj].x, silu);
+              float x1 = bias_act(acc[4 * (j0 + jj) + 2 * h + 1], bscale * b[jj].y, silu);
+              if (ro.f32) {
+                *reinterpret_cast<float2*>(ro.f32 + c) = make_float2(x0, x1);
+              } else {
+                if (ro.res) {
+                  const float2 f = unpack_bf16x2(r[jj]);
+                  x0 += f.x;
+                  x1 += f.y;
+                }
+                const uint32_t v = pack_bf16x2(x0, x1);
+                for (int rep = 0; rep < reps; ++rep)
+                  *reinterpret_cast<uint32_t*>(ro.out + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + c) = v;
               }
-              const uint32_t v = pack_bf16x2(x0, x1);
-              for (int rep = 0; rep < reps; ++rep)
-                *reinterpret_cast<uint32_t*>(ro.out + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + c) = v;
             }
           }
         }
@@ -405,26 +519,20 @@ int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
     attr_set = true;
   }
   ConvTcArgs args = plan.args;
+  const bool out_tile = C::kStaged && args.out_f32 == nullptr;  // as the kernel decides (staged_out)
+  const uint32_t reserve = out_tile ? C::kOutBytes : 0u;
+  const int b_steps = args.taps * args.kblocks;
   args.bres = plan.bres;
-  args.stages = plan.bres ? C::bres_stages(args.taps * args.kblocks) : C::kStages;
-  if (args.stages < 3) {  // not enough ring left beside the resident weights: fall back to streaming them
+  args.stages = plan.bres ? C::bres_stages(b_steps, reserve) : C::ring_stages(reserve);
+  if (args.bres && args.stages < 3) {  // not enough ring left beside the resident weights: fall back to streaming them
     args.bres = 0;
-    args.stages = C::kStages;
-  }
-  if (C::kResSmem && args.res) {  // the residual staging buffer takes its bytes from the ring
-    const int ring = int(kSmemBudget - C::kResBytes) - (args.bres ? int(C::bres_bytes(args.taps * args.kblocks)) : 0);
-    args.stages = ring / int(args.bres ? C::kABytes : C::kStageBytes);
-    if (args.stages > C::kMaxStages) args.stages = C::kMaxStages;
-    if (args.stages < 3) {
-      args.bres = 0;
-      args.stages = int(kSmemBudget - C::kResBytes) / int(C::kStageBytes);
-    }
+    args.stages = C::ring_stages(reserve);
   }
   // the 1 KB alignment of the base comes out of the allocation's slack
   if (args.stages < 2 || args.stages > C::kMaxStages ||
-      C::smem_end(args.stages, args.bres != 0, args.taps * args.kblocks, C::kResSmem && args.res) + 1024u > C::kSmemBytes)
-    return set_error(Y3_ERR_BAD_ARG, "conv_tc: %d ring stages (resident weights %d, residual %d) do not fit %zu bytes of shared memory (N=%d K=%d)",
-                     args.stages, args.bres, args.res != nullptr, C::kSmemBytes, BLOCK_N, BLOCK_K);
+      C::smem_end(args.stages, args.bres != 0, b_steps, out_tile) + 1024u > C::kSmemBytes)
+    return set_error(Y3_ERR_BAD_ARG, "conv_tc: %d ring stages (resident weights %d, output tile %d) do not fit %zu bytes of shared memory (N=%d K=%d)",
+                     args.stages, args.bres, int(out_tile), C::kSmemBytes, BLOCK_N, BLOCK_K);
   // the kernel parks at pdl_wait() after its prologue (y3_common.cuh)
   Y3_CHECK_CUDA(launch_pdl(kern, dim3(plan.grid), dim3(kThreads), C::kSmemBytes, stream, plan.map_a, plan.map_b, args));
   return Y3_OK;
