@@ -39,7 +39,8 @@ int y3_last_error(char* buf, size_t n);
 int y3_device_check(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror definitions:
  * 0 y3_conv_desc, 1 y3_first_desc, 2 y3_pool_desc, 3 y3_detect_level, 4 y3_decode_desc, 5 y3_op, 6 y3_nms_params,
- * 7 y3_loss_desc. */
+ * 7 y3_loss_desc, 8 y3_bn_act_desc, 9 y3_bn_bwd_desc, 10 y3_wgrad_desc, 11 y3_pack_item, 12 y3_letterbox_desc,
+ * 13 y3_amax_desc. */
 int64_t y3_abi_sizeof(int32_t which);
 /* Programmatic dependent launch between consecutive kernels of a stream (on by default; env Y3_PDL=0 or on=0 turns it off).
  * Results are identical either way — only the launch boundaries overlap.  Returns the previous setting.  A tuning switch with
@@ -77,7 +78,16 @@ typedef struct y3_conv_desc {
   int32_t out_f32_ld;    /* >= c_out_pad, multiple of 4 */
   int32_t* err;          /* optional device int32 error word written by the in-kernel watchdog */
   int32_t weight_layout; /* Y3_W_*: how `weight` is packed (0 = tap-major as documented above) */
+  /* FP8 inference (all zero = bf16 as above).  An e4m3 tensor holds code q for the value q * s of its per-tensor scale s. */
+  int32_t in_fmt;        /* Y3_FMT_*: format of `in` and of `weight` (e4m3: c_in % 32 == 0, in_ld % 16 == 0) */
+  int32_t out_fmt;       /* Y3_FMT_*: format of `out` and of `res` (ignored with out_f32); e4m3: out_ld, out_coff,
+                            res_ld, res_coff % 16 == 0 */
+  const float* dq;       /* e4m3 input: fp32 [c_out_pad], dq[n] = s_in * s_w[n]; y = act(acc * dq[n] + bias[n]) */
+  float res_scale;       /* e4m3 output with res: > 0, the residual adds res_scale * r (the residual's own scale) */
+  float out_inv_scale;   /* e4m3 output: stores sat_e4m3(y * out_inv_scale) */
 } y3_conv_desc;
+#define Y3_FMT_BF16 0
+#define Y3_FMT_E4M3 1   /* float8_e4m3fn: max 448, stored round-to-nearest-even with saturation */
 int y3_conv_bn_act_fwd(const y3_conv_desc* d, y3_stream_t stream);
 /* Input gradient of a STRIDE-2 3x3 conv (training; autograd of Conv.forward, models/common.py:71-75) as four parity-class
  * convolutions of the un-stuffed output gradient: `in` = dy, padded NHWC [n, h+2, w+2, in_ld] on the conv's OUTPUT grid (h, w =
@@ -136,6 +146,8 @@ typedef struct y3_pool_desc {
   int32_t n, h, w, c;    /* input size (unpadded), channels (multiple of 8) */
   int32_t ho, wo;
   int32_t k, stride, off, oob_zero;
+  int32_t fmt;           /* Y3_FMT_* of `in` and `out` (0 = bf16); the e4m3 pool is exact and keeps the input's scale;
+                            e4m3: c, ld and coff % 16 == 0.  The training entry points below take bf16 only */
 } y3_pool_desc;
 int y3_maxpool_fwd(const y3_pool_desc* d, y3_stream_t stream);
 /* Training mode (SPP, models/common.py:281-290, under autograd): the forward also records idx[n, ho, wo, c] (uint8) =
@@ -144,6 +156,12 @@ int y3_maxpool_fwd(const y3_pool_desc* d, y3_stream_t stream);
  * descriptor's `in` is dOut (geometry ho x wo), `out` is dIn (geometry h x w); oob_zero windows are not supported. */
 int y3_maxpool_train_fwd(const y3_pool_desc* d, uint8_t* idx, y3_stream_t stream);
 int y3_maxpool_bwd(const y3_pool_desc* d, const uint8_t* idx, int32_t accumulate, y3_stream_t stream);
+
+/* FP8 calibration: amax = max(amax, max |x|) over the n*h*w interior pixels of a padded NHWC slice [coff, coff+c) of
+ * format fmt (Y3_FMT_*), in stored units (e4m3: codes); c, ld and coff % 8 == 0 (bf16) or % 16 == 0 (e4m3).
+ * Order-independent (an atomic max on the float bits): deterministic. */
+int y3_amax_nhwc(const void* x, int32_t fmt, int32_t ld, int32_t coff, int32_t n, int32_t h, int32_t w, int32_t c,
+                 float* amax, y3_stream_t stream);
 
 /* Layout helpers (tests / feeding intermediate tensors): NCHW fp32 <-> padded NHWC bf16 channel slice. */
 int y3_nchw_to_padded_nhwc(const float* src, int32_t n, int32_t c, int32_t h, int32_t w, void* dst, int32_t dst_ld,
@@ -415,12 +433,19 @@ int y3_sgd_step(float* p, const float* g, float* m, float* ema, const uint8_t* g
 #define Y3_OP_CONV 2
 #define Y3_OP_MAXPOOL 3
 #define Y3_OP_DECODE 4
+#define Y3_OP_AMAX 5     /* FP8 calibration: y3_amax_nhwc of one producer's output, right after the producer */
+typedef struct y3_amax_desc {
+  const void* x;
+  int32_t fmt, ld, coff, n, h, w, c;
+  float* amax;
+} y3_amax_desc;
 typedef struct y3_op {
   int32_t kind;          /* Y3_OP_*: selects which member below is read */
   y3_conv_desc conv;
   y3_first_desc first;
   y3_pool_desc pool;
   y3_decode_desc decode;
+  y3_amax_desc amax;
 } y3_op;
 typedef struct y3_model y3_model;
 int y3_model_create(const y3_op* ops, int32_t n_ops, y3_model** out);

@@ -30,6 +30,8 @@ class ConvDesc(C.Structure):
         ("out_f32", C.c_void_p), ("out_f32_ld", C.c_int32),
         ("err", C.c_void_p),
         ("weight_layout", C.c_int32),
+        ("in_fmt", C.c_int32), ("out_fmt", C.c_int32),
+        ("dq", C.c_void_p), ("res_scale", C.c_float), ("out_inv_scale", C.c_float),
     ]
 
 
@@ -41,6 +43,7 @@ class ConvPlanInfo(C.Structure):
 
 
 W_TAPS, W_XPAIR = 0, 1
+FMT_BF16, FMT_E4M3 = 0, 1
 MAX_LEVELS, MAX_ANCHORS = 5, 6
 
 
@@ -68,7 +71,8 @@ class PoolDesc(C.Structure):
                 ("out", C.c_void_p), ("out_ld", C.c_int32), ("out_coff", C.c_int32),
                 ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("c", C.c_int32),
                 ("ho", C.c_int32), ("wo", C.c_int32),
-                ("k", C.c_int32), ("stride", C.c_int32), ("off", C.c_int32), ("oob_zero", C.c_int32)]
+                ("k", C.c_int32), ("stride", C.c_int32), ("off", C.c_int32), ("oob_zero", C.c_int32),
+                ("fmt", C.c_int32)]
 
 
 class DecodeDesc(C.Structure):
@@ -78,15 +82,22 @@ class DecodeDesc(C.Structure):
                 ("no", C.c_int32), ("z", C.c_void_p)]
 
 
-OP_CONV_FIRST, OP_CONV, OP_MAXPOOL, OP_DECODE = 1, 2, 3, 4
+OP_CONV_FIRST, OP_CONV, OP_MAXPOOL, OP_DECODE, OP_AMAX = 1, 2, 3, 4, 5
 IN_F32, IN_U8 = 0, 1
+
+
+class AmaxDesc(C.Structure):
+    """struct y3_amax_desc."""
+
+    _fields_ = [("x", C.c_void_p), ("fmt", C.c_int32), ("ld", C.c_int32), ("coff", C.c_int32),
+                ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("c", C.c_int32), ("amax", C.c_void_p)]
 
 
 class Op(C.Structure):
     """struct y3_op."""
 
     _fields_ = [("kind", C.c_int32), ("conv", ConvDesc), ("first", FirstDesc), ("pool", PoolDesc),
-                ("decode", DecodeDesc)]
+                ("decode", DecodeDesc), ("amax", AmaxDesc)]
 
 
 class NmsParams(C.Structure):
@@ -180,6 +191,7 @@ def _declare(lib):
         "y3_set_bn_async": ([i32], C.c_int),
         "y3_conv_first_fwd": ([C.POINTER(FirstDesc), vp], C.c_int),
         "y3_maxpool_fwd": ([C.POINTER(PoolDesc), vp], C.c_int),
+        "y3_amax_nhwc": ([vp, i32, i32, i32, i32, i32, i32, i32, vp, vp], C.c_int),
         "y3_maxpool_train_fwd": ([C.POINTER(PoolDesc), vp, vp], C.c_int),
         "y3_maxpool_bwd": ([C.POINTER(PoolDesc), vp, i32, vp], C.c_int),
         "y3_bn_partial_blocks": ([i32, i32, i32, i32], i32),
@@ -244,7 +256,7 @@ def lib():
         _lib = C.CDLL(str(_LIB_PATH))
         SYMBOLS.update(_declare(_lib))
         for which, st in enumerate((ConvDesc, FirstDesc, PoolDesc, DetectLevel, DecodeDesc, Op, NmsParams, LossDesc, BnActDesc,
-                                    BnBwdDesc, WgradDesc, PackItem, LetterboxDesc)):
+                                    BnBwdDesc, WgradDesc, PackItem, LetterboxDesc, AmaxDesc)):
             if _lib.y3_abi_sizeof(which) != C.sizeof(st):
                 raise Y3Error(f"ABI mismatch: sizeof({st.__name__}) is {C.sizeof(st)} here, "
                               f"{_lib.y3_abi_sizeof(which)} in {_LIB_PATH.name}; rebuild the library")

@@ -21,8 +21,14 @@
 //   3. drain: the store warp waits on `done` and writes the tile out with 16-byte stores (halo and out-of-range rows
 //      skipped, concat offset, nearest-2x upsample), then stages the next tile into the same buffer.
 // The fp32 Detect-head launches (a 128 x 256 fp32 tile does not fit beside the ring) and the N <= 128 launches (Cfg::kStaged)
-// store straight from the consumers' registers.  While the consumers finish a tile the producer already fills the ring for
-// their next one.
+// store straight from the consumers' registers.  While the consumers finish a tile the producer
+// already fills the ring for their next one.
+// FP8 (IN_FMT / OUT_FMT = Y3_FMT_E4M3): an e4m3 k-block of 2 * BLOCK_K channels has the byte geometry of a bf16 k-block of
+// BLOCK_K channels (same swizzled rows, descriptors and halo offsets) and one k32 e4m3 wgmma consumes the 32 bytes of one
+// k16 bf16 step, so ring, halo / patch modes and the producer's addressing are shared; BLOCK_K counts bf16-equivalent
+// columns (half a row's bytes).  The epilogue dequantises with dq[n] = s_in * s_w[n] and stores sat_e4m3(y / s_out).  The
+// N = 256 e4m3-output launches keep the store warp: their tile is 128 x 256 bytes in channel order (16-byte chunks of 16
+// channels), the residual is staged as e4m3, and an e4m3 input stages its dq floats beside the bias.
 #include <cuda_bf16.h>
 
 #include <cstdlib>
@@ -48,7 +54,9 @@ constexpr int kSmemBudget = 221 * 1024;  // ring (+ resident weights); alignment
 // start address is not aligned to the swizzle pattern (the swizzle is a function of the absolute shared-memory address,
 // so the descriptor's base offset stays 0).  A rows fetched per k-block drop from 9*128 to 3*130 and the producer runs a
 // third of the pipeline stages.
-template <int BLOCK_N, int BLOCK_K, bool HALO>
+// STAGE_ES: bytes per element of the staged output tile (2 bf16, 1 e4m3; 0: never staged, the fp32-only head instances).
+// STAGE_DQ: an e4m3 input, whose BLOCK_N dq floats are staged beside the bias.
+template <int BLOCK_N, int BLOCK_K, bool HALO, int STAGE_ES = 2, bool STAGE_DQ = false>
 struct Cfg {
   static constexpr uint32_t kARows = HALO ? kBlockM + 2 : kBlockM;
   static constexpr uint32_t kATxBytes = kARows * BLOCK_K * 2;                         // bytes one A box delivers (flat mode)
@@ -61,9 +69,9 @@ struct Cfg {
   // and the tile's BLOCK_N bias floats beside the ring, and those bytes come out of the ring's budget (`reserve`).
   // Thinner tiles run only a few microseconds each: one warp cannot drain and restage them in that time, and their
   // epilogue from the registers (batched bias and residual loads) costs less than the store warp's turn-around.
-  static constexpr bool kStaged = BLOCK_N == 256;
-  static constexpr uint32_t kTileBytes = kBlockM * BLOCK_N * 2;
-  static constexpr uint32_t kOutBytes = kTileBytes + BLOCK_N * 4;
+  static constexpr bool kStaged = BLOCK_N == 256 && STAGE_ES > 0;
+  static constexpr uint32_t kTileBytes = kBlockM * BLOCK_N * (STAGE_ES > 0 ? STAGE_ES : 2);
+  static constexpr uint32_t kOutBytes = kTileBytes + BLOCK_N * 4 * (STAGE_DQ ? 2 : 1);
   __host__ __device__ static constexpr int ring_stages(uint32_t reserve) {
     const int s = int(kSmemBudget - reserve) / int(kStageBytes);
     return s > kMaxStages ? kMaxStages : s;
@@ -101,6 +109,15 @@ __device__ __forceinline__ float bias_act(float a, float b, bool silu) {
   return fmaf(h, t, h);
 }
 
+// FP8 form: y = act(acc * dq + b).  `s`, `b` hold dq/2, b/2 for SiLU layers (one FFMA, as above).
+__device__ __forceinline__ float bias_act_dq(float a, float s, float b, bool silu) {
+  const float h = fmaf(a, s, b);
+  if (!silu) return h;
+  float t;
+  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
+  return fmaf(h, t, h);
+}
+
 __device__ __forceinline__ void cp_async16(uint32_t saddr, const void* gptr) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(gptr) : "memory");
 }
@@ -119,6 +136,14 @@ struct RowOut {
   const __nv_bfloat16* res; // residual
 };
 
+// element offset -> pointer for elements of ES bytes (ES = 1: e4m3 behind the same pointer types)
+template <int ES, typename T>
+__device__ __forceinline__ T* elem_ptr(T* p, long long off) {
+  if (ES == 2) return p + off;
+  return reinterpret_cast<T*>(reinterpret_cast<uintptr_t>(p) + off * ES);
+}
+
+template <int ES = 2>
 __device__ __forceinline__ RowOut row_out(const ConvTcArgs& p, int mt, int n0, int m) {
   RowOut o{nullptr, nullptr, nullptr};
   bool valid;
@@ -147,22 +172,26 @@ __device__ __forceinline__ RowOut row_out(const ConvTcArgs& p, int mt, int n0, i
   long long conv_row = (static_cast<long long>(img) * (oh + 2) + oy + 1) * (ow + 2) + ox + 1;
   if (p.phase)  // one parity class of a transposed stride-2 conv: (oy, ox) -> (2 oy + a, 2 ox + b) of the 2x grid
     conv_row = (static_cast<long long>(img) * (2 * oh + 2) + 2 * oy + p.ph_a + 1) * (2 * ow + 2) + 2 * ox + p.ph_b + 1;
-  if (p.res) o.res = p.res + conv_row * p.res_ld + p.res_coff + n0;
+  if (p.res) o.res = elem_ptr<ES>(p.res, conv_row * p.res_ld + p.res_coff + n0);
   if (p.out_f32) {
     o.f32 = p.out_f32 + ((static_cast<long long>(img) * oh + oy) * ow + ox) * p.out_f32_ld + n0;
   } else if (p.upsample) {
     const long long r00 = (static_cast<long long>(img) * (2 * oh + 2) + 2 * oy + 1) * (2 * ow + 2) + 2 * ox + 1;
-    o.out = p.out + r00 * p.out_ld + p.out_coff + n0;
+    o.out = elem_ptr<ES>(p.out, r00 * p.out_ld + p.out_coff + n0);
   } else {
-    o.out = p.out + conv_row * p.out_ld + p.out_coff + n0;
+    o.out = elem_ptr<ES>(p.out, conv_row * p.out_ld + p.out_coff + n0);
   }
   return o;
 }
 
-template <int BLOCK_N, int BLOCK_K, bool HALO>
+template <int BLOCK_N, int BLOCK_K, bool HALO, int IN_FMT = Y3_FMT_BF16, int OUT_FMT = Y3_FMT_BF16>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const ConvTcArgs p) {
-  using C = Cfg<BLOCK_N, BLOCK_K, HALO>;
+  constexpr bool kInE4m3 = IN_FMT == Y3_FMT_E4M3, kOutE4m3 = OUT_FMT == Y3_FMT_E4M3;
+  using C = Cfg<BLOCK_N, BLOCK_K, HALO, kOutE4m3 ? 1 : (kInE4m3 ? 0 : 2), kInE4m3 && kOutE4m3>;
+  constexpr int kOes = kOutE4m3 ? 1 : 2;  // bytes per output / residual element
+  constexpr int kKch = kInE4m3 ? 2 * BLOCK_K : BLOCK_K;  // input channels per k-block
+  using Mma = std::conditional_t<kInE4m3, WgmmaE4m3<BLOCK_N>, Wgmma<BLOCK_N>>;
   const int STAGES = p.stages;
   const bool bres = p.bres != 0;
   constexpr uint32_t kBStage = C::kTaps * C::kBBytes;  // B bytes per stage (ring mode)
@@ -184,6 +213,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   // one row of warp w
   uint32_t* stile = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(full_bar) + C::kBarBytes);
   float* sbias = reinterpret_cast<float*>(stile + C::kTileBytes / 4);
+  float* sdq = sbias + BLOCK_N;  // e4m3 input (Cfg STAGE_DQ)
   const bool staged_out = C::kStaged && p.out_f32 == nullptr;
 
   const int warp = threadIdx.x >> 5;
@@ -220,7 +250,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       mbar_expect_tx(bres_bar, uint32_t(b_steps) * C::kBBytes);
       for (int st = 0; st < b_steps; ++st) {
         const int kb = st / p.taps, tap = st - kb * p.taps;
-        tma_load_2d(smem_b + st * C::kBBytes, &map_b, bres_bar, (p.custom_taps ? p.tap_wcol[tap] : tap) * p.cin + kb * BLOCK_K, 0);
+        tma_load_2d(smem_b + st * C::kBBytes, &map_b, bres_bar, (p.custom_taps ? p.tap_wcol[tap] : tap) * p.cin + kb * kKch, 0);
       }
     }
     __syncwarp();
@@ -253,7 +283,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
           if (elect_one()) {
             uint8_t* a_dst = smem_a + stage * C::kABytes;
             uint8_t* b_dst = smem_b + stage * kBStage;
-            const int kcol = kb * BLOCK_K;
+            const int kcol = kb * kKch;
             // flat mode: the tap's A box is the tile's pixel rows shifted by (r-1)*wp + (s-1) (HALO: a whole filter row)
             const int shift = HALO ? (tap - 1) * wp - 1 : (custom ? p.tap_shift[tap] : (nine ? (r - 1) * wp + (s - 1) : 0));
             // patch mode: filter row r, column s.  x-paired weights (stride 2, in_ld == c_in): one box covers the two
@@ -312,17 +342,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BLOCK_N;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const RowOut ro = row_out(p, mt, n0, 32 * q + lane);
+        const RowOut ro = row_out<kOes>(p, mt, n0, 32 * q + lane);
         R.out[q] = ro.out;
         R.res[q] = ro.res;
       }
     };
-    auto chunk = [&](int h, int w, int j) { return uint32_t((h * BLOCK_N / 8 + j) * 64 + w * 8 + r); };  // 16-byte index
+    // 16-byte chunk j of a row: channels [kCh j, kCh j + kCh)
+    constexpr int kCh = 16 / kOes, kRowChunks = BLOCK_N / kCh;
+    auto chunk = [&](int h, int w, int j) { return uint32_t((h * kRowChunks + j) * 64 + w * 8 + r); };  // 16-byte index
     auto src_lane = [&](int h, int w) { return (w & 1) * 16 + 8 * h + r; };
     auto stage_bias = [&](int tile) {
       const int n0 = (tile % p.n_tiles) * BLOCK_N;
       for (int i = lane; i < BLOCK_N / 4; i += 32)
-        if (n0 + 4 * i < p.cout) cp_async16(smem_u32(sbias + 4 * i), p.bias + n0 + 4 * i);
+        if (n0 + 4 * i < p.cout) {
+          cp_async16(smem_u32(sbias + 4 * i), p.bias + n0 + 4 * i);
+          if (kInE4m3) cp_async16(smem_u32(sdq + 4 * i), p.dq + n0 + 4 * i);
+        }
     };
     // With res == out (training dgrad) a tile's residual is read before that tile is written, and tiles are disjoint.
     // c_out % 32 == 0: a group of 4 chunks is either inside c_out or outside.
@@ -337,8 +372,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
                 __shfl_sync(~0u, reinterpret_cast<unsigned long long>(R.res[2 * (w >> 2) + ((w & 3) >> 1)]), src_lane(h, w)));
             if (!res) continue;
 #pragma unroll 1
-            for (int jg = 0; jg < BLOCK_N / 32; ++jg)
-              if (n0 + 32 * jg < p.cout) cp_async16(stile_s + 16u * chunk(h, w, 4 * jg + c), res + 8 * (4 * jg + c));
+            for (int jg = 0; jg < kRowChunks / 4; ++jg) {
+              const int j = 4 * jg + c;
+              // bf16: a group of 4 chunks (32 channels) is inside c_out or outside; e4m3: each chunk of 16 is
+              if (kOutE4m3 ? n0 + kCh * j < p.cout : n0 + 32 * jg < p.cout)
+                cp_async16(stile_s + 16u * chunk(h, w, j), elem_ptr<kOes>(res, kCh * j));
+            }
           }
       }
       cp_async_wait_all();
@@ -357,12 +396,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
               __shfl_sync(~0u, reinterpret_cast<unsigned long long>(R.out[2 * (w >> 2) + ((w & 3) >> 1)]), src_lane(h, w)));
           if (!out) continue;
 #pragma unroll 2
-          for (int jg = 0; jg < BLOCK_N / 32; ++jg) {
-            if (n0 + 32 * jg >= p.cout) break;
+          for (int jg = 0; jg < kRowChunks / 4; ++jg) {
             const int j = 4 * jg + c;
+            if (kOutE4m3 ? n0 + kCh * j >= p.cout : n0 + 32 * jg >= p.cout) break;
             const uint4 v = tile16[chunk(h, w, j)];
             for (int rep = 0; rep < reps; ++rep)
-              *reinterpret_cast<uint4*>(out + (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + 8 * j) = v;
+              *reinterpret_cast<uint4*>(elem_ptr<kOes>(out, (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + kCh * j)) = v;
           }
         }
     };
@@ -410,7 +449,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             // HALO: tap t reads the A box shifted by t pixel rows (start address off the swizzle pattern)
             const uint64_t adesc = wgmma_desc(kDescHi, a_st + t * C::kSwizzleBytes + k * 32);
             const uint64_t bdesc = wgmma_desc(kDescHi, b_st + t * C::kBBytes + k * 32);
-            Wgmma<BLOCK_N>::template mma<0, 0>(acc, adesc, bdesc, (it != 0 || t != 0 || k != 0) ? 1u : 0u);
+            Mma::template mma<0, 0>(acc, adesc, bdesc, (it != 0 || t != 0 || k != 0) ? 1u : 0u);
           }
         }
         wgmma_commit();
@@ -437,6 +476,38 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         mbar_wait(staged_bar, tphase, p.err, 8);  // the tile's residual and bias have landed
         tphase ^= 1u;
         const bool has_res = p.res != nullptr;
+        if constexpr (kOutE4m3) {
+          // this thread's column pair j of row m0 + 8 h: bytes (j & 1) * 8 + cq of 16-byte chunk j / 2 of that row (the
+          // residual pair before, the output pair after; channel order, as the store warp copies it)
+          uint8_t* tb = reinterpret_cast<uint8_t*>(stile) + ((warp * 8 + (lane >> 2)) * 16 + cq);
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const float2 b = *reinterpret_cast<const float2*>(sbias + 8 * j + cq);
+            float2 q = b;
+            if (kInE4m3) q = *reinterpret_cast<const float2*>(sdq + 8 * j + cq);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              uint16_t& hw = *reinterpret_cast<uint16_t*>(tb + (h * BLOCK_N / 16 + j / 2) * 64 * 16 + (j & 1) * 8);
+              float x0, x1;
+              if (kInE4m3) {
+                x0 = bias_act_dq(acc[4 * j + 2 * h], bscale * q.x, bscale * b.x, silu);
+                x1 = bias_act_dq(acc[4 * j + 2 * h + 1], bscale * q.y, bscale * b.y, silu);
+              } else {
+                x0 = bias_act(acc[4 * j + 2 * h], bscale * b.x, silu);
+                x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b.y, silu);
+              }
+              if (has_res) {
+                const float2 f = unpack_e4m3x2(hw);
+                x0 = fmaf(p.res_scale, f.x, x0);
+                x1 = fmaf(p.res_scale, f.y, x1);
+              }
+              hw = pack_e4m3x2(x0 * p.out_inv_scale, x1 * p.out_inv_scale);
+            }
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(done_bar);
+          continue;
+        }
         uint32_t* words = stile + threadIdx.x;
 #pragma unroll
         for (int j = 0; j < BLOCK_N / 8; ++j) {
@@ -457,40 +528,60 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         __syncwarp();
         if (lane == 0) mbar_arrive(done_bar);
       } else {
-        // N <= 128 tiles and the fp32 Detect heads: straight from the registers, one row at a time, so only that row's
+        // N <= 128 tiles, the fp32 Detect heads and the FP8 launches: straight from the registers, one row at a time, so only that row's
         // three output pointers are live beside the accumulators.  The residual may alias the output (training dgrad:
         // res == out), so the compiler keeps every residual load behind the stores that precede it in program order.
         // Loading a whole chunk of column pairs (bias and residual) before the first store of that chunk makes it one trip
         // to memory per chunk instead of one per column pair.  Correct with res == out: a thread reads exactly the
-        // elements it then overwrites, and tiles are disjoint.  (N = 256 only comes here for the heads, which have no
+        // elements it then overwrites, and tiles are disjoint.  (N = 256 only comes here for the fp32 heads, which have no
         // residual, and has no registers left for a chunk.)
         const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BLOCK_N;
         const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
         const int reps = p.upsample ? 4 : 1;
-        constexpr int kChunk = C::kStaged ? 1 : (BLOCK_N / 8 < 16 ? BLOCK_N / 8 : 16);  // column pairs per batch
+        // column pairs per batch (an e4m3 input also holds the batch's dq pairs: half the batch at N = 128 keeps 0 spills)
+        constexpr int kChunk = BLOCK_N == 256 ? 1 : (kInE4m3 && BLOCK_N == 128 ? 8 : (BLOCK_N / 8 < 16 ? BLOCK_N / 8 : 16));
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const RowOut ro = row_out(p, mt, n0, m0 + 8 * h);
+          const RowOut ro = row_out<kOes>(p, mt, n0, m0 + 8 * h);
           if (!ro.f32 && !ro.out) continue;
 #pragma unroll
           for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
-            float2 b[kChunk];
+            float2 b[kChunk], q[kChunk];
             uint32_t r[kChunk];
 #pragma unroll
             for (int jj = 0; jj < kChunk; ++jj) {
               const int c = 8 * (j0 + jj) + cq;
               const bool in = p.out_f32 || n0 + c < p.cout;  // c_out % 32 == 0: a column pair is either inside or outside
               b[jj] = in ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
-              r[jj] = (in && ro.res) ? __ldcg(reinterpret_cast<const unsigned int*>(ro.res + c)) : 0u;
+              if (kInE4m3) q[jj] = in ? __ldg(reinterpret_cast<const float2*>(p.dq + n0 + c)) : make_float2(0.f, 0.f);
+              if (kOutE4m3)
+                r[jj] = (in && ro.res) ? __ldcg(reinterpret_cast<const unsigned short*>(elem_ptr<1>(ro.res, c))) : 0u;
+              else
+                r[jj] = (in && ro.res) ? __ldcg(reinterpret_cast<const unsigned int*>(ro.res + c)) : 0u;
             }
 #pragma unroll
             for (int jj = 0; jj < kChunk; ++jj) {
               const int c = 8 * (j0 + jj) + cq;
               if (!p.out_f32 && n0 + c >= p.cout) continue;
-              float x0 = bias_act(acc[4 * (j0 + jj) + 2 * h], bscale * b[jj].x, silu);
-              float x1 = bias_act(acc[4 * (j0 + jj) + 2 * h + 1], bscale * b[jj].y, silu);
+              float x0, x1;
+              if (kInE4m3) {
+                x0 = bias_act_dq(acc[4 * (j0 + jj) + 2 * h], bscale * q[jj].x, bscale * b[jj].x, silu);
+                x1 = bias_act_dq(acc[4 * (j0 + jj) + 2 * h + 1], bscale * q[jj].y, bscale * b[jj].y, silu);
+              } else {
+                x0 = bias_act(acc[4 * (j0 + jj) + 2 * h], bscale * b[jj].x, silu);
+                x1 = bias_act(acc[4 * (j0 + jj) + 2 * h + 1], bscale * b[jj].y, silu);
+              }
               if (ro.f32) {
                 *reinterpret_cast<float2*>(ro.f32 + c) = make_float2(x0, x1);
+              } else if (kOutE4m3) {
+                if (ro.res) {
+                  const float2 f = unpack_e4m3x2(static_cast<uint16_t>(r[jj]));
+                  x0 = fmaf(p.res_scale, f.x, x0);
+                  x1 = fmaf(p.res_scale, f.y, x1);
+                }
+                const uint16_t v = pack_e4m3x2(x0 * p.out_inv_scale, x1 * p.out_inv_scale);
+                for (int rep = 0; rep < reps; ++rep)
+                  *reinterpret_cast<uint16_t*>(elem_ptr<1>(ro.out, (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + c)) = v;
               } else {
                 if (ro.res) {
                   const float2 f = unpack_bf16x2(r[jj]);
@@ -509,10 +600,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   }
 }
 
-template <int BLOCK_N, int BLOCK_K, bool HALO = false>
+template <int BLOCK_N, int BLOCK_K, bool HALO = false, int IN_FMT = Y3_FMT_BF16, int OUT_FMT = Y3_FMT_BF16>
 int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
-  using C = Cfg<BLOCK_N, BLOCK_K, HALO>;
-  auto kern = conv_tc_kernel<BLOCK_N, BLOCK_K, HALO>;
+  constexpr bool kInE4m3 = IN_FMT == Y3_FMT_E4M3, kOutE4m3 = OUT_FMT == Y3_FMT_E4M3;
+  using C = Cfg<BLOCK_N, BLOCK_K, HALO, kOutE4m3 ? 1 : (kInE4m3 ? 0 : 2), kInE4m3 && kOutE4m3>;  // as conv_tc_kernel
+  auto kern = conv_tc_kernel<BLOCK_N, BLOCK_K, HALO, IN_FMT, OUT_FMT>;
   static bool attr_set = false;  // benign race: idempotent attribute
   if (!attr_set) {
     Y3_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, int(C::kSmemBytes)));
@@ -540,26 +632,30 @@ int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
 
 int pick_block_n(int cout) { return cout <= 32 ? 32 : (cout <= 64 ? 64 : (cout <= 128 ? 128 : 256)); }
 
-}  // namespace
-
-int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream) {
-#define Y3_DISPATCH_K(BN)                                              \
-  switch (plan.block_k) {                                              \
-    case 64: return launch_cfg<BN, 64>(plan, stream);                  \
-    case 32: return launch_cfg<BN, 32>(plan, stream);                  \
-    case 16: return launch_cfg<BN, 16>(plan, stream);                  \
-  }                                                                    \
+template <int IN_FMT, int OUT_FMT>
+int launch_fmt(const ConvTcPlan& plan, cudaStream_t stream) {
+#define Y3_DISPATCH_K(BN)                                                        \
+  switch (plan.block_k) {                                                        \
+    case 64: return launch_cfg<BN, 64, false, IN_FMT, OUT_FMT>(plan, stream);    \
+    case 32: return launch_cfg<BN, 32, false, IN_FMT, OUT_FMT>(plan, stream);    \
+    case 16: return launch_cfg<BN, 16, false, IN_FMT, OUT_FMT>(plan, stream);    \
+  }                                                                              \
   break;
+  // e4m3 in, fp32 out: only the Detect heads (1x1, never halo)
+  constexpr bool kHalo = !(IN_FMT == Y3_FMT_E4M3 && OUT_FMT == Y3_FMT_BF16);
   if (plan.halo) {  // stride-1 3x3: K = 64 with N <= 128, K = 32 (c_in = 32 layers, 64-byte rows) with N <= 64
-    if (plan.block_k == 64) {
-      if (plan.block_n == 128) return launch_cfg<128, 64, true>(plan, stream);
-      if (plan.block_n == 64) return launch_cfg<64, 64, true>(plan, stream);
-      if (plan.block_n == 32) return launch_cfg<32, 64, true>(plan, stream);
-    } else if (plan.block_k == 32) {
-      if (plan.block_n == 64) return launch_cfg<64, 32, true>(plan, stream);
-      if (plan.block_n == 32) return launch_cfg<32, 32, true>(plan, stream);
+    if constexpr (kHalo) {
+      if (plan.block_k == 64) {
+        if (plan.block_n == 128) return launch_cfg<128, 64, true, IN_FMT, OUT_FMT>(plan, stream);
+        if (plan.block_n == 64) return launch_cfg<64, 64, true, IN_FMT, OUT_FMT>(plan, stream);
+        if (plan.block_n == 32) return launch_cfg<32, 64, true, IN_FMT, OUT_FMT>(plan, stream);
+      } else if (plan.block_k == 32) {
+        if (plan.block_n == 64) return launch_cfg<64, 32, true, IN_FMT, OUT_FMT>(plan, stream);
+        if (plan.block_n == 32) return launch_cfg<32, 32, true, IN_FMT, OUT_FMT>(plan, stream);
+      }
     }
-    return set_error(Y3_ERR_BAD_ARG, "conv_tc: no halo kernel for tile N=%d K=%d", plan.block_n, plan.block_k);
+    return set_error(Y3_ERR_BAD_ARG, "conv_tc: no halo kernel for tile N=%d K=%d (formats %d -> %d)", plan.block_n,
+                     plan.block_k, IN_FMT, OUT_FMT);
   }
   switch (plan.block_n) {
     case 32: Y3_DISPATCH_K(32)
@@ -569,6 +665,18 @@ int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream) {
   }
 #undef Y3_DISPATCH_K
   return set_error(Y3_ERR_BAD_ARG, "conv_tc: no kernel for tile N=%d K=%d", plan.block_n, plan.block_k);
+}
+
+}  // namespace
+
+// Instances: bf16 -> bf16 (training and the default inference), and for FP8 inference bf16 -> e4m3 (the first tensor-core
+// conv), e4m3 -> e4m3, and e4m3 -> fp32 (Detect heads).  conv_tc_prepare rejects every other combination.
+int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream) {
+  if (plan.in_fmt == Y3_FMT_BF16 && plan.out_fmt == Y3_FMT_BF16) return launch_fmt<Y3_FMT_BF16, Y3_FMT_BF16>(plan, stream);
+  if (plan.in_fmt == Y3_FMT_BF16 && plan.out_fmt == Y3_FMT_E4M3) return launch_fmt<Y3_FMT_BF16, Y3_FMT_E4M3>(plan, stream);
+  if (plan.in_fmt == Y3_FMT_E4M3 && plan.out_fmt == Y3_FMT_E4M3) return launch_fmt<Y3_FMT_E4M3, Y3_FMT_E4M3>(plan, stream);
+  if (plan.in_fmt == Y3_FMT_E4M3 && plan.out_fmt == Y3_FMT_BF16) return launch_fmt<Y3_FMT_E4M3, Y3_FMT_BF16>(plan, stream);
+  return set_error(Y3_ERR_BAD_ARG, "conv_tc: formats %d -> %d", plan.in_fmt, plan.out_fmt);
 }
 
 // Y3_CONV_HALO=0 disables the halo-reuse A path (A/B measurements).
@@ -608,7 +716,7 @@ static void fast_div_for(uint32_t d, uint32_t* mul, uint32_t* shr) {
 }
 
 static bool conv_prefers_xpair(const y3_conv_desc& d) {
-  return d.ksize == 3 && d.stride == 2 && (d.c_in == 32 || d.c_in == 16) && d.in_ld == d.c_in && d.in_coff == 0;
+  return d.in_fmt == Y3_FMT_BF16 && d.ksize == 3 && d.stride == 2 && (d.c_in == 32 || d.c_in == 16) && d.in_ld == d.c_in && d.in_coff == 0;
 }
 
 // select_only: tile / mode selection without encoding the tensor maps (y3_conv_plan: host-side tests of the heuristics)
@@ -623,7 +731,28 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
                  (reinterpret_cast<uintptr_t>(d.bias) & 15) == 0,
              "conv: pointers must be 16-byte aligned");
   const bool head = d.out_f32 != nullptr;
+  Y3_REQUIRE((d.in_fmt == Y3_FMT_BF16 || d.in_fmt == Y3_FMT_E4M3) && (d.out_fmt == Y3_FMT_BF16 || d.out_fmt == Y3_FMT_E4M3),
+             "conv: unknown format %d -> %d", d.in_fmt, d.out_fmt);
+  const bool in8 = d.in_fmt == Y3_FMT_E4M3, out8 = !head && d.out_fmt == Y3_FMT_E4M3;
+  const int es = in8 ? 1 : 2;  // input / weight element bytes
+  if (in8) {
+    Y3_REQUIRE(d.c_in % 32 == 0, "conv: an e4m3 input needs c_in %% 32 == 0 (c_in=%d)", d.c_in);
+    Y3_REQUIRE(d.in_ld % 16 == 0, "conv: an e4m3 input needs in_ld %% 16 == 0 (in_ld=%d)", d.in_ld);
+    Y3_REQUIRE(d.dq && (reinterpret_cast<uintptr_t>(d.dq) & 15) == 0, "conv: an e4m3 input needs 16-byte aligned dq");
+    Y3_REQUIRE(head || out8, "conv: an e4m3 input writes e4m3 or the fp32 head output");
+    Y3_REQUIRE(!extra, "conv: the transposed (dgrad) form is bf16 only");
+  }
+  if (out8) {
+    Y3_REQUIRE(d.out_inv_scale > 0.f, "conv: an e4m3 output needs out_inv_scale > 0");
+    // the N = 256 store warp moves 16-byte chunks of 16 e4m3 channels (output and staged residual)
+    Y3_REQUIRE(d.out_ld % 16 == 0 && d.out_coff % 16 == 0, "conv: an e4m3 output needs out_ld and out_coff %% 16 == 0");
+    if (d.res)
+      Y3_REQUIRE(d.res_ld % 16 == 0 && d.res_coff % 16 == 0 && d.res_scale > 0.f,
+                 "conv: an e4m3 residual needs res_ld and res_coff %% 16 == 0 and res_scale > 0");
+    Y3_REQUIRE(!extra, "conv: the transposed (dgrad) form is bf16 only");
+  }
   if (head) {
+    Y3_REQUIRE(d.out_fmt == Y3_FMT_BF16, "conv: out_fmt must be 0 with the fp32 output");
     Y3_REQUIRE(d.stride == 1 && !d.upsample && !d.res, "conv: fp32 output supports plain stride-1 convs only");
     Y3_REQUIRE(d.out_f32_ld % 4 == 0 && (reinterpret_cast<uintptr_t>(d.out_f32) & 15) == 0, "conv: bad fp32 output");
   } else {
@@ -643,7 +772,10 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
   const int bn = pick_block_n(d.c_out);
   // x-paired: the GEMM sees 3 x 2 taps of 2*c_in channels (the phantom 4th column carries zero weights)
   const int gemm_cin = xpair ? 2 * d.c_in : d.c_in;
-  const int bk = gemm_cin % 64 == 0 ? 64 : (gemm_cin % 32 == 0 ? 32 : 16);
+  // bk: half a k-block row's bytes (bf16: channels; e4m3: half the channels)
+  const int row2 = gemm_cin * es / 2;
+  const int bk = row2 % 64 == 0 ? 64 : (row2 % 32 == 0 ? 32 : 16);
+  const int kch = bk * 2 / es;  // channels per k-block
   const int cout_pad = (d.c_out + bn - 1) / bn * bn;
   const int taps = extra ? extra->ntaps : (xpair ? 6 : d.ksize * d.ksize);
   const int hp = d.h + 2, wp = d.w + 2;
@@ -651,10 +783,12 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
 
   ConvTcArgs& a = plan->args;
   a = ConvTcArgs{};
+  plan->in_fmt = d.in_fmt;
+  plan->out_fmt = out8 ? Y3_FMT_E4M3 : Y3_FMT_BF16;
   plan->block_n = bn;
   plan->block_k = bk;
   a.taps = taps;
-  a.kblocks = gemm_cin / bk;
+  a.kblocks = gemm_cin / kch;
   a.cin = gemm_cin;
   a.xpair = xpair ? 1 : 0;
   a.a_coff = d.in_coff;
@@ -673,6 +807,9 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
   a.out_f32 = d.out_f32;
   a.out_f32_ld = d.out_f32_ld;
   a.err = d.err;
+  a.dq = in8 ? d.dq : nullptr;
+  a.res_scale = d.res_scale;
+  a.out_inv_scale = d.out_inv_scale;
   if (head) {
     a.out = nullptr;
     Y3_REQUIRE(d.out_f32_ld >= (d.c_out + pick_block_n(d.c_out) - 1) / pick_block_n(d.c_out) * pick_block_n(d.c_out),
@@ -705,9 +842,9 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     const uint32_t a_rows = plan->halo ? kBlockM + 2 : kBlockM;
     a.a_tx_bytes = a_rows * bk * 2;
     const uint64_t dims[2] = {static_cast<uint64_t>(d.in_ld), static_cast<uint64_t>(rows)};
-    const uint64_t strides[2] = {0, static_cast<uint64_t>(d.in_ld) * 2};
-    const uint32_t box[2] = {static_cast<uint32_t>(bk), a_rows};
-    rc = select_only ? Y3_OK : encode_tensor_map_bf16(&plan->map_a, d.in, 2, dims, strides, box, bk * 2);
+    const uint64_t strides[2] = {0, static_cast<uint64_t>(d.in_ld) * es};
+    const uint32_t box[2] = {static_cast<uint32_t>(kch), a_rows};
+    rc = select_only ? Y3_OK : encode_tensor_map(&plan->map_a, d.in_fmt, d.in, 2, dims, strides, box, bk * 2);
     if (rc) return rc;
   } else {
     plan->halo = 0;
@@ -737,18 +874,18 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     const uint64_t ld = static_cast<uint64_t>(d.in_ld);
     const uint64_t dims[5] = {2 * ld, static_cast<uint64_t>(wp / 2), 2, static_cast<uint64_t>(hp / 2),
                               static_cast<uint64_t>(d.n)};
-    const uint64_t strides[5] = {0, 2 * ld * 2, static_cast<uint64_t>(wp) * ld * 2, 2ull * wp * ld * 2,
-                                 static_cast<uint64_t>(hp) * wp * ld * 2};
-    const uint32_t box[5] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(a.tw), 1, static_cast<uint32_t>(a.th), 1};
-    rc = select_only ? Y3_OK : encode_tensor_map_bf16(&plan->map_a, d.in, 5, dims, strides, box, bk * 2);
+    const uint64_t strides[5] = {0, 2 * ld * es, static_cast<uint64_t>(wp) * ld * es, 2ull * wp * ld * es,
+                                 static_cast<uint64_t>(hp) * wp * ld * es};
+    const uint32_t box[5] = {static_cast<uint32_t>(kch), static_cast<uint32_t>(a.tw), 1, static_cast<uint32_t>(a.th), 1};
+    rc = select_only ? Y3_OK : encode_tensor_map(&plan->map_a, d.in_fmt, d.in, 5, dims, strides, box, bk * 2);
     if (rc) return rc;
   }
   {
     const uint64_t ktot = static_cast<uint64_t>(extra ? d.ksize * d.ksize : taps) * gemm_cin;  // the whole weight matrix
     const uint64_t dims[2] = {ktot, static_cast<uint64_t>(cout_pad)};
-    const uint64_t strides[2] = {0, ktot * 2};
-    const uint32_t box[2] = {static_cast<uint32_t>(bk), static_cast<uint32_t>(bn)};
-    rc = select_only ? Y3_OK : encode_tensor_map_bf16(&plan->map_b, d.weight, 2, dims, strides, box, bk * 2);
+    const uint64_t strides[2] = {0, ktot * es};
+    const uint32_t box[2] = {static_cast<uint32_t>(kch), static_cast<uint32_t>(bn)};
+    rc = select_only ? Y3_OK : encode_tensor_map(&plan->map_b, d.in_fmt, d.weight, 2, dims, strides, box, bk * 2);
     if (rc) return rc;
   }
   {

@@ -26,9 +26,14 @@ int set_error(int code, const char* fmt, ...);
   } while (0)
 
 // ---- TMA descriptor encoding through the driver entry point (no link-time libcuda dependency)
-// dims/strides innermost first; strides in BYTES for dims 1..rank-1; swizzle_bytes in {32,64,128}.
-int encode_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
-                           const uint32_t* box, int swizzle_bytes);
+// fmt: Y3_FMT_* of the elements (coordinates, dims and box count elements); dims/strides innermost first; strides in
+// BYTES for dims 1..rank-1; swizzle_bytes in {32,64,128}.
+int encode_tensor_map(CUtensorMap* out, int fmt, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                      const uint32_t* box, int swizzle_bytes);
+inline int encode_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                                  const uint32_t* box, int swizzle_bytes) {
+  return encode_tensor_map(out, Y3_FMT_BF16, base, rank, dims, strides, box, swizzle_bytes);
+}
 
 int num_sms();
 int pdl_enabled();   // programmatic dependent launch on (default; Y3_PDL=0 or y3_set_pdl(0) turns it off)
@@ -69,6 +74,9 @@ struct ConvTcArgs {
   int custom_taps;
   int tap_shift[4], tap_wcol[4];
   int phase, ph_a, ph_b;
+  // FP8 (y3_conv_desc): per-channel dequantisation of an e4m3 input, residual scale and output scale of an e4m3 output
+  const float* dq;
+  float res_scale, out_inv_scale;
 };
 
 struct ConvTcExtra {  // host side of the above (conv_tc_prepare)
@@ -80,6 +88,7 @@ struct ConvTcExtra {  // host side of the above (conv_tc_prepare)
 
 struct ConvTcPlan {
   CUtensorMap map_a, map_b;
+  int in_fmt, out_fmt;  // Y3_FMT_*: selects the kernel instance
   int halo;    // 1: stride-1 3x3 with one A box per filter row (halo reuse)
   int bres;    // 1: weights resident in shared memory (single N tile, small K)
   ConvTcArgs args;
@@ -89,6 +98,7 @@ struct ConvTcPlan {
 int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only = false, const ConvTcExtra* extra = nullptr);
 int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream);
 int pool_launch(const y3_pool_desc& d, cudaStream_t stream);
+int amax_launch(const y3_amax_desc& d, cudaStream_t stream);
 int wgrad_tc_enabled();
 int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream);
 int wgrad_tc_s2_supported(int h, int w);

@@ -13,6 +13,7 @@ struct y3_model {
     y3_first_desc first;
     y3_pool_desc pool;
     y3_decode_desc decode;
+    y3_amax_desc amax;
   };
   std::vector<Step> steps;
 };
@@ -39,6 +40,9 @@ extern "C" int y3_model_create(const y3_op* ops, int32_t n_ops, y3_model** out) 
         break;
       case Y3_OP_DECODE:
         s.decode = ops[i].decode;
+        break;
+      case Y3_OP_AMAX:
+        s.amax = ops[i].amax;
         break;
       default:
         rc = y3::set_error(Y3_ERR_BAD_ARG, "model_create: op %d has unknown kind %d", i, ops[i].kind);
@@ -68,6 +72,8 @@ static int launch_step(const y3_model::Step& s, const void* input, y3_stream_t s
       return y3::pool_launch(s.pool, stream);
     case Y3_OP_DECODE:
       return y3_detect_head_decode_fwd(&s.decode, stream_);
+    case Y3_OP_AMAX:
+      return y3::amax_launch(s.amax, stream);
   }
   return Y3_OK;
 }

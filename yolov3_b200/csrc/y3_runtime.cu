@@ -62,8 +62,8 @@ int pdl_enabled() {
 }
 void pdl_set(int on) { g_pdl = on ? 1 : 0; }
 
-int encode_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
-                           const uint32_t* box, int swizzle_bytes) {
+int encode_tensor_map(CUtensorMap* out, int fmt, const void* base, int rank, const uint64_t* dims, const uint64_t* strides,
+                      const uint32_t* box, int swizzle_bytes) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return set_error(Y3_ERR_CUDA, "cuTensorMapEncodeTiled is not available from this driver");
   cuuint64_t gdim[5], gstr[4];
@@ -78,7 +78,9 @@ int encode_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, const u
                                 : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
                                 : swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
                                                       : CU_TENSOR_MAP_SWIZZLE_NONE;
-  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank), const_cast<void*>(base),
+  // e4m3 moves as raw bytes: TMA only copies, the wgmma reads the format
+  const CUtensorMapDataType dt = fmt == Y3_FMT_E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  const CUresult r = enc(out, dt, static_cast<cuuint32_t>(rank), const_cast<void*>(base),
                          gdim, gstr, bdim, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -138,6 +140,7 @@ extern "C" int64_t y3_abi_sizeof(int32_t which) {
     case 10: return sizeof(y3_wgrad_desc);
     case 11: return sizeof(y3_pack_item);
     case 12: return sizeof(y3_letterbox_desc);
+    case 13: return sizeof(y3_amax_desc);
   }
   return -1;
 }

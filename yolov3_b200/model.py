@@ -8,6 +8,9 @@ What is kept from the reference surface (SURVEY.md §8b): ``Model(cfg, ch, nc, a
 ``.fuse() .eval() .half() .float() .to()`` (no-ops or bookkeeping: BN folding and bf16 packing happen when an engine is
 built).  ``.train()`` switches forward/backward to the training engine (train.py: batch-statistics BatchNorm, saved
 activations, gradients into the flat parameter store).
+
+FP8 inference is opt-in: ``calibrate_fp8(batches)`` records one activation scale per tensor from bf16 forwards, then
+``precision = "fp8"`` makes every inference engine run the e4m3 tensor-core convs (DESIGN.md §2-§3).
 """
 from __future__ import annotations
 
@@ -88,6 +91,8 @@ class Model:
         self.ddp = None  # parallel.DDP(model): overlapped gradient exchange
         self._train_engines: dict = {}
         self._wver = 0  # bumped whenever the weights an Engine baked into its TMA descriptors may have changed
+        self._precision = "bf16"
+        self._fp8_scales = None  # {tensor name: scale} from calibrate_fp8 / load_fp8_scales
 
     # ------------------------------------------------------------------------------------------------ parameters
     def _init_params(self):
@@ -115,10 +120,100 @@ class Model:
     MAX_ENGINES = 4  # lowered inference engines kept alive (one per input shape/dtype); older ones are destroyed
 
     def _invalidate(self):
-        """The packed bf16 weights (whose device addresses live inside every Engine's TMA descriptors) are stale."""
+        """The packed bf16 weights (whose device addresses live inside every Engine's TMA descriptors) are stale.  The FP8
+        calibration was taken with those weights: it goes too."""
         self._wver += 1
         self._packed = None
+        self._fp8_scales = None
         self._engines.clear()
+
+    # ------------------------------------------------------------------------------------------------ FP8 inference
+    PRECISIONS = ("bf16", "fp8")
+
+    @property
+    def precision(self) -> str:
+        """Inference precision of the engines ``forward`` / ``engine()`` build: "bf16" (default) or "fp8" (e4m3 activations
+        and weights with calibrated per-tensor activation scales and per-channel weight scales).  Training is always bf16."""
+        return self._precision
+
+    @precision.setter
+    def precision(self, value: str):
+        if value not in self.PRECISIONS:
+            raise ValueError(f"precision must be one of {self.PRECISIONS}, not {value!r}")
+        if value == "fp8" and self._fp8_scales is None:
+            raise RuntimeError("precision = 'fp8' needs activation scales: run model.calibrate_fp8(batches) or "
+                               "model.load_fp8_scales(scales) first")
+        self._precision = value
+
+    @property
+    def fp8_scales(self) -> dict | None:
+        """{tensor name: scale} of the current calibration (None when there is none).  A value x of a tensor is stored
+        as e4m3(x / scale); names are conv weight prefixes (the tensor that conv writes) and ``model.<i>`` of Concat nodes."""
+        return None if self._fp8_scales is None else dict(self._fp8_scales)
+
+    def load_fp8_scales(self, scales: dict):
+        """Restore a calibration saved from ``fp8_scales`` (same weights and YAML)."""
+        scales = {str(k): float(v) for k, v in scales.items()}
+        if any(not (v > 0 and math.isfinite(v)) for v in scales.values()):
+            raise ValueError("fp8 scales must be positive and finite")
+        missing = [k for k in self.fp8_tensor_names() if k not in scales]
+        if missing:
+            raise KeyError(f"load_fp8_scales: no scale for {missing[:4]}...")
+        self._fp8_scales = scales
+        self._engines.clear()
+
+    def fp8_tensor_names(self):
+        """Every name the FP8 lowering looks a scale up for (from a dry-run calibration lowering: nothing is launched)."""
+        e = Engine(self, 1, *(2 * [int(max(self.detect.stride.tolist()))]), precision="calib", dry_run=True)
+        return list(e.amax_names) + list(e.cat_members)
+
+    @torch.no_grad()
+    def calibrate_fp8(self, batches):
+        """Per-tensor activation scales s_t = amax_t / 448 (amax over every image of every batch; zero amax -> 1) from bf16
+        forwards of ``batches`` (iterable of [n, ch, h, w] device tensors, uint8 or fp32).  A Concat buffer takes the max
+        over its producers.  Returns the scales (see ``fp8_scales``)."""
+        amax: dict[str, float] = {}
+        cats: dict[str, list[str]] = {}
+        engines = {}  # one calibration engine per input shape for the whole call
+        for x in batches:
+            if not x.is_cuda:
+                raise RuntimeError("calibrate_fp8: batches must be device tensors")
+            if x.dtype not in (torch.float32, torch.uint8):
+                x = x.float()
+            x = x.contiguous()
+            n, _, h, w = x.shape
+            key = (n, h, w, x.dtype)
+            if key not in engines:
+                engines[key] = Engine(self, n, h, w, x.dtype, 255.0 if x.dtype == torch.uint8 else 0.0, precision="calib")
+            e = engines[key]
+            e.amax.zero_()
+            e.run(x)
+            vals = e.amax.cpu().tolist()
+            for i, name in enumerate(e.amax_names):
+                amax[name] = max(amax.get(name, 0.0), vals[i])
+            cats = e.cat_members
+        if not amax:
+            raise ValueError("calibrate_fp8: no batches")
+        for cat, members in cats.items():
+            amax[cat] = max(amax[m] for m in members)
+        self._fp8_scales = {k: (v / ops.E4M3_MAX if v > 0 else 1.0) for k, v in amax.items()}
+        self._engines.clear()
+        return self.fp8_scales
+
+    def packed_e4m3(self, prefix):
+        """(e4m3 weights, bias, s_w) of one conv (BN folded for the backbone convs; Detect heads as they are), cached inside
+        ``packed()``'s dict so that every invalidation drops it."""
+        W = self.packed()
+        key = prefix + "#e4m3"
+        if key not in W:
+            P = self.params
+            if prefix + ".bn.weight" in P:
+                w, b = self.fold_bn(P[prefix + ".conv.weight"], P[prefix + ".bn.weight"], P[prefix + ".bn.bias"],
+                                    P[prefix + ".bn.running_mean"], P[prefix + ".bn.running_var"])
+            else:
+                w, b = P[prefix + ".weight"], P[prefix + ".bias"]
+            W[key] = ops.pack_conv_weight_e4m3(w, b, self.device)
+        return W[key]
 
     def state_dict(self):
         """Reference-named fp32 tensors (host copies).  While device masters exist (training) they are the truth."""
@@ -197,7 +292,7 @@ class Model:
         return self
 
     def half(self):
-        return self  # storage precision is fixed: bf16 activations/weights, fp32 accumulation and heads
+        return self  # storage is bf16 activations/weights (or e4m3 with precision = "fp8"), fp32 accumulation and heads
 
     def float(self):
         return self
@@ -254,10 +349,11 @@ class Model:
 
     # ------------------------------------------------------------------------------------------------ forward
     def engine(self, n, h, w, in_dtype=torch.float32, in_div=0.0) -> "Engine":
-        key = (n, h, w, in_dtype, float(in_div))
+        """The inference engine for one input shape at the model's ``precision`` (LRU-cached)."""
+        key = (n, h, w, in_dtype, float(in_div), self.precision)
         e = self._engines.get(key)
         if e is None:
-            e = self._engines[key] = Engine(self, n, h, w, in_dtype, in_div)
+            e = self._engines[key] = Engine(self, n, h, w, in_dtype, in_div, precision=self.precision)
             while len(self._engines) > self.MAX_ENGINES:  # variable-shape inference (rect / auto-letterbox): bounded memory
                 self._engines.popitem(last=False)
         else:
@@ -307,13 +403,21 @@ def _out_hw(h, w, k, s, p):
 class Engine:
     """One lowered instance of the graph for a fixed (n, h, w): buffers + prepared launches."""
 
-    def __init__(self, model: Model, n, h, w, in_dtype=torch.float32, in_div=0.0, dry_run=False):
+    def __init__(self, model: Model, n, h, w, in_dtype=torch.float32, in_div=0.0, dry_run=False, precision=None):
         """dry_run=True lowers the graph on whatever device the model names (CPU included) WITHOUT creating the
-        executor — host-logic tests only; nothing can be launched from a dry-run engine."""
+        executor — host-logic tests only; nothing can be launched from a dry-run engine.
+        precision: "bf16", "fp8" (needs the model's calibration) or "calib" (bf16 with an amax op after every producer;
+        ``amax`` [len(amax_names)] collects max |x| of each named tensor).  Default: the model's precision."""
         from . import tensors as _t
 
         L = _lib.lib()
         self.model, self.n, self.h, self.w = model, n, h, w
+        self.precision = model.precision if precision is None else precision
+        if self.precision not in ("bf16", "fp8", "calib"):
+            raise ValueError(f"unknown precision {self.precision!r}")
+        if self.precision == "fp8" and model._fp8_scales is None:
+            raise _lib.Y3Error("this model has no FP8 calibration (it was never calibrated, or load_state_dict / eval() "
+                               "after training / to() dropped it): run model.calibrate_fp8(batches) first")
         dev = model.device
         self.dry_run = dry_run
         if dry_run:
@@ -335,6 +439,21 @@ class Engine:
         if h % gs or w % gs:
             raise ValueError(f"image size {h}x{w} must be a multiple of the max stride {gs} (utils/general.py:281-292)")
         self.static_in = torch.zeros(n, model.ch, h, w, dtype=in_dtype, device=dev)
+
+        # ---- precision: with FP8 every tensor a tensor-core conv writes is e4m3 with its calibrated scale (a Concat
+        #      buffer's for its producers, cv1's for the SPP buffer; max-pools keep their input's format and scale); the
+        #      conv_first output (and pools of it) stays bf16.  A conv runs the e4m3 MMA exactly when its input is e4m3.
+        fp8, calib = self.precision == "fp8", self.precision == "calib"
+        S = model._fp8_scales
+        adt = torch.float8_e4m3fn if fp8 else torch.bfloat16
+
+        def sc(name):
+            return S[name] if fp8 else 1.0
+
+        self.amax_names: list[str] = []          # calib: tensor of amax[i]
+        self.cat_members: dict[str, list[str]] = {}  # Concat name -> the convs writing into it
+        self.amax = torch.zeros(len(model.conv_specs), dtype=torch.float32, device=dev) if calib else None
+        self.op_meta: dict[int, dict] = {}       # op index -> what a conv op computes (tests, inspection)
 
         # ---- shape inference
         shp: dict[int, tuple[int, int, int]] = {}
@@ -380,8 +499,9 @@ class Engine:
             if nd.type != "Concat":
                 continue
             c, hh, ww = shp[nd.i]
-            cat = PaddedNHWC.zeros(n, hh, ww, c, device=dev)
+            cat = PaddedNHWC.zeros(n, hh, ww, c, device=dev, dtype=adt, scale=sc(f"model.{nd.i}"))
             bufs[nd.i] = cat
+            self.cat_members[f"model.{nd.i}"] = []
             off = 0
             for s in nd.srcs:
                 cs = shp[s][0]
@@ -399,12 +519,16 @@ class Engine:
                         raise NotImplementedError("a tensor feeding two Concat layers would need a copy kernel")
                     alias[s] = sl
 
-        def out_buf(i):
-            """Where node i must leave its result."""
+        cat_of = {b.buf.data_ptr(): f"model.{i}" for i, b in bufs.items()}
+
+        def out_buf(i, dtype=torch.bfloat16, scale=1.0):
+            """Where node i must leave its result (a Concat slice keeps the Concat's format and scale)."""
             if i in alias:
+                if alias[i].buf.dtype != dtype:
+                    raise NotImplementedError("a bf16 tensor feeding an e4m3 Concat buffer")
                 return alias[i]
             c, hh, ww = shp[i]
-            b = PaddedNHWC.zeros(n, hh, ww, c, device=dev)
+            b = PaddedNHWC.zeros(n, hh, ww, c, device=dev, dtype=dtype, scale=scale)
             self.keep.append(b)
             return b
 
@@ -412,14 +536,33 @@ class Engine:
         self.err = torch.zeros(1, dtype=torch.int32, device=dev)
 
         def emit_conv(x, prefix, c_out, k, s, act, out=None, res=None, upsample=False, out_f32=None):
-            wt, bs_ = W[prefix]
+            dq = None
+            if x.fmt == _lib.FMT_E4M3:
+                wt, bs_, sw = model.packed_e4m3(prefix)
+                dq = (sw * x.scale).contiguous()  # dq[n] = s_in * s_w[n]
+                self.keep.append(dq)
+            else:
+                wt, bs_ = W[prefix]
             o = _lib.Op()
             o.kind = _lib.OP_CONV
-            o.conv = ops.conv_desc(x, wt, bs_, c_out, k, s, act, out, res, upsample, out_f32, self.err)
+            o.conv = ops.conv_desc(x, wt, bs_, c_out, k, s, act, out, res, upsample, out_f32, self.err, dq=dq)
             if L.y3_conv_weight_layout(C.byref(o.conv)) == _lib.W_XPAIR and prefix + ".bn.weight" in model.params:
                 wx, _ = model.packed_xpair(prefix)
+                wt = wx
                 o.conv.weight, o.conv.weight_layout = wx.data_ptr(), _lib.W_XPAIR
             op_list.append(o)
+            self.op_meta[len(op_list) - 1] = dict(name=prefix, x=x, out=out, res=res, out_f32=out_f32, k=k, s=s, act=act,
+                                                  upsample=upsample, weight=wt, bias=bs_, dq=dq)
+            if out_f32 is None:
+                cat = cat_of.get(out.buf.data_ptr())
+                if cat is not None:
+                    self.cat_members[cat].append(prefix)
+                if calib:  # Bottleneck ping buffers are reused: the amax must be taken right after the producer
+                    a = _lib.Op()
+                    a.kind = _lib.OP_AMAX
+                    a.amax = ops.amax_desc(out, self.amax[len(self.amax_names):])
+                    self.amax_names.append(prefix)
+                    op_list.append(a)
 
         tens: dict[int, object] = {}  # node -> PaddedNHWC (or ("zeropad", tensor))
         for nd in nodes[:-1]:
@@ -446,7 +589,8 @@ class Engine:
                         y = None
                     else:
                         ho, wo = _out_hw(x.h, x.w, k, s, k // 2)
-                        y = out_buf(nd.i) if last else PaddedNHWC.zeros(n, ho, wo, c2, device=dev)
+                        y = out_buf(nd.i, adt, sc(r)) if last else PaddedNHWC.zeros(n, ho, wo, c2, device=dev, dtype=adt,
+                                                                                    scale=sc(r))
                         emit_conv(x, r, c2, k, s, ops.ACT_SILU, out=y)
                     self.keep.append(y)
                     x = y
@@ -457,15 +601,18 @@ class Engine:
                 assert len(rest) < 2 or rest[1] == 1, "grouped Bottleneck is not used by the YOLOv3 YAMLs"
                 x = srcs[0]
                 c_ = int(c2 * 0.5)
-                tmp = PaddedNHWC.zeros(n, x.h, x.w, c_, device=dev)
-                ping = [PaddedNHWC.zeros(n, x.h, x.w, c2, device=dev) for _ in range(min(2, max(0, len(reps) - 1)))]
+                tmp = PaddedNHWC.zeros(n, x.h, x.w, c_, device=dev, dtype=adt)
+                ping = [PaddedNHWC.zeros(n, x.h, x.w, c2, device=dev, dtype=adt)
+                        for _ in range(min(2, max(0, len(reps) - 1)))]
                 self.keep += [tmp, *ping]
-                final = out_buf(nd.i)
+                final = out_buf(nd.i, adt, sc(reps[-1] + ".cv2"))
                 for ri, r in enumerate(reps):
-                    y = final if ri == len(reps) - 1 else ping[ri % 2]
+                    # the shared buffers carry the scale of the conv that writes them this time
+                    t = PaddedNHWC(tmp.buf, 0, c_, sc(r + ".cv1"))
+                    y = final if ri == len(reps) - 1 else PaddedNHWC(ping[ri % 2].buf, 0, c2, sc(r + ".cv2"))
                     add = shortcut and c1 == c2
-                    emit_conv(x, r + ".cv1", c_, 1, 1, ops.ACT_SILU, out=tmp)
-                    emit_conv(tmp, r + ".cv2", c2, 3, 1, ops.ACT_SILU, out=y, res=x if add else None)
+                    emit_conv(x, r + ".cv1", c_, 1, 1, ops.ACT_SILU, out=t)
+                    emit_conv(t, r + ".cv2", c2, 3, 1, ops.ACT_SILU, out=y, res=x if add else None)
                     x, c1 = y, c2
                 tens[nd.i] = x
             elif nd.type == "SPP":
@@ -474,7 +621,7 @@ class Engine:
                 assert ks == (5, 9, 13), "SPP kernels other than (5, 9, 13) are not used by the YOLOv3 YAMLs"
                 x = srcs[0]
                 c_ = c1 // 2
-                cat = PaddedNHWC.zeros(n, x.h, x.w, 4 * c_, device=dev)
+                cat = PaddedNHWC.zeros(n, x.h, x.w, 4 * c_, device=dev, dtype=adt, scale=sc(base + ".cv1"))
                 self.keep.append(cat)
                 emit_conv(x, base + ".cv1", c_, 1, 1, ops.ACT_SILU, out=cat.slice(0, c_))
                 for q in range(3):  # 5x5 cascade == 5/9/13 pools with -inf padding
@@ -482,7 +629,7 @@ class Engine:
                     o.kind = _lib.OP_MAXPOOL
                     o.pool = ops.pool_desc(cat.slice(q * c_, c_), cat.slice((q + 1) * c_, c_), 5, 1, -2, False)
                     op_list.append(o)
-                y = out_buf(nd.i)
+                y = out_buf(nd.i, adt, sc(base + ".cv2"))
                 emit_conv(cat, base + ".cv2", c2, 1, 1, ops.ACT_SILU, out=y)
                 tens[nd.i] = y
             elif nd.type == "MaxPool2d":
@@ -495,7 +642,10 @@ class Engine:
                     _, x, pad = x
                     assert tuple(pad) == (0, 1, 0, 1) and (k, s, p) == (2, 1, 0), "only ZeroPad2d([0,1,0,1])+MaxPool2d(2,1,0)"
                     oob_zero = True
-                y = out_buf(nd.i)
+                if nd.i in alias and self.precision != "bf16":
+                    # its codes would carry the input's scale, not the Concat's, and calibration would miss it
+                    raise NotImplementedError("FP8: a max-pool writing into a Concat buffer")
+                y = out_buf(nd.i, x.buf.dtype, x.scale)
                 o = _lib.Op()
                 o.kind = _lib.OP_MAXPOOL
                 o.pool = ops.pool_desc(x, y, k, s, -p, oob_zero)
