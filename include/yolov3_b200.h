@@ -35,7 +35,7 @@ typedef void* y3_stream_t; /* cudaStream_t */
 int y3_version(void);
 /* Copies the calling thread's last error text into buf (NUL-terminated); returns its length. */
 int y3_last_error(char* buf, size_t n);
-/* Y3_OK iff the current CUDA device is compute capability 10.x. */
+/* Y3_OK iff the current CUDA device is compute capability 9.0. */
 int y3_device_check(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror definitions:
  * 0 y3_conv_desc, 1 y3_first_desc, 2 y3_pool_desc, 3 y3_detect_level, 4 y3_decode_desc, 5 y3_op, 6 y3_nms_params,
@@ -46,11 +46,6 @@ int64_t y3_abi_sizeof(int32_t which);
  * Results are identical either way — only the launch boundaries overlap.  Returns the previous setting.  A tuning switch with
  * no counterpart in the reference. */
 int y3_set_pdl(int32_t on);
-/* Kernel-variant switch of y3_bn_act_bwd (non-upsample layers): 1 (default) = the cp.async shared-memory-ring kernels (three
- * work units requested ahead per thread), 0 = the register-staged ones.  Same unit order and arithmetic: results are
- * bit-identical (tests/test_bn_variants_gpu.py).  Env Y3_BN_ASYNC=0/1 sets the initial value.  Returns the
- * previous setting.  A tuning switch with no counterpart in the reference. */
-int y3_set_bn_async(int32_t on);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Conv + folded-BN + SiLU (+ residual add, + nearest-2x upsample, + concat-offset store, or fp32 head store).

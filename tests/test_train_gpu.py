@@ -22,13 +22,23 @@ def _padded(x, ld=None, coff=0):
     return t.load_nchw(x.cuda())
 
 
-@pytest.mark.parametrize("c,ld,coff,upsample,res", [(64, None, 0, False, False), (128, 192, 64, False, True), (32, None, 0, True, False)])
-def test_bn_forward_and_backward(c, ld, coff, upsample, res):
+@pytest.mark.parametrize("n,h,w,c,ld,coff,upsample,res", [
+    (3, 10, 14, 64, None, 0, False, False),
+    (3, 10, 14, 128, 192, 64, False, True),
+    (3, 10, 14, 32, None, 0, True, False),
+    (2, 5, 7, 64, None, 0, False, False),        # less than one work unit per row, fewer units than blocks
+    (3, 13, 13, 512, None, 0, False, False),     # 832 items per row: one full + one partial unit
+    (2, 2, 2, 1024, None, 0, False, False),      # the 64x64 test images' deepest layer
+    (2, 32, 32, 16, None, 0, False, False),      # yolov3-tiny's 16-channel layer
+    (4, 80, 80, 256, None, 0, False, False),     # several units per block (one wave of 396 blocks)
+    (2, 160, 160, 64, None, 0, False, False),
+    (2, 20, 20, 256, None, 0, True, False),      # 2x-upsample layer
+])
+def test_bn_forward_and_backward(n, h, w, c, ld, coff, upsample, res):
     from yolov3_b200 import train_ops as T
     from yolov3_b200.tensors import PaddedNHWC
 
     g = torch.Generator().manual_seed(1)
-    n, h, w = 3, 10, 14
     y = (torch.randn(n, c, h, w, generator=g) * 1.5 + 0.3).bfloat16().float()
     gamma, beta = torch.rand(c, generator=g) + 0.5, torch.randn(c, generator=g) * 0.2
     r = torch.randn(n, c, h, w, generator=g).bfloat16().float() if res else None

@@ -1,9 +1,8 @@
-"""Run ONE conv layer shape of the yolov3 graph repeatedly (ncu target / A-B timing of kernel variants).
+"""Run ONE conv layer shape of the yolov3 graph repeatedly (ncu target / kernel timing).
 
   python tools/probe_layer.py --cin 32 --cout 64 --k 3 --s 2 --hw 640 --n 32 [--res] [--iters 5] [--time]
 
-With --time prints the CUDA-event average over the iterations (inputs of the big early layers exceed L2 on their own).
-Environment toggles of the library (Y3_CONV_HALO / _BRES) apply."""
+With --time prints the CUDA-event average over the iterations (inputs of the big early layers exceed L2 on their own)."""
 import argparse
 import sys
 from pathlib import Path

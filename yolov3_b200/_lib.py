@@ -188,7 +188,6 @@ def _declare(lib):
         "y3_conv_plan": ([C.POINTER(ConvDesc), C.POINTER(ConvPlanInfo)], C.c_int),
         "y3_abi_sizeof": ([i32], C.c_int64),
         "y3_set_pdl": ([i32], C.c_int),
-        "y3_set_bn_async": ([i32], C.c_int),
         "y3_conv_first_fwd": ([C.POINTER(FirstDesc), vp], C.c_int),
         "y3_maxpool_fwd": ([C.POINTER(PoolDesc), vp], C.c_int),
         "y3_amax_nhwc": ([vp, i32, i32, i32, i32, i32, i32, i32, vp, vp], C.c_int),

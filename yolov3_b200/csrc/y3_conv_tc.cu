@@ -31,7 +31,6 @@
 // channels), the residual is staged as e4m3, and an e4m3 input stages its dq floats beside the bias.
 #include <cuda_bf16.h>
 
-#include <cstdlib>
 #include <type_traits>
 
 #include "y3_common.cuh"
@@ -679,26 +678,6 @@ int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream) {
   return set_error(Y3_ERR_BAD_ARG, "conv_tc: formats %d -> %d", plan.in_fmt, plan.out_fmt);
 }
 
-// Y3_CONV_HALO=0 disables the halo-reuse A path (A/B measurements).
-static bool halo_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("Y3_CONV_HALO");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
-
-// Y3_CONV_BRES=0 streams the weights through the ring everywhere (A/B measurements).
-static bool bres_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("Y3_CONV_BRES");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
-
 // Layer 1 of yolov3 (32 -> 64, stride 2 at 640x640) moved 64-byte rows through 9 five-dimensional TMA boxes per tile
 // and ran at 0.2 PFLOP/s; paired, the same tile is 6 boxes of full 128-byte rows and one K = 64 MMA group per box.
 // (mul, shr) such that n / d == (t + ((n - t) >> 1)) >> (shr - 1), t = umulhi(n, mul), for every 32-bit n (d >= 2);
@@ -828,7 +807,7 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     a.rows_total = static_cast<int>(rows);
     a.m_tiles = static_cast<int>((rows + kBlockM - 1) / kBlockM);
     // halo reuse needs >= 2 stages of (17 KB + 3 B tiles): N <= 128 (N = 256 would leave room for one stage)
-    plan->halo = (!extra && taps == 9 && ((bk == 64 && bn <= 128) || (bk == 32 && bn <= 64)) && halo_enabled()) ? 1 : 0;
+    plan->halo = (!extra && taps == 9 && ((bk == 64 && bn <= 128) || (bk == 32 && bn <= 64))) ? 1 : 0;
     if (extra) {
       a.custom_taps = 1;
       for (int t = 0; t < extra->ntaps; ++t) {
@@ -892,7 +871,7 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     // resident weights: one N tile whose (taps x k-blocks) boxes fit beside a useful A ring.  The TMA unit's row rate
     // (not bytes) bounds the thin layers, and re-fetching the same <= 96 KB of weights for every M tile was most of it.
     const long long b_bytes = static_cast<long long>(taps) * a.kblocks * bn * bk * 2;
-    plan->bres = (a.n_tiles == 1 && b_bytes <= 96 * 1024 && bres_enabled()) ? 1 : 0;
+    plan->bres = (a.n_tiles == 1 && b_bytes <= 96 * 1024) ? 1 : 0;
   }
   const int sms = num_sms();
   const long long total = static_cast<long long>(a.m_tiles) * a.n_tiles;
@@ -921,12 +900,7 @@ extern "C" int y3_conv_plan(const y3_conv_desc* d, y3_conv_plan_info* out) {
 
 extern "C" int y3_conv_weight_layout(const y3_conv_desc* d) {
   if (!d) return y3::set_error(Y3_ERR_BAD_ARG, "conv: null descriptor");
-  static int enabled = -1;  // Y3_CONV_XPAIR=0 keeps the plain tap-major layout everywhere (A/B measurements)
-  if (enabled < 0) {
-    const char* e = getenv("Y3_CONV_XPAIR");
-    enabled = (e && e[0] == '0') ? 0 : 1;
-  }
-  return (enabled && y3::conv_prefers_xpair(*d)) ? Y3_W_XPAIR : Y3_W_TAPS;
+  return y3::conv_prefers_xpair(*d) ? Y3_W_XPAIR : Y3_W_TAPS;
 }
 
 extern "C" int y3_conv_cout_pad(int32_t c_out) {

@@ -38,10 +38,6 @@ inline int encode_tensor_map_bf16(CUtensorMap* out, const void* base, int rank, 
 int num_sms();
 int pdl_enabled();   // programmatic dependent launch on (default; Y3_PDL=0 or y3_set_pdl(0) turns it off)
 void pdl_set(int on);
-// Kernel-variant switch (A/B-able at run time; results are bit-identical either way, see y3_set_bn_async in the public header)
-#ifndef Y3_BN_ASYNC_DEFAULT
-#define Y3_BN_ASYNC_DEFAULT 1
-#endif
 
 // ---- tensor-core conv: kernel arguments (device view) and a prepared launch
 struct ConvTcArgs {
@@ -99,7 +95,6 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only = 
 int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream);
 int pool_launch(const y3_pool_desc& d, cudaStream_t stream);
 int amax_launch(const y3_amax_desc& d, cudaStream_t stream);
-int wgrad_tc_enabled();
 int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream);
 int wgrad_tc_s2_supported(int h, int w);
 int pool_train_fwd(const y3_pool_desc& d, uint8_t* idx, cudaStream_t stream);

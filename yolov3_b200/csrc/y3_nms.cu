@@ -1,12 +1,12 @@
 // yolov3_b200 — batched non-maximum suppression entirely on the device, no host synchronisation.
 // Replaces non_max_suppression (reference utils/general.py:630-750) together with torchvision.ops.nms (:733):
-//   K1 candidates : obj > thr, conf = obj*cls, best class (or every class > thr when multi_label), class filter
-//                   -> 64-bit key (conf bits | ~candidate id) appended per image               (general.py:669-718)
-//   K2 sort       : bitonic sort of the keys, descending == stable sort by conf               (general.py:728)
-//   K3 gather     : rank r < min(count, max_nms): xywh -> xyxy, class-offset boxes            (general.py:705,731-732)
-//   K4 sort       : (class, rank) keys ascending -> per-class segments in confidence order
-//   K5 segments   : greedy suppression inside each (image, class) segment, strict IoU > thr   (torchvision nms)
-//   K6 compact    : first max_det kept ranks in confidence order -> out rows + counts         (general.py:734,743)
+//   candidates : obj > thr, conf = obj*cls, best class (or every class > thr when multi_label), class filter
+//                -> 64-bit key (conf bits | ~candidate id) and the row's xywh, appended per image (general.py:669-718)
+//   bucket     : max_nms cut by key (general.py:728), xywh -> xyxy (general.py:705), counting sort by class into
+//                per-(image, class) segments
+//   segments   : rank each segment's members by key, greedy suppression of class-offset boxes, strict IoU > thr
+//                (general.py:731-732, torchvision nms); segment mask for <= 512 members, segment block above
+//   output     : the max_det largest survivor keys in confidence order -> out rows + sources + counts (general.py:734,743)
 // Exactness: every floating-point step is a separately rounded fp32 operation in the reference's order (this file is
 // compiled with -fmad=false and without fast-math), so kept sets and output rows are bit-identical to the reference on
 // identical inputs whenever confidences are tie-free (ties: lower candidate index first, i.e. a stable sort; the
@@ -15,7 +15,6 @@
 // violate that bound (or agnostic=True) take the single-segment path over all candidates.
 // The reference's wall-clock time_limit break (general.py:675,746-748) is deliberately not reproduced.
 #include <cmath>
-#include <cstdlib>
 #include <cstring>
 
 #include "y3_common.cuh"
@@ -24,7 +23,7 @@
 namespace y3 {
 namespace {
 
-constexpr int kSortTile = 4096;   // keys sorted per CTA in shared memory
+constexpr int kMinCap = 4096;     // smallest candidate capacity per image
 constexpr int kRankCap = 32768;   // >= max_nms (30000), power of two
 constexpr int kSegSmemBoxes = 2048;
 
@@ -35,18 +34,14 @@ struct NmsArgs {
   double iou_mid;  // midpoint between iou_thres and the next float above it (division-free exact IoU test)
   int iou_odd;     // mantissa LSB of iou_thres: where a quotient exactly at the midpoint rounds to
   int multi_label, agnostic, max_det, max_nms;
-  int cap;  // candidate capacity per image (power of two >= kSortTile)
+  int cap;  // candidate capacity per image (power of two >= kMinCap)
   uint32_t cls_mask[32];
   int use_mask;
   // workspace
   unsigned long long* keys;  // [bs, cap]
-  float4* cand_box;          // [bs, cap] (cx, cy, w, h) of the candidate's row, written beside its key (v2: K2 reads no pred row)
+  float4* cand_box;          // [bs, cap] (cx, cy, w, h) of the candidate's row, written beside its key (bucketing reads no pred row)
   int* count;                // [bs] candidates found (may exceed cap)
-  int* flags;                // [bs] bit0: needs single-segment path; bit1: has a class segment too long for one warp
-  float* det;                // [bs, kRankCap, 6]
-  uint32_t* seg_keys;        // [bs, kRankCap]
-  uint8_t* keep;             // [bs, kRankCap]
-  // v2 (class-bucketed) workspace
+  int* flags;                // [bs] bit0: needs single-segment path
   int* seg_off;                  // [bs, nc + 1] first member of every class segment (conf-unordered members)
   unsigned long long* seg_key2;  // [bs, kRankCap] candidate keys grouped by class
   float4* box4;                  // [bs, kRankCap] xyxy of the member at the same position
@@ -64,7 +59,7 @@ struct NmsArgs {
 
 __device__ __forceinline__ int next_pow2(int v) { return v <= 1 ? 1 : 1 << (32 - __clz(v - 1)); }
 
-// ------------------------------------------------------------------------------------------------ K1 candidates
+// ------------------------------------------------------------------------------------------------ candidates
 // One warp per 32 consecutive prediction rows: the lanes test obj of 32 rows with one strided load, then the warp visits
 // only the rows that passed (85 contiguous floats each), and one atomic per warp reserves the key slots.  The first
 // version spent a warp, two block barriers and a share of a block atomic on EVERY row and was bound by those serial
@@ -216,167 +211,6 @@ __global__ void __launch_bounds__(32 * kCandWarps) nms_candidates_kernel(const N
   }
 }
 
-// ------------------------------------------------------------------------------------------------ bitonic sort
-// Sorts, per image, the first npow2(count) keys (padding written by the caller).  DESC=true: descending.
-template <typename T, bool DESC>
-__device__ __forceinline__ void cmp_swap(T& a, T& b, bool up) {
-  // `up` = this pair must end ascending (a <= b) in the un-flipped network
-  const bool swap = DESC ? (up ? a < b : a > b) : (up ? a > b : a < b);
-  if (swap) {
-    const T t = a;
-    a = b;
-    b = t;
-  }
-}
-
-__device__ __forceinline__ int sort_len(const NmsArgs& p, int img, bool second) {
-  int c = p.count[img];
-  if (!second) {
-    c = c < p.cap ? c : p.cap;
-  } else {
-    c = c < p.cap ? c : p.cap;
-    c = c < p.max_nms ? c : p.max_nms;
-  }
-  return next_pow2(c);
-}
-
-// full sort of each kSortTile-sized tile in shared memory (k = 2 .. kSortTile)
-template <typename T, bool DESC>
-__global__ void __launch_bounds__(1024) bitonic_local_kernel(const NmsArgs p, T* base, int stride, bool second) {
-  __shared__ T s[kSortTile];
-  const int img = blockIdx.y;
-  const int n = sort_len(p, img, second);
-  const int t0 = blockIdx.x * kSortTile;
-  if (t0 >= n) return;
-  T* g = base + static_cast<size_t>(img) * stride + t0;
-  for (int i = threadIdx.x; i < kSortTile; i += blockDim.x) s[i] = g[i];
-  __syncthreads();
-  for (int k = 2; k <= kSortTile; k <<= 1) {
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int t = threadIdx.x; t < kSortTile / 2; t += blockDim.x) {
-        const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-        const bool up = (((t0 + i) & k) == 0);
-        cmp_swap<T, DESC>(s[i], s[i | j], up);
-      }
-      __syncthreads();
-    }
-  }
-  for (int i = threadIdx.x; i < kSortTile; i += blockDim.x) g[i] = s[i];
-}
-
-// one global compare-exchange step (k > kSortTile, j >= kSortTile)
-template <typename T, bool DESC>
-__global__ void __launch_bounds__(256) bitonic_global_kernel(const NmsArgs p, T* base, int stride, bool second, int k,
-                                                             int j) {
-  const int img = blockIdx.y;
-  const int n = sort_len(p, img, second);
-  if (k > n) return;
-  const int t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n / 2) return;
-  const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-  T* g = base + static_cast<size_t>(img) * stride;
-  T a = g[i], b = g[i | j];
-  const bool up = ((i & k) == 0);
-  const T a0 = a, b0 = b;
-  cmp_swap<T, DESC>(a, b, up);
-  if (a != a0) {
-    g[i] = a;
-    g[i | j] = b;
-  }
-  (void)b0;
-}
-
-// finish merge level k inside each tile (j = kSortTile/2 .. 1)
-template <typename T, bool DESC>
-__global__ void __launch_bounds__(1024) bitonic_merge_kernel(const NmsArgs p, T* base, int stride, bool second, int k) {
-  __shared__ T s[kSortTile];
-  const int img = blockIdx.y;
-  const int n = sort_len(p, img, second);
-  if (k > n) return;
-  const int t0 = blockIdx.x * kSortTile;
-  if (t0 >= n) return;
-  T* g = base + static_cast<size_t>(img) * stride + t0;
-  for (int i = threadIdx.x; i < kSortTile; i += blockDim.x) s[i] = g[i];
-  __syncthreads();
-  for (int j = kSortTile >> 1; j > 0; j >>= 1) {
-    for (int t = threadIdx.x; t < kSortTile / 2; t += blockDim.x) {
-      const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
-      const bool up = (((t0 + i) & k) == 0);
-      cmp_swap<T, DESC>(s[i], s[i | j], up);
-    }
-    __syncthreads();
-  }
-  for (int i = threadIdx.x; i < kSortTile; i += blockDim.x) g[i] = s[i];
-}
-
-// write padding so that the sort networks see a full power-of-two array (at least one tile)
-__global__ void __launch_bounds__(256) pad_keys_kernel(const NmsArgs p) {
-  const int img = blockIdx.y;
-  int c = p.count[img];
-  c = c < p.cap ? c : p.cap;
-  int n = next_pow2(c);
-  n = n < kSortTile ? kSortTile : n;
-  unsigned long long* keys = p.keys + static_cast<size_t>(img) * p.cap;
-  for (int i = c + blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) keys[i] = 0ull;
-}
-
-// ------------------------------------------------------------------------------------------------ K3 gather
-__global__ void __launch_bounds__(256) nms_gather_kernel(const NmsArgs p) {
-  const int img = blockIdx.y;
-  int c = p.count[img];
-  c = c < p.cap ? c : p.cap;
-  const int n = c < p.max_nms ? c : p.max_nms;
-  int npad = next_pow2(n);
-  npad = npad < kSortTile ? kSortTile : npad;
-  const int r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= npad) return;
-  uint32_t* sk = p.seg_keys + static_cast<size_t>(img) * kRankCap;
-  if (r >= n) {
-    sk[r] = 0xFFFFFFFFu;
-    return;
-  }
-  const unsigned long long key = p.keys[static_cast<size_t>(img) * p.cap + r];
-  const uint32_t id = 0xFFFFFFFFu - static_cast<uint32_t>(key & 0xFFFFFFFFull);
-  const float conf = __uint_as_float(static_cast<uint32_t>(key >> 32));
-  const int row = id / p.nc, cls = id - row * p.nc;
-  const float* x = p.pred + (static_cast<size_t>(img) * p.n_rows + row) * p.no;
-  const float cx = __ldg(x), cy = __ldg(x + 1), w = __ldg(x + 2), h = __ldg(x + 3);
-  const float hw = __fdiv_rn(w, 2.0f), hh = __fdiv_rn(h, 2.0f);
-  const float x1 = __fsub_rn(cx, hw), y1 = __fsub_rn(cy, hh), x2 = __fadd_rn(cx, hw), y2 = __fadd_rn(cy, hh);
-  float* d = p.det + (static_cast<size_t>(img) * kRankCap + r) * 6;
-  d[0] = x1;
-  d[1] = y1;
-  d[2] = x2;
-  d[3] = y2;
-  d[4] = conf;
-  d[5] = static_cast<float>(cls);
-  p.keep[static_cast<size_t>(img) * kRankCap + r] = 0;
-  sk[r] = p.agnostic ? static_cast<uint32_t>(r) : ((static_cast<uint32_t>(cls) << 15) | static_cast<uint32_t>(r));
-  // class-split greedy NMS is only exact while offset boxes of different classes cannot intersect
-  const float lim = p.max_wh * 0.5f;
-  const bool inside = (x1 > -lim) && (x2 < lim) && (x1 <= x2);
-  if (!inside && !p.agnostic) atomicOr(&p.flags[img], 1);
-}
-
-// ------------------------------------------------------------------------------------------------ K5 segments
-// 32-ary search by one warp: 3 probes of 32 positions instead of 15 dependent global loads
-__device__ __forceinline__ int lower_bound_warp(const uint32_t* a, int n, uint32_t v, int lane) {
-  int lo = 0, hi = n;  // invariant: a[lo-1] < v <= a[hi]
-  while (hi - lo > 0) {
-    const int span = hi - lo;
-    const int step = (span + 32) / 33;  // 32 probes split the span into 33 pieces
-    const int pos = lo + (lane + 1) * step - 1;
-    const bool less = pos < hi && a[pos] < v;
-    const unsigned b = __ballot_sync(0xffffffffu, less);
-    const int k = __popc(b);  // probes 0..k-1 are < v (monotone)
-    const int new_lo = k ? lo + k * step : lo;
-    const int new_hi = k < 32 ? min(hi, lo + (k + 1) * step - 1) : hi;
-    lo = min(new_lo, hi);
-    hi = new_hi;
-  }
-  return lo;
-}
-
 // fdiv_rn(inter, uni) > thr  without the division: the correctly rounded quotient exceeds thr iff the exact quotient lies
 // above the midpoint `mid` of thr and its successor (or exactly on it when round-to-nearest-even picks the successor).
 // uni has 24 and mid at most 25 significant bits, so uni * mid is exact in double.  Degenerate operands (uni <= 0, NaN,
@@ -402,212 +236,19 @@ __device__ __forceinline__ bool box_suppresses(const float4& bi, float ai, const
   return iou_exceeds(inter, __fsub_rn(__fadd_rn(ai, aj), inter), p);
 }
 
-// One WARP per (image, class) segment of up to 512 members: boxes live in registers (member j -> lane j % 32, slot j / 32),
-// the box of the current keeper is broadcast by shuffle, no block barrier in the greedy loop.  The block-per-segment
-// kernel below spent 8 warps and a __syncthreads per keeper and was issue-bound (5 blocks per SM in lock-step).
-constexpr int kWarpSlots = 16;
-constexpr int kWarpSegMax = 32 * kWarpSlots;
-
-__global__ void __launch_bounds__(256) nms_segments_warp_kernel(const NmsArgs p) {
-  const unsigned full = 0xffffffffu;
-  const int img = blockIdx.y;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int seg = blockIdx.x * 8 + warp;
-  if (seg >= p.nc) return;
-  int c = p.count[img];
-  c = c < p.cap ? c : p.cap;
-  const int n = c < p.max_nms ? c : p.max_nms;
-  if (n == 0 || p.agnostic || (p.flags[img] & 1)) return;  // single-segment images go to the block kernel
-  const uint32_t* sk = p.seg_keys + static_cast<size_t>(img) * kRankCap;
-  const int lo = lower_bound_warp(sk, n, static_cast<uint32_t>(seg) << 15, lane);
-  const int hi = lower_bound_warp(sk, n, static_cast<uint32_t>(seg + 1) << 15, lane);
-  const int m = hi - lo;
-  if (m <= 0) return;
-  if (m > kWarpSegMax) {
-    if (lane == 0) atomicOr(&p.flags[img], 2);
-    return;
-  }
-  const float* det = p.det + static_cast<size_t>(img) * kRankCap * 6;
-  float4 b[kWarpSlots];
-  uint32_t supp = 0;  // bit s: my member of slot s is suppressed (or does not exist)
-#pragma unroll
-  for (int s = 0; s < kWarpSlots; ++s) {
-    const int j = s * 32 + lane;
-    b[s] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (j < m) {
-      const float* d = det + static_cast<size_t>(sk[lo + j] & 0x7FFFu) * 6;
-      const float off = __fmul_rn(d[5], p.max_wh);
-      b[s] = make_float4(__fadd_rn(d[0], off), __fadd_rn(d[1], off), __fadd_rn(d[2], off), __fadd_rn(d[3], off));
-    } else {
-      supp |= 1u << s;
-    }
-  }
-#pragma unroll
-  for (int s = 0; s < kWarpSlots; ++s) {
-    if (s * 32 >= m) break;
-    unsigned dead = __ballot_sync(full, (supp >> s) & 1u);  // warp-uniform view of slot s
-    const int cnt = min(32, m - s * 32);
-    for (int l = 0; l < cnt; ++l) {
-      if ((dead >> l) & 1u) continue;
-      float4 bi;
-      bi.x = __shfl_sync(full, b[s].x, l);
-      bi.y = __shfl_sync(full, b[s].y, l);
-      bi.z = __shfl_sync(full, b[s].z, l);
-      bi.w = __shfl_sync(full, b[s].w, l);
-      const float ai = __fmul_rn(__fsub_rn(bi.z, bi.x), __fsub_rn(bi.w, bi.y));
-      const bool hit = lane > l && !((supp >> s) & 1u) && box_suppresses(bi, ai, b[s], p);
-      if (hit) supp |= 1u << s;
-      dead |= __ballot_sync(full, hit);
-#pragma unroll
-      for (int s2 = s + 1; s2 < kWarpSlots; ++s2) {
-        if (s2 * 32 >= m) break;
-        if (!((supp >> s2) & 1u) && box_suppresses(bi, ai, b[s2], p)) supp |= 1u << s2;
-      }
-    }
-  }
-  uint8_t* keep = p.keep + static_cast<size_t>(img) * kRankCap;
-#pragma unroll
-  for (int s = 0; s < kWarpSlots; ++s) {
-    const int j = s * 32 + lane;
-    if (j < m && !((supp >> s) & 1u)) keep[sk[lo + j] & 0x7FFFu] = 1;
-  }
-}
-
-__global__ void __launch_bounds__(256) nms_segments_kernel(const NmsArgs p) {
-  __shared__ float4 s_box[kSegSmemBoxes];
-  __shared__ uint16_t s_rank[kSegSmemBoxes];
-  __shared__ uint32_t s_supp[(kRankCap + 31) / 32];
-  __shared__ int s_bounds[2];
-  const int img = blockIdx.y, seg = blockIdx.x;
-  int c = p.count[img];
-  c = c < p.cap ? c : p.cap;
-  const int n = c < p.max_nms ? c : p.max_nms;
-  if (n == 0) return;
-  const int fl = p.flags[img];
-  const bool single = p.agnostic || (fl & 1);
-  if (single && seg != 0) return;
-  if (!single && !(fl & 2)) return;  // every class segment of this image fitted the warp kernel
-  const uint32_t* sk = p.seg_keys + static_cast<size_t>(img) * kRankCap;
-  if (!single) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp < 2) {
-      const int b = lower_bound_warp(sk, n, static_cast<uint32_t>(seg + warp) << 15, lane);
-      if (lane == 0) s_bounds[warp] = b;
-    }
-    __syncthreads();
-  }
-  const int lo = single ? 0 : s_bounds[0], hi = single ? n : s_bounds[1];
-  const int m = hi - lo;
-  if (m <= 0) return;
-  if (!single && m <= kWarpSegMax) return;  // done by nms_segments_warp_kernel
-  const float* det = p.det + static_cast<size_t>(img) * kRankCap * 6;
-  uint8_t* keep = p.keep + static_cast<size_t>(img) * kRankCap;
-  // member j of the segment (confidence order) -> rank
-  auto rank_of = [&](int j) -> int { return single ? j : static_cast<int>(sk[lo + j] & 0x7FFFu); };
-  auto load_box = [&](int rank) -> float4 {
-    const float* d = det + static_cast<size_t>(rank) * 6;
-    const float off = p.agnostic ? 0.0f : __fmul_rn(d[5], p.max_wh);
-    return make_float4(__fadd_rn(d[0], off), __fadd_rn(d[1], off), __fadd_rn(d[2], off), __fadd_rn(d[3], off));
-  };
-  const bool in_smem = m <= kSegSmemBoxes;
-  for (int j = threadIdx.x; j < (m + 31) / 32; j += blockDim.x) s_supp[j] = 0;
-  if (in_smem) {
-    for (int j = threadIdx.x; j < m; j += blockDim.x) {
-      const int rk = rank_of(j);
-      const float4 b = load_box(rk);
-      s_rank[j] = static_cast<uint16_t>(rk);
-      s_box[j] = b;
-    }
-  }
-  __syncthreads();
-  // greedy pass: nothing inside the serial loop touches global memory when the segment fits in shared memory
-  for (int i = 0; i < m; ++i) {
-    if ((s_supp[i >> 5] >> (i & 31)) & 1u) continue;  // uniform: every thread reads the same word
-    float4 bi;
-    float ai;
-    bi = in_smem ? s_box[i] : load_box(rank_of(i));
-    ai = __fmul_rn(__fsub_rn(bi.z, bi.x), __fsub_rn(bi.w, bi.y));
-    if (i + 1 >= m) break;
-    for (int j = i + 1 + threadIdx.x; j < m; j += blockDim.x) {
-      if ((s_supp[j >> 5] >> (j & 31)) & 1u) continue;
-      const float4 bj = in_smem ? s_box[j] : load_box(rank_of(j));
-      if (box_suppresses(bi, ai, bj, p)) atomicOr(&s_supp[j >> 5], 1u << (j & 31));
-    }
-    __syncthreads();
-  }
-  __syncthreads();
-  // a member that was never suppressed was kept (gather zeroed the keep flags)
-  for (int j = threadIdx.x; j < m; j += blockDim.x)
-    if (!((s_supp[j >> 5] >> (j & 31)) & 1u)) keep[in_smem ? static_cast<int>(s_rank[j]) : rank_of(j)] = 1;
-}
-
-// ------------------------------------------------------------------------------------------------ K6 compact
-__global__ void __launch_bounds__(1024) nms_compact_kernel(const NmsArgs p) {
-  __shared__ int s_warp[32];
-  __shared__ int s_run;
-  const int img = blockIdx.x;
-  int c = p.count[img];
-  if (p.overflow && threadIdx.x == 0) p.overflow[img] = c > p.cap ? c : 0;
-  c = c < p.cap ? c : p.cap;
-  const int n = c < p.max_nms ? c : p.max_nms;
-  const uint8_t* keep = p.keep + static_cast<size_t>(img) * kRankCap;
-  const float* det = p.det + static_cast<size_t>(img) * kRankCap * 6;
-  float* out = p.out + static_cast<size_t>(img) * p.max_det * 6;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) s_run = 0;
-  __syncthreads();
-  for (int base = 0; base < n; base += blockDim.x) {
-    const int run = s_run;
-    if (run >= p.max_det) break;
-    const int r = base + threadIdx.x;
-    const int k = (r < n) ? keep[r] : 0;
-    const unsigned bal = __ballot_sync(0xffffffffu, k);
-    if (lane == 0) s_warp[warp] = __popc(bal);
-    __syncthreads();
-    int woff = 0, tot = 0;
-    for (int w = 0; w < 32; ++w) {
-      const int v = s_warp[w];
-      if (w < warp) woff += v;
-      tot += v;
-    }
-    const int pos = run + woff + __popc(bal & ((1u << lane) - 1u));
-    if (k && pos < p.max_det) {
-      const float* d = det + static_cast<size_t>(r) * 6;
-      float* o = out + static_cast<size_t>(pos) * 6;
-#pragma unroll
-      for (int q = 0; q < 6; ++q) o[q] = d[q];
-      if (p.out_src) {
-        const unsigned long long key = p.keys[static_cast<size_t>(img) * p.cap + r];
-        const uint32_t id = 0xFFFFFFFFu - static_cast<uint32_t>(key & 0xFFFFFFFFull);
-        p.out_src[(static_cast<size_t>(img) * p.max_det + pos) * 2 + 0] = id / p.nc;
-        p.out_src[(static_cast<size_t>(img) * p.max_det + pos) * 2 + 1] = id % p.nc;
-      }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) s_run = run + tot;
-    __syncthreads();
-  }
-  const int total = s_run < p.max_det ? s_run : p.max_det;
-  if (threadIdx.x == 0) p.out_count[img] = total;
-  for (int i = total * 6 + threadIdx.x; i < p.max_det * 6; i += blockDim.x) out[i] = 0.f;
-}
-
-// ================================================================================================ v2 pipeline
-// The first version sorted every candidate twice with global bitonic networks (conf, then (class, rank)): ~25 launches, the
-// two sorts most of the time.  Nothing needs a GLOBAL order except
-// the <= max_det rows that are returned, so v2 is:
-//   K1 candidates (unchanged)           keys (conf bits | ~id), unordered, per image
-//   K2 nms_bucket_kernel   1 CTA/image  max_nms cut (exact radix select, only when count > max_nms), xywh -> xyxy, counting
-//                                       sort of the candidates by class (shared-memory histogram + scan + scatter)
-//   K3 nms_seg_mask_kernel 1 CTA/(image,class), <= 128 and <= 512 members: rank the members by key (counting in shared memory),
-//                                       suppression matrix (intersection bits by ballot, exact division-free IoU on the
-//                                       intersecting pairs), one warp resolves the greedy order with bit operations, survivors
-//                                       appended to the image's survivor list
-//      nms_seg_block_kernel             segments > 512 members (multi-label at low conf; agnostic / out-of-range images, whose
-//                                       single segment is ranked by all the image's CTAs and finished by the last one)
-//   K4 nms_output_kernel   1 CTA/image  top max_det survivors by key: shared-memory bitonic sort (<= 4096 survivors) or exact
-//                                       radix select + sort of the selected, rows + (row, class) sources + counts
-// Same exactness contract as v1: all arithmetic in the reference's order, ties broken by candidate id (stable).
+// ================================================================================================ bucket, segments, output
+// No candidate is ever sorted globally: nothing needs a global order except the <= max_det rows that are returned.
+//   nms_bucket_kernel    1 CTA/image  max_nms cut (exact radix select, only when count > max_nms), xywh -> xyxy, counting
+//                                     sort of the candidates by class (shared-memory histogram + scan + scatter)
+//   nms_seg_mask_kernel  1 CTA/(image,class), <= 128 and <= 512 members: rank the members by key (counting in shared memory),
+//                                     suppression matrix (intersection bits by ballot, exact division-free IoU on the
+//                                     intersecting pairs), one warp resolves the greedy order with bit operations, survivors
+//                                     appended to the image's survivor list
+//   nms_seg_block_kernel              segments > 512 members (multi-label at low conf; agnostic / out-of-range images, whose
+//                                     single segment is ranked by all the image's CTAs and finished by the last one)
+//   nms_output_kernel    1 CTA/image  top max_det survivors by key: shared-memory bitonic sort (<= 4096 survivors) or exact
+//                                     radix select + sort of the selected, rows + (row, class) sources + counts
+// All arithmetic in the reference's order, ties broken by candidate id (stable).
 constexpr int kBucketThreads = 1024;
 constexpr int kOutSortMax = 8192;  // survivors sorted in shared memory (64 KB keys + 16 KB positions, dynamic)
 
@@ -1191,10 +832,7 @@ extern "C" int64_t y3_nms_workspace_bytes(int32_t bs, int32_t cap) {
   size_t b = 0;
   b += y3::align_up(sizeof(unsigned long long) * size_t(bs) * cap, 256);
   b += y3::align_up(sizeof(int) * size_t(bs) * 2, 256);
-  b += y3::align_up(sizeof(float) * size_t(bs) * y3::kRankCap * 6, 256);
-  b += y3::align_up(sizeof(uint32_t) * size_t(bs) * y3::kRankCap, 256);
-  b += y3::align_up(size_t(bs) * y3::kRankCap, 256);
-  // v2: seg_off, seg_key2, box4, surv_cnt + done_cnt, surv_key, surv_pos, ord
+  // seg_off, seg_key2, box4, surv_cnt + done_cnt, surv_key, surv_pos, ord
   b += y3::align_up(sizeof(int) * size_t(bs) * 1025, 256);
   b += y3::align_up(sizeof(unsigned long long) * size_t(bs) * y3::kRankCap, 256);
   b += y3::align_up(sizeof(float4) * size_t(bs) * y3::kRankCap, 256);
@@ -1208,8 +846,8 @@ extern "C" int64_t y3_nms_workspace_bytes(int32_t bs, int32_t cap) {
 
 extern "C" int32_t y3_nms_default_capacity(int32_t n_rows, int32_t nc, int32_t multi_label) {
   long long want = multi_label ? 4ll * n_rows : n_rows;  // multi-label: room for 4 labels/row before an exact retry
-  if (want < y3::kSortTile) want = y3::kSortTile;
-  long long cap = y3::kSortTile;
+  if (want < y3::kMinCap) want = y3::kMinCap;
+  long long cap = y3::kMinCap;
   while (cap < want) cap <<= 1;
   (void)nc;
   return static_cast<int32_t>(cap);
@@ -1225,8 +863,7 @@ extern "C" int y3_nms_batched(const float* pred, const y3_nms_params* q, void* w
   Y3_REQUIRE(q->conf_thres >= 0.f && q->conf_thres <= 1.f, "nms: invalid confidence threshold %f", q->conf_thres);
   Y3_REQUIRE(q->iou_thres >= 0.f && q->iou_thres <= 1.f, "nms: invalid IoU threshold %f", q->iou_thres);
   Y3_REQUIRE(q->max_det > 0 && q->max_nms > 0 && q->max_nms <= kRankCap, "nms: max_det/max_nms out of range");
-  Y3_REQUIRE(q->cap >= kSortTile && (q->cap & (q->cap - 1)) == 0, "nms: capacity must be a power of two >= %d",
-             kSortTile);
+  Y3_REQUIRE(q->cap >= kMinCap && (q->cap & (q->cap - 1)) == 0, "nms: capacity must be a power of two >= %d", kMinCap);
   Y3_REQUIRE(static_cast<long long>(q->n_rows) * q->nc < (1ll << 32), "nms: n_rows*nc overflows the candidate id");
   Y3_REQUIRE(workspace_bytes >= y3_nms_workspace_bytes(q->bs, q->cap), "nms: workspace too small");
   Y3_REQUIRE(q->bs <= 65535, "nms: batch too large");
@@ -1264,12 +901,6 @@ extern "C" int y3_nms_batched(const float* pred, const y3_nms_params* q, void* w
   a.count = reinterpret_cast<int*>(w);
   a.flags = a.count + a.bs;
   w += align_up(sizeof(int) * size_t(a.bs) * 2, 256);
-  a.det = reinterpret_cast<float*>(w);
-  w += align_up(sizeof(float) * size_t(a.bs) * kRankCap * 6, 256);
-  a.seg_keys = reinterpret_cast<uint32_t*>(w);
-  w += align_up(sizeof(uint32_t) * size_t(a.bs) * kRankCap, 256);
-  a.keep = w;
-  w += align_up(size_t(a.bs) * kRankCap, 256);
   a.seg_off = reinterpret_cast<int*>(w);
   w += align_up(sizeof(int) * size_t(a.bs) * 1025, 256);
   a.seg_key2 = reinterpret_cast<unsigned long long*>(w);
@@ -1292,61 +923,22 @@ extern "C" int y3_nms_batched(const float* pred, const y3_nms_params* q, void* w
   a.overflow = overflow;
 
   Y3_CHECK_CUDA(cudaMemsetAsync(a.count, 0, sizeof(int) * size_t(a.bs) * 2, stream));
-  // K1
   Y3_CHECK_CUDA(::y3::launch_pdl(nms_candidates_kernel, dim3((a.n_rows + 32 * kCandWarps - 1) / (32 * kCandWarps), a.bs), dim3(32 * kCandWarps), 0, stream, a));
-  static int v1 = -1;  // Y3_NMS_V1=1: the round-1 pipeline (two global bitonic sorts), kept for A/B measurements
-  if (v1 < 0) {
-    const char* e = getenv("Y3_NMS_V1");
-    v1 = (e && e[0] == '1') ? 1 : 0;
-  }
-  if (!v1) {
-    Y3_CHECK_CUDA(::y3::launch_pdl(nms_bucket_kernel, dim3(a.bs), dim3(kBucketThreads), 0, stream, a));
-    // the first matrix kernel (one thread per mask word, full test on all 32 pairs) beat a warp-per-segment kernel only at
-    // <= 128 members per class and lost at a few hundred.  The two-phase pair test (ballot of intersections, exact test on those) is what made the matrix form win there too.
-    if (int rc = launch_seg_mask<kMaskSmall, 128>(a, 0, stream)) return rc;
-    if (int rc = launch_seg_mask<kMaskLarge, 256>(a, kMaskSmall, stream)) return rc;
-    Y3_CHECK_CUDA(::y3::launch_pdl(nms_seg_block_kernel, dim3(a.nc, a.bs), dim3(256), 0, stream, a));
-    {
-      constexpr int kOutSmem = kOutSortMax * (sizeof(unsigned long long) + sizeof(uint16_t));
-      static bool attr_set = false;
-      if (!attr_set) {
-        Y3_CHECK_CUDA(cudaFuncSetAttribute(nms_output_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kOutSmem));
-        attr_set = true;
-      }
-      Y3_CHECK_CUDA(::y3::launch_pdl(nms_output_kernel, dim3(a.bs), dim3(1024), kOutSmem, stream, a));
-    }
-    Y3_CHECK_CUDA(cudaGetLastError());
-    return Y3_OK;
-  }
-  pad_keys_kernel<<<dim3(8, a.bs), 256, 0, stream>>>(a);
-  // K2: sort candidates by confidence (descending)
+  Y3_CHECK_CUDA(::y3::launch_pdl(nms_bucket_kernel, dim3(a.bs), dim3(kBucketThreads), 0, stream, a));
+  // the first matrix kernel (one thread per mask word, full test on all 32 pairs) beat a warp-per-segment kernel only at
+  // <= 128 members per class and lost at a few hundred.  The two-phase pair test (ballot of intersections, exact test on those) is what made the matrix form win there too.
+  if (int rc = launch_seg_mask<kMaskSmall, 128>(a, 0, stream)) return rc;
+  if (int rc = launch_seg_mask<kMaskLarge, 256>(a, kMaskSmall, stream)) return rc;
+  Y3_CHECK_CUDA(::y3::launch_pdl(nms_seg_block_kernel, dim3(a.nc, a.bs), dim3(256), 0, stream, a));
   {
-    using T = unsigned long long;
-    const int tiles = a.cap / kSortTile;
-    bitonic_local_kernel<T, true><<<dim3(tiles, a.bs), 1024, 0, stream>>>(a, a.keys, a.cap, false);
-    for (int k = 2 * kSortTile; k <= a.cap; k <<= 1) {
-      for (int j = k >> 1; j >= kSortTile; j >>= 1)
-        bitonic_global_kernel<T, true><<<dim3(a.cap / 2 / 256, a.bs), 256, 0, stream>>>(a, a.keys, a.cap, false, k, j);
-      bitonic_merge_kernel<T, true><<<dim3(tiles, a.bs), 1024, 0, stream>>>(a, a.keys, a.cap, false, k);
+    constexpr int kOutSmem = kOutSortMax * (sizeof(unsigned long long) + sizeof(uint16_t));
+    static bool attr_set = false;
+    if (!attr_set) {
+      Y3_CHECK_CUDA(cudaFuncSetAttribute(nms_output_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kOutSmem));
+      attr_set = true;
     }
+    Y3_CHECK_CUDA(::y3::launch_pdl(nms_output_kernel, dim3(a.bs), dim3(1024), kOutSmem, stream, a));
   }
-  // K3
-  nms_gather_kernel<<<dim3(kRankCap / 256, a.bs), 256, 0, stream>>>(a);
-  // K4: (class, rank) ascending
-  {
-    using T = uint32_t;
-    const int tiles = kRankCap / kSortTile;
-    bitonic_local_kernel<T, false><<<dim3(tiles, a.bs), 1024, 0, stream>>>(a, a.seg_keys, kRankCap, true);
-    for (int k = 2 * kSortTile; k <= kRankCap; k <<= 1) {
-      for (int j = k >> 1; j >= kSortTile; j >>= 1)
-        bitonic_global_kernel<T, false><<<dim3(kRankCap / 2 / 256, a.bs), 256, 0, stream>>>(a, a.seg_keys, kRankCap, true, k, j);
-      bitonic_merge_kernel<T, false><<<dim3(tiles, a.bs), 1024, 0, stream>>>(a, a.seg_keys, kRankCap, true, k);
-    }
-  }
-  // K5, K6
-  nms_segments_warp_kernel<<<dim3((a.nc + 7) / 8, a.bs), 256, 0, stream>>>(a);
-  nms_segments_kernel<<<dim3(a.nc, a.bs), 256, 0, stream>>>(a);
-  nms_compact_kernel<<<a.bs, 1024, 0, stream>>>(a);
   Y3_CHECK_CUDA(cudaGetLastError());
   return Y3_OK;
 }

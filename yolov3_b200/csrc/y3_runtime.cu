@@ -97,7 +97,7 @@ int encode_tensor_map(CUtensorMap* out, int fmt, const void* base, int rank, con
 
 }  // namespace y3
 
-extern "C" int y3_version(void) { return 100; }
+extern "C" int y3_version(void) { return 101; }
 
 extern "C" int y3_last_error(char* buf, size_t n) {
   const size_t len = strlen(y3::g_err);

@@ -5,16 +5,16 @@
 //   bn_stats        per-channel sum / sum of squares of the conv output y (padded NHWC bf16; the zero halo adds nothing)
 //   bn_finalize     batch mean/var -> (scale, shift), saved (mean, rstd), running-stat update (unbiased var, momentum)
 //   bn_act_fwd      a = SiLU(y*scale + shift) (+ residual), optional nearest-2x store / concat-offset store
-//   bn_act_bwd_red  dz = da * SiLU'(z);  per-channel sum(dz), sum(dz * yhat)          (dgamma, dbeta)
-//   bn_act_bwd      dy = scale * (dz - mean(dz) - yhat * mean(dz*yhat))               (input of dgrad / wgrad)
+//   bn_act_bwd      reduce pass: dz = da * SiLU'(z);  per-channel sum(dz), sum(dz * yhat)          (dgamma, dbeta)
+//                   apply pass:  dy = scale * (dz - mean(dz) - yhat * mean(dz*yhat))               (input of dgrad / wgrad)
+//                   through a per-thread cp.async shared-memory ring; the 2x-upsample layers sum four da replicas per
+//                   item in registers instead
 //   pack_weights    fp32 master weights [co,ci,k,k] -> bf16 forward pack [co_pad, tap*ci+c] and dgrad pack
 //                   [ci_pad, tap'*co+o] (taps flipped), every optimizer step
 //   zero_stuff      dy of a stride-2 conv scattered onto the even positions of a zero 2x grid (its dgrad is then a
 //                   stride-1 conv with flipped weights)
 //   wgrad           dW[co, tap, ci] = sum_p dy[p, co] * x[p + shift(tap), ci]  (warp-level bf16 MMA, split over pixels)
 //   bias_grad       Detect heads: db[co] = sum_p dy[p, co]
-#include <cstdlib>
-
 #include "y3_common.cuh"
 #include "y3_internal.h"
 
@@ -295,8 +295,9 @@ __device__ __forceinline__ float silu_grad(float z) {
   return s * fmaf(z, 1.0f - s, 1.0f);
 }
 
-template <bool APPLY, bool UPS>
-__global__ void __launch_bounds__(256, UPS ? 2 : 3) bn_act_bwd_kernel(const BnBwdArgs p) {
+// the reduce / apply passes of the 2x-upsample layers: a unit's 16-byte vectors stay in registers between issue and use
+template <bool APPLY>
+__global__ void __launch_bounds__(256, 2) bn_act_bwd_ups_kernel(const BnBwdArgs p) {
   pdl_entry();
   // block = 256 threads; thread t keeps channel group t % c8 for the whole kernel (256 % c8 == 0)
   extern __shared__ float sh[];
@@ -324,25 +325,20 @@ __global__ void __launch_bounds__(256, UPS ? 2 : 3) bn_act_bwd_kernel(const BnBw
     const int r = u / g.upr, e0 = (u - r * g.upr) * (256 * kUnitIters) + threadIdx.x;
     const long long rb = row_base(g, r);
     const long long ub = p.upsample ? row_base(g, r, 2) : rb;
-    // raw 16-byte vectors stay packed until they are consumed (registers: the reduction pass keeps 48 per-channel values);
-    // only the 2x-upsample variant (2 layers) sums its four da replicas right away
-    uint4 vy[kUnitIters], vd[kUnitIters];
-    float du[UPS ? kUnitIters : 1][8];
+    // raw y vectors stay packed until they are consumed (registers: the reduction pass keeps 48 per-channel values); the
+    // four da replicas are summed right away
+    uint4 vy[kUnitIters];
+    float du[kUnitIters][8];
 #pragma unroll
     for (int k = 0; k < kUnitIters; ++k) {
       const int e = e0 + k * 256;
       const int x = g.c8_shift >= 0 ? e >> g.c8_shift : e / g.c8;  // cg is loop-invariant: 256 % c8 == 0
-      vy[k] = vd[k] = make_uint4(0, 0, 0, 0);  // dz = 0 beyond the row: adds nothing to the sums
-      if (UPS) {
+      vy[k] = make_uint4(0, 0, 0, 0);  // dz = 0 beyond the row: adds nothing to the sums
 #pragma unroll
-        for (int q = 0; q < 8; ++q) du[UPS ? k : 0][q] = 0.f;
-      }
+      for (int q = 0; q < 8; ++q) du[k][q] = 0.f;
       if (e < items) {
         vy[k] = __ldg(reinterpret_cast<const uint4*>(p.y.p + (rb + x) * p.y.ld + p.y.coff + cg * 8));
-        if (UPS)
-          load_da(p, rb, ub, x, cg, du[UPS ? k : 0]);
-        else
-          vd[k] = __ldg(reinterpret_cast<const uint4*>(p.da.p + (rb + x) * p.da.ld + p.da.coff + cg * 8));
+        load_da(p, rb, ub, x, cg, du[k]);
       }
     }
 #pragma unroll
@@ -351,12 +347,8 @@ __global__ void __launch_bounds__(256, UPS ? 2 : 3) bn_act_bwd_kernel(const BnBw
       const int x = g.c8_shift >= 0 ? e >> g.c8_shift : e / g.c8;
       float yv[8], d[8], o[8];
       unpack8(vy[k], yv);
-      if (UPS) {
 #pragma unroll
-        for (int q = 0; q < 8; ++q) d[q] = du[UPS ? k : 0][q];
-      } else {
-        unpack8(vd[k], d);
-      }
+      for (int q = 0; q < 8; ++q) d[q] = du[k][q];
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
         const float z = fmaf(yv[q], sc[q], shf[q]);
@@ -376,17 +368,15 @@ __global__ void __launch_bounds__(256, UPS ? 2 : 3) bn_act_bwd_kernel(const BnBw
     block_reduce_store(a_dz, a_dzy, g.c8, sh, p.partial + static_cast<long long>(blockIdx.x) * 2 * g.c8 * 8, g.c8 * 8);
 }
 
-// ---------------------------------------------------------------------------------------------- cp.async ring variant
-// bn_act_bwd_kernel keeps a unit's 16-byte vectors in registers between issue and use: 4 loads per thread in flight, three
-// blocks per SM, a bubble at every unit boundary, long-scoreboard stalls on top; a
-// register look-ahead halved the resident blocks and gained nothing.  The variant below stages
-// the SAME units through a per-thread shared-memory ring with cp.async: a thread copies its own 16-byte items kRingDepth-1
-// units ahead into its own slots and reads them back itself, so there is no barrier and no mbarrier anywhere
-// (cp.async.wait_group cannot dead-lock) and 144 KB per SM are in flight without costing registers.  Unit order, item order
-// and operations are exactly those of bn_act_bwd_kernel: results are bit-identical (A/B script: tests/diag/ab_shot.py).
-// The same ring under bn_stats gained nothing and under bn_act_fwd lost (three 64 KB blocks per SM instead of five or six
-// register-only ones): those two were removed again — the passes are bound by resident warps x issue, not by bytes in flight.
-// Switch: y3_set_bn_async / Y3_BN_ASYNC (default on).
+// ---------------------------------------------------------------------------------------------- cp.async ring
+// Keeping a unit's 16-byte vectors in registers between issue and use (as bn_act_bwd_ups_kernel does) leaves, at three
+// blocks per SM, 4 loads per thread in flight, a bubble at every unit boundary and long-scoreboard stalls on top; a register
+// look-ahead halves the resident blocks and gains nothing.  The non-upsample passes therefore stage their units through a
+// per-thread shared-memory ring with cp.async: a thread copies its own 16-byte items kRingDepth-1 units ahead into its own
+// slots and reads them back itself, so there is no barrier and no mbarrier anywhere (cp.async.wait_group cannot dead-lock)
+// and 144 KB per SM are in flight without costing registers.
+// The same ring under bn_stats gains nothing and under bn_act_fwd loses (three 64 KB blocks per SM instead of five or six
+// register-only ones): those passes are bound by resident warps x issue, not by bytes in flight.
 __device__ __forceinline__ void cp_async16(uint32_t saddr, const void* gptr) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(gptr) : "memory");
 }
@@ -433,7 +423,7 @@ __device__ __forceinline__ void ring_issue(const Rows& g, const Slice& t, int s,
   }
 }
 
-// the non-upsample reduce / apply passes (the two 2x-upsample layers stay on bn_act_bwd_kernel<*, true>)
+// the non-upsample reduce / apply passes (the 2x-upsample layers run bn_act_bwd_ups_kernel)
 template <bool APPLY>
 __global__ void __launch_bounds__(256, 3) bn_act_bwd_async_kernel(const BnBwdArgs p) {
   pdl_entry();
@@ -444,7 +434,7 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_async_kernel(const BnBwdArg
   const int cg = threadIdx.x % g.c8;  // fixed per thread: 256 % c8 == 0
   const int items = g.w * g.c8, nb = units_of_block(g);
   float a_dz[8] = {0, 0, 0, 0, 0, 0, 0, 0}, a_dzy[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  float sc[8], shf[8], c2[8], c3[8];  // as in bn_act_bwd_kernel
+  float sc[8], shf[8], c2[8], c3[8];  // as in bn_act_bwd_ups_kernel
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     sc[k] = p.scale[cg * 8 + k];
@@ -874,14 +864,6 @@ Rows make_rows(int n, int h, int w, int c) {
   g.upr = (w * g.c8 + 256 * kUnitIters - 1) / (256 * kUnitIters);
   return g;
 }
-int g_bn_async = -1;
-int bn_async_enabled() {
-  if (g_bn_async < 0) {
-    const char* e = getenv("Y3_BN_ASYNC");
-    g_bn_async = e ? (e[0] != '0') : Y3_BN_ASYNC_DEFAULT;
-  }
-  return g_bn_async;
-}
 // ring kernels: opt in to > 48 KB of dynamic shared memory and ask for the largest shared-memory carve-out, so that three
 // 64 KB blocks are resident per SM (both attributes are idempotent; the carve-out is a hint)
 template <auto Kern>
@@ -913,12 +895,6 @@ __global__ void __launch_bounds__(1024) bn_bwd_finalize_kernel(const float* __re
 }
 }  // namespace
 }  // namespace y3
-
-extern "C" int y3_set_bn_async(int32_t on) {
-  const int prev = y3::bn_async_enabled();
-  y3::g_bn_async = on ? 1 : 0;
-  return prev;
-}
 
 extern "C" int32_t y3_bn_partial_blocks(int32_t n, int32_t h, int32_t w, int32_t c) {
   // work units of the streaming kernels (c == 0: one unit per image row, the Detect-head gradient pack), capped
@@ -995,28 +971,25 @@ extern "C" int y3_bn_act_bwd(const y3_bn_bwd_desc* d, y3_stream_t stream_) {
   const long long pixels = static_cast<long long>(d->n) * d->h * d->w;
   a.inv_count = 1.0f / (d->count > 0.f ? d->count : static_cast<float>(pixels));
   const int nblk = y3_bn_partial_blocks(d->n, d->h, d->w, d->c);
-  const bool async = y3::bn_async_enabled() != 0;
   if (d->phase != 2) {
-    if (d->upsample)
-      Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_kernel<false, true>, dim3(nblk), dim3(256), 2 * 256 * 8 * sizeof(float), stream, a));
-    else if (async) {
+    if (d->upsample) {
+      Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_ups_kernel<false>, dim3(nblk), dim3(256), 2 * 256 * 8 * sizeof(float), stream, a));
+    } else {
       Y3_CHECK_CUDA(y3::allow_smem<y3::bn_act_bwd_async_kernel<false>>(y3::ring_bytes<2>()));
       Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_async_kernel<false>, dim3(nblk), dim3(256), y3::ring_bytes<2>(), stream, a));
-    } else
-      Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_kernel<false, false>, dim3(nblk), dim3(256), 2 * 256 * 8 * sizeof(float), stream, a));
+    }
     Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_bwd_finalize_kernel, dim3((2 * d->c + 31) / 32), dim3(32, 32), 0, stream, d->partial, nblk, d->c, d->sums, d->dbeta_acc,
                                                                                   d->dgamma_acc));
   }
   if (d->phase != 1) {
     const long long units = static_cast<long long>(d->n) * d->h * a.g.upr;
     const long long cap = 3ll * y3::num_sms();  // one wave at the kernel's 3 resident blocks per SM
-    if (d->upsample)
-      Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_kernel<true, true>, dim3(static_cast<unsigned>(units < cap ? units : cap)), dim3(256), 0, stream, a));
-    else if (async) {
+    if (d->upsample) {
+      Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_ups_kernel<true>, dim3(static_cast<unsigned>(units < cap ? units : cap)), dim3(256), 0, stream, a));
+    } else {
       Y3_CHECK_CUDA(y3::allow_smem<y3::bn_act_bwd_async_kernel<true>>(y3::ring_bytes<2>()));
       Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_async_kernel<true>, dim3(static_cast<unsigned>(units < cap ? units : cap)), dim3(256), y3::ring_bytes<2>(), stream, a));
-    } else
-      Y3_CHECK_CUDA(::y3::launch_pdl(y3::bn_act_bwd_kernel<true, false>, dim3(static_cast<unsigned>(units < cap ? units : cap)), dim3(256), 0, stream, a));
+    }
   }
   Y3_CHECK_CUDA(cudaGetLastError());
   return Y3_OK;
@@ -1073,10 +1046,10 @@ extern "C" int y3_conv_wgrad(const y3_wgrad_desc* d, y3_stream_t stream) {
   Y3_REQUIRE(d->co % 8 == 0 && d->ci % 8 == 0 && (d->ksize == 1 || d->ksize == 3) && d->n > 0 && d->h > 0 && d->w > 0,
              "wgrad: c_out/c_in must be multiples of 8 (got %d/%d), ksize 1|3", d->co, d->ci);
   Y3_REQUIRE(d->dy_ld % 8 == 0 && d->dy_coff % 8 == 0 && d->x_ld % 8 == 0 && d->x_coff % 8 == 0, "wgrad: bad slices");
-  Y3_REQUIRE(d->stride == 0 || d->stride == 1 || (d->stride == 2 && y3::wgrad_tc_enabled() && d->ci % 32 == 0),
+  Y3_REQUIRE(d->stride == 0 || d->stride == 1 || (d->stride == 2 && d->ci % 32 == 0),
              "wgrad: stride must be 1, or 2 with the tensor-core kernel (c_in % 32 == 0)");
   // wgmma kernel (csrc/y3_wgrad_tc.cu) whenever its tiling fits; the warp-level MMA kernel below otherwise
-  if (y3::wgrad_tc_enabled() && d->ci % 32 == 0 && (reinterpret_cast<uintptr_t>(d->dy) & 15) == 0 &&
+  if (d->ci % 32 == 0 && (reinterpret_cast<uintptr_t>(d->dy) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(d->x) & 15) == 0)
     return y3::wgrad_tc(*d, static_cast<cudaStream_t>(stream));
   Y3_REQUIRE(d->dw_layout == Y3_DW_OIHW || d->dw_layout == Y3_DW_OHWI,
@@ -1109,9 +1082,9 @@ extern "C" int y3_conv_wgrad(const y3_wgrad_desc* d, y3_stream_t stream) {
   return Y3_OK;
 }
 
-extern "C" int y3_conv_wgrad_s2_supported(int32_t h, int32_t w) { return y3::wgrad_tc_enabled() ? y3::wgrad_tc_s2_supported(h, w) : 0; }
+extern "C" int y3_conv_wgrad_s2_supported(int32_t h, int32_t w) { return y3::wgrad_tc_s2_supported(h, w); }
 
-extern "C" int y3_conv_wgrad_tap_major(int32_t c_in) { return (y3::wgrad_tc_enabled() && c_in % 32 == 0) ? 1 : 0; }
+extern "C" int y3_conv_wgrad_tap_major(int32_t c_in) { return c_in % 32 == 0 ? 1 : 0; }
 
 extern "C" int y3_colsum_f32(const float* g, int32_t ld, int32_t c, int64_t rows, float* out, y3_stream_t stream) {
   Y3_REQUIRE(g && out && c > 0 && c <= 256 && rows > 0, "colsum: bad arguments");

@@ -11,8 +11,6 @@
 // (reference: autograd of Conv.forward, models/common.py:71-75).
 #include <cuda_bf16.h>
 
-#include <cstdlib>
-
 #include "y3_common.cuh"
 #include "y3_internal.h"
 
@@ -49,7 +47,7 @@ struct WgCfg {
   static_assert(kStages >= 2, "wgrad: the ring needs two stages");
 };
 
-// N = ci tile width (32 .. 256); KB = pixels per K block
+// N = ci tile width (32 .. 128); KB = pixels per K block
 template <int N, int KB>
 __global__ void __launch_bounds__(kWgThreads, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constant__ CUtensorMap map_x, const WgTcArgs p) {
@@ -198,16 +196,6 @@ int wgrad_tc_launch(const CUtensorMap& mdy, const CUtensorMap& mx, const WgTcArg
 
 }  // namespace
 
-// Y3_WGRAD_TC=0 keeps the warp-level MMA kernel.
-int wgrad_tc_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("Y3_WGRAD_TC");
-    v = (e && e[0] == '0') ? 0 : 1;
-  }
-  return v;
-}
-
 // (tw, th) with tw * th == 80, tw | wo, th | ho for the stride-2 patch mode; false: no such tiling (caller zero-stuffs)
 static bool s2_patch(int ho, int wo, int* tw, int* th) {
   for (int cand_th = 1; cand_th <= 80; ++cand_th) {
@@ -302,12 +290,7 @@ int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream) {
   const int taps = d.ksize * d.ksize;
   const long long rows = static_cast<long long>(d.n) * (d.h + 2) * (d.w + 2);
   Y3_REQUIRE(rows < (1ll << 31) - 4096, "wgrad: too many pixels");
-  static int n_max = -1;  // Y3_WGRAD_NMAX=256 allows 256-wide ci tiles; default 128
-  if (n_max < 0) {
-    const char* e = getenv("Y3_WGRAD_NMAX");
-    n_max = (e && atoi(e) == 256) ? 256 : 128;
-  }
-  const int n_tile = (d.ci >= 256 && n_max == 256) ? 256 : (d.ci >= 128 ? 128 : (d.ci >= 64 ? 64 : 32));
+  const int n_tile = d.ci >= 128 ? 128 : (d.ci >= 64 ? 64 : 32);
   Y3_REQUIRE(d.ci % 32 == 0 || d.ci < 32, "wgrad_tc: c_in=%d must be a multiple of 32", d.ci);
   CUtensorMap mdy, mx;
   {
@@ -354,7 +337,6 @@ int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream) {
   a.single = (splits == 1 && !d.accumulate) ? 1 : 0;
   const dim3 grid(splits, static_cast<unsigned>(tiles), static_cast<unsigned>(taps));
   switch (n_tile) {
-    case 256: return wgrad_tc_launch<256, kWgK>(mdy, mx, a, grid, stream);
     case 128: return wgrad_tc_launch<128, kWgK>(mdy, mx, a, grid, stream);
     case 64: return wgrad_tc_launch<64, kWgK>(mdy, mx, a, grid, stream);
     default: return wgrad_tc_launch<32, kWgK>(mdy, mx, a, grid, stream);

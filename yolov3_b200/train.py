@@ -50,7 +50,6 @@ class TrainEngine:
     use_graphs = True        # replay forward / backward segments as CUDA graphs after one eager warm-up step
     deterministic = False    # True: wgrad without split-K (bit-reproducible steps; slower on the early layers)
     n_buckets = 4            # gradient ranges all-reduced separately, each as soon as its layers are done
-    dgrad_phases = True      # stride-2 dgrad as four parity-class convs of the un-stuffed dy (False: conv of the zero-stuffed dy)
 
     def __init__(self, model, n, h, w, keep_all=False):
         """keep_all=True gives every block its own dy buffer (per-layer gradient checks in the tests); the default shares
@@ -496,14 +495,12 @@ class TrainEngine:
                              count=self.n * b.y.h * b.y.w * self.world)
             else:
                 T.bn_act_bwd(b.y, da, b.dy, st, st["sums"], self.partial, b.dbeta, b.dgamma, b.upsample)
-            src = b.dy
-            direct_w = b.s == 2 and T.wgrad_s2_supported(b.x.h, b.x.w)
-            if b.s == 2 and not (direct_w and self.dgrad_phases):
-                src = T.zero_stuff(b.dy, b.dy_up)  # fallback: stride-1 formulations on the zero-stuffed dy
-            if direct_w:
+            if b.s == 2 and T.wgrad_s2_supported(b.x.h, b.x.w):
                 # wgrad straight from the un-stuffed dy (x through its parity view): a quarter of the pixels, no zeros multiplied
                 T.conv_wgrad(b.dy, b.x, b.dw, b.k, layout=_lib.DW_OHWI, accumulate=True, deterministic=det_flag, stride=2)
             else:
+                # a stride-2 input the direct form cannot tile: stride-1 wgrad on the zero-stuffed dy
+                src = T.zero_stuff(b.dy, b.dy_up) if b.s == 2 else b.dy
                 T.conv_wgrad(src, b.x, b.dw, b.k, layout=_lib.DW_OHWI, accumulate=True, deterministic=det_flag)
             if b.res is not None:
                 # Bottleneck shortcut: the block output's gradient also flows to its input.  It is folded into the next
@@ -516,11 +513,8 @@ class TrainEngine:
                 self._pending_add[key] = (da, r)
             if not b.first:
                 key = (b.x.buf.data_ptr(), b.x.coff, b.x.c)
-                if b.s == 2 and self.dgrad_phases:
-                    # transposed stride-2 conv by parity classes on the un-stuffed dy (4 launches, a quarter of the MMA work)
-                    self._contribute_conv(b.dy, b.wd, b.c1, b.k, b.x, s2=True)
-                else:
-                    self._contribute_conv(src, b.wd, b.c1, b.k, b.x)
+                # stride 2: transposed conv by parity classes on the un-stuffed dy (4 launches, a quarter of the MMA work)
+                self._contribute_conv(b.dy, b.wd, b.c1, b.k, b.x, s2=b.s == 2)
                 self._pending_add.pop(key, None)
         self._flush_pending()  # a segment is one CUDA graph: nothing may stay pending across its end
         return None
