@@ -20,9 +20,15 @@
 //      write the bf16 pairs back into the same words, arrive on `done` and go straight on to the next tile's MMAs;
 //   3. drain: the store warp waits on `done` and writes the tile out with 16-byte stores (halo and out-of-range rows
 //      skipped, concat offset, nearest-2x upsample), then stages the next tile into the same buffer.
-// The fp32 Detect-head launches (a 128 x 256 fp32 tile does not fit beside the ring) and the N <= 128 launches (Cfg::kStaged)
-// store straight from the consumers' registers.  While the consumers finish a tile the producer
-// already fills the ring for their next one.
+// N <= 128 launches with a bf16 / e4m3 output (Cfg::kPair, ConvTcArgs::tile_tma) run the same three steps with TWO tile
+// buffers in the swizzled layout of their TMA maps, and the store warp's lane 0 moves whole tiles with the bulk-copy engine:
+// it loads tile i's residual into buffer i & 1 by TMA (one tile ahead), the consumers finish the tile in place and fence
+// it for the async proxy, and the store warp writes it out with one TMA store per 128-byte-wide box (the maps clip pixels
+// outside the output and channels past c_out; flat-mode halo rows carry zeros), then restages the buffer for tile i + 2
+// once that store has read it.
+// The fp32 Detect-head launches (a 128 x 256 fp32 tile does not fit beside the ring), the upsampling launches (a 2 x 2
+// replicated write is not one box) and the parity classes of the transposed stride-2 conv store straight from the
+// consumers' registers.  While the consumers finish a tile the producer already fills the ring for their next one.
 // FP8 (IN_FMT / OUT_FMT = Y3_FMT_E4M3): an e4m3 k-block of 2 * BLOCK_K channels has the byte geometry of a bf16 k-block of
 // BLOCK_K channels (same swizzled rows, descriptors and halo offsets) and one k32 e4m3 wgmma consumes the 32 bytes of one
 // k16 bf16 step, so ring, halo / patch modes and the producer's addressing are shared; BLOCK_K counts bf16-equivalent
@@ -64,13 +70,23 @@ struct Cfg {
   static constexpr uint32_t kBBytes = BLOCK_N * BLOCK_K * 2;
   static constexpr uint32_t kStageBytes = kABytes + kTaps * kBBytes;
   static constexpr int kMaxStages = 8;
+  static constexpr uint32_t kBarBytes = 256;  // mbarriers
   // N = 256 bf16-output launches hand the finished tile to the store warp: they keep the output tile (128 x BLOCK_N bf16)
   // and the tile's BLOCK_N bias floats beside the ring, and those bytes come out of the ring's budget (`reserve`).
-  // Thinner tiles run only a few microseconds each: one warp cannot drain and restage them in that time, and their
-  // epilogue from the registers (batched bias and residual loads) costs less than the store warp's turn-around.
+  // Thinner tiles run only a few microseconds each: one warp's 16-byte copies cannot drain and restage them in that time,
+  // so they use two buffers and the bulk-copy engine instead (kPair below).
   static constexpr bool kStaged = BLOCK_N == 256 && STAGE_ES > 0;
   static constexpr uint32_t kTileBytes = kBlockM * BLOCK_N * (STAGE_ES > 0 ? STAGE_ES : 2);
   static constexpr uint32_t kOutBytes = kTileBytes + BLOCK_N * 4 * (STAGE_DQ ? 2 : 1);
+  // N <= 128 launches whose tile leaves by TMA (ConvTcArgs::tile_tma) keep two output tiles, 1 KB aligned after the
+  // barriers, in the TMA maps' swizzled layout: each row is split into boxes of kBoxBytes (at most 128, the widest
+  // swizzle), box k of all 128 rows is one region of 128 x kBoxBytes, and 16-byte chunk c of row m sits at chunk
+  // c ^ ((m * kBoxBytes / 128) mod (kBoxBytes / 16)) of that row (the TMA swizzle of that width)
+  static constexpr bool kPair = BLOCK_N <= 128 && STAGE_ES > 0;
+  static constexpr uint32_t kRowBytes = BLOCK_N * (STAGE_ES > 0 ? STAGE_ES : 2);
+  static constexpr uint32_t kBoxBytes = kRowBytes < 128 ? kRowBytes : 128;
+  static constexpr uint32_t kBoxes = kRowBytes / kBoxBytes;
+  static constexpr uint32_t kPairBytes = 1024 - kBarBytes + 2 * kTileBytes;
   __host__ __device__ static constexpr int ring_stages(uint32_t reserve) {
     const int s = int(kSmemBudget - reserve) / int(kStageBytes);
     return s > kMaxStages ? kMaxStages : s;
@@ -83,18 +99,18 @@ struct Cfg {
   }
   static constexpr uint32_t kSwizzleBytes = BLOCK_K * 2;  // 32 / 64 / 128: one smem row of an operand tile
   static constexpr uint32_t kSbo = 8 * kSwizzleBytes;
-  static constexpr uint32_t kBarBytes = 256;              // mbarriers
   // Shared-memory layout from the 1 KB-aligned base, as conv_tc_kernel lays it out: A ring, then B ring or resident
-  // weights, then the mbarriers (bar_offset), then the output tile and the bias (kStaged bf16-output launches).  launch_cfg
-  // checks smem_end() against the allocation before every launch.
+  // weights, then the mbarriers (bar_offset), then `reserve` bytes: the output tile and the bias (kStaged launches,
+  // kOutBytes) or the two TMA output tiles (kPairBytes).  launch_cfg checks smem_end() against the allocation before
+  // every launch.
   __host__ __device__ static constexpr uint32_t bar_offset(int stages, bool bres, int b_steps) {
     return uint32_t(stages) * kABytes + (bres ? bres_bytes(b_steps) : uint32_t(stages) * kTaps * kBBytes);
   }
-  __host__ __device__ static constexpr uint32_t smem_end(int stages, bool bres, int b_steps, bool out_tile) {
-    return bar_offset(stages, bres, b_steps) + kBarBytes + (out_tile ? kOutBytes : 0u);
+  __host__ __device__ static constexpr uint32_t smem_end(int stages, bool bres, int b_steps, uint32_t reserve) {
+    return bar_offset(stages, bres, b_steps) + kBarBytes + reserve;
   }
   static constexpr size_t kSmemBytes = size_t(kSmemBudget) + 1024 /*align*/ + kBarBytes;
-  static_assert(ring_stages(kStaged ? kOutBytes : 0u) >= 2, "pipeline needs at least two stages");
+  static_assert(ring_stages(kStaged ? kOutBytes : (kPair ? kPairBytes : 0u)) >= 2, "pipeline needs at least two stages");
   static_assert(!HALO || BLOCK_K >= 32, "halo reuse: rows of 64 or 128 bytes");
 };
 
@@ -185,7 +201,8 @@ __device__ __forceinline__ RowOut row_out(const ConvTcArgs& p, int mt, int n0, i
 
 template <int BLOCK_N, int BLOCK_K, bool HALO, int IN_FMT = Y3_FMT_BF16, int OUT_FMT = Y3_FMT_BF16>
 __global__ void __launch_bounds__(kThreads, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, const ConvTcArgs p) {
+conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
+               const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_res, const ConvTcArgs p) {
   constexpr bool kInE4m3 = IN_FMT == Y3_FMT_E4M3, kOutE4m3 = OUT_FMT == Y3_FMT_E4M3;
   using C = Cfg<BLOCK_N, BLOCK_K, HALO, kOutE4m3 ? 1 : (kInE4m3 ? 0 : 2), kInE4m3 && kOutE4m3>;
   constexpr int kOes = kOutE4m3 ? 1 : 2;  // bytes per output / residual element
@@ -204,8 +221,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + (bres ? C::bres_bytes(b_steps) : uint32_t(STAGES) * kBStage));
   uint64_t* empty_bar = full_bar + C::kMaxStages;
   uint64_t* bres_bar = empty_bar + C::kMaxStages;
-  uint64_t* staged_bar = bres_bar + 1;  // store warp -> consumers: the tile's residual and bias are in shared memory
-  uint64_t* done_bar = bres_bar + 2;    // consumers -> store warp: the finished tile is in shared memory
+  // [b]: output tile buffer b (kPair launches use two, kStaged launches buffer 0)
+  uint64_t* staged_bar = bres_bar + 1;  // store warp -> consumers: the tile's residual (and bias) are in shared memory
+  uint64_t* done_bar = bres_bar + 3;    // consumers -> store warp: the finished tile is in shared memory
   // output tile: word (h * BLOCK_N / 8 + j) * 256 + t holds consumer thread t's column pair j of its row m0 + 8 h (the
   // residual pair before the consumers finish the tile, the output pair after).  Lanes 4 r .. 4 r + 3 of a consumer warp
   // hold 8 consecutive columns of one row, so 16 bytes at word (h * BLOCK_N / 8 + j) * 256 + 32 w + 4 r are 8 channels of
@@ -214,6 +232,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   float* sbias = reinterpret_cast<float*>(stile + C::kTileBytes / 4);
   float* sdq = sbias + BLOCK_N;  // e4m3 input (Cfg STAGE_DQ)
   const bool staged_out = C::kStaged && p.out_f32 == nullptr;
+  // two output tiles (Cfg::kPair), 1 KB aligned for the 128-byte swizzle
+  uint8_t* ptile = reinterpret_cast<uint8_t*>(full_bar) + 1024;
+  const bool pair_out = C::kPair && p.tile_tma != 0;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -221,13 +242,20 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
+    if (pair_out) {
+      tma_prefetch_desc(&map_out);
+      if (p.res) tma_prefetch_desc(&map_res);
+    }
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
     }
     mbar_init(bres_bar, 1);
-    mbar_init(staged_bar, 32);  // every store-warp lane, after its own copies have landed
-    mbar_init(done_bar, 8);     // one arrival per consumer warp
+    for (int b = 0; b < 2; ++b) {
+      // kStaged: every store-warp lane, after its own copies have landed; kPair: the store warp's one TMA issuing lane
+      mbar_init(&staged_bar[b], pair_out ? 1 : 32);
+      mbar_init(&done_bar[b], 8);  // one arrival per consumer warp
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -324,7 +352,63 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     else
       run(std::integral_constant<int, 1>{});
   } else if (warp == kStoreWarp) {
-    // ------------------------------------------------------------------ store warp (N = 256 bf16-output launches)
+    // ------------------------------------------------------------------ store warp
+    if (pair_out) {
+      // N <= 128 (kPair): lane 0 moves whole tiles with the bulk-copy engine.  Tile i of this CTA uses buffer i & 1: its
+      // residual is loaded while the consumers run tile i - 1 or i - 2, and the buffer is restaged for tile i + 2 as soon
+      // as tile i's store has finished reading it.  With res == out (training dgrad) a tile's residual is loaded before
+      // that tile is stored, and tiles are disjoint.
+      if (lane != 0) return;
+      const uint32_t res_tx = uint32_t(p.mode == 0 ? kBlockM : p.tw * p.th) * C::kRowBytes;  // out-of-range parts count
+      constexpr int kBoxCh = C::kBoxBytes / kOes;
+      // load (residual) or store (output) the boxes of `tile` from / to buffer b
+      auto move = [&](int tile, int b, bool load) {
+        const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BLOCK_N;
+        int c1 = mt * kBlockM, c2 = 0, c3 = 0;  // flat: first pixel row; patch: (ow0, oh0, img) of the interior view
+        if (p.mode != 0) {
+          const int per_img = p.tiles_w * p.tiles_h;
+          c3 = mt / per_img;
+          const int t = mt - c3 * per_img;
+          c1 = (t % p.tiles_w) * p.tw;
+          c2 = (t / p.tiles_w) * p.th;
+        }
+#pragma unroll
+        for (uint32_t k = 0; k < C::kBoxes; ++k) {
+          uint8_t* s = ptile + b * C::kTileBytes + k * kBlockM * C::kBoxBytes;
+          const int c0 = (load ? p.res_coff : p.out_coff) + n0 + int(k) * kBoxCh;
+          if (load) {
+            if (p.mode == 0) tma_load_2d(s, &map_res, &staged_bar[b], c0, c1);
+            else tma_load_4d(s, &map_res, &staged_bar[b], c0, c1, c2, c3);
+          } else {
+            if (p.mode == 0) tma_store_2d(&map_out, s, c0, c1);
+            else tma_store_4d(&map_out, s, c0, c1, c2, c3);
+          }
+        }
+      };
+      auto stage = [&](int tile, int b) {
+        if (p.res) {
+          mbar_expect_tx(&staged_bar[b], res_tx);
+          move(tile, b, true);
+        } else {
+          mbar_arrive(&staged_bar[b]);
+        }
+      };
+      const int step = int(gridDim.x);
+      if (int(blockIdx.x) < total_tiles) stage(blockIdx.x, 0);
+      if (int(blockIdx.x) + step < total_tiles) stage(blockIdx.x + step, 1);
+      for (int tile = blockIdx.x, i = 0; tile < total_tiles; tile += step, ++i) {
+        const int b = i & 1;
+        mbar_wait(&done_bar[b], uint32_t(i >> 1) & 1u, p.err, 9);  // the consumers have finished tile i in buffer b
+        move(tile, b, false);
+        bulk_commit_group();
+        if (tile + 2 * step < total_tiles) {
+          bulk_wait_read_all();  // the store has read buffer b
+          stage(tile + 2 * step, b);
+        }
+      }
+      bulk_wait_all();  // the output is in global memory before the grid completes (the next grid's griddepcontrol.wait)
+      return;
+    }
     if (!staged_out) return;
     // lane = 8 c + r: row r of 8 rows of one consumer warp's block, chunk c of 4 consecutive 16-byte chunks.  Each quarter
     // warp reads 128 contiguous bytes of the tile (no bank conflict) and each row gets a 64-byte global segment.
@@ -433,7 +517,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     const uint32_t b_base = smem_u32(smem_b);
     uint32_t stage = 0, phase = 0, tphase = 0;
     if (bres && int(blockIdx.x) < total_tiles) mbar_wait(bres_bar, 0, p.err, 6);  // resident weights have landed
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    for (int tile = blockIdx.x, ti = 0; tile < total_tiles; tile += gridDim.x, ++ti) {
       float acc[BLOCK_N / 2];
       uint32_t prev = 0;
       for (int it = 0; it < k_iters; ++it) {
@@ -526,9 +610,82 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
         __syncwarp();
         if (lane == 0) mbar_arrive(done_bar);
+      } else if (pair_out) {
+        // N <= 128 (kPair): finish the tile in buffer ti & 1, in place over its residual, with the arithmetic of the
+        // register epilogue below.  Every column pair is written; the TMA store clips columns past c_out and pixels outside
+        // the output.  Flat mode: halo rows get zeros, so the halo stays zero.
+        // Bank conflicts: a warp's 32 lanes access rows m0 .. m0 + 7 (m0 % 8 == 0) at lanes 4 r .. 4 r + 3, each quad a
+        // contiguous 8 (bf16) or 4 (e4m3) bytes inside one 16-byte chunk of its row.  128-byte boxes: the 8 rows are 8
+        // different 128-byte lines, i.e. the same 32 banks, and the swizzle puts row r's chunk at c ^ r: 8 different
+        // chunks, 32 different banks (e4m3: 16 banks, two lanes per word).  64-byte boxes: rows 2 s and 2 s + 1 share a
+        // line at byte 64 (r & 1) and the chunk is c ^ (r >> 1): again 8 different 16-byte bank groups.  32-byte boxes
+        // (e4m3 N = 32): rows r and r + 4 share bank group 8 (r & 3) and differ in the chunk (c ^ (r >> 2)).
+        const int b = ti & 1;
+        mbar_wait(&staged_bar[b], uint32_t(ti >> 1) & 1u, p.err, 10);  // the tile's residual has landed, the buffer is free
+        uint8_t* tb = ptile + b * C::kTileBytes;
+        const int n0 = (tile % p.n_tiles) * BLOCK_N;
+        const bool has_res = p.res != nullptr;
+        uint32_t rowoff[2], sw[2];
+        bool valid[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int m = m0 + 8 * h;
+          rowoff[h] = uint32_t(m) * C::kBoxBytes;
+          sw[h] = ((rowoff[h] >> 7) & (C::kBoxBytes / 16 - 1)) << 4;
+          valid[h] = true;
+          if (p.mode == 0) {
+            const int row = (tile / p.n_tiles) * kBlockM + m;
+            const int img = static_cast<int>(fast_div(static_cast<uint32_t>(row), p.plane_mul, p.plane_shr));
+            const int rem = row - img * (p.hp * p.wp);
+            const int yp = static_cast<int>(fast_div(static_cast<uint32_t>(rem), p.wp_mul, p.wp_shr)), xp = rem - yp * p.wp;
+            valid[h] = yp >= 1 && yp <= p.hp - 2 && xp >= 1 && xp <= p.wp - 2;
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j) {
+          const int c = 8 * j + cq;
+          const bool in = n0 + c < p.cout;  // c_out % 32 == 0: a column pair is either inside or outside
+          const float2 bv = in ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
+          float2 qv = bv;
+          if (kInE4m3) qv = in ? __ldg(reinterpret_cast<const float2*>(p.dq + n0 + c)) : make_float2(0.f, 0.f);
+          const uint32_t xb = uint32_t(8 * j * kOes);  // byte of column 8 j in the row
+          const uint32_t region = xb / C::kBoxBytes * (kBlockM * C::kBoxBytes), xin = xb % C::kBoxBytes;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            uint8_t* pp = tb + region + rowoff[h] + (xin ^ sw[h]) + cq * kOes;
+            float x0, x1;
+            if (kInE4m3) {
+              x0 = bias_act_dq(acc[4 * j + 2 * h], bscale * qv.x, bscale * bv.x, silu);
+              x1 = bias_act_dq(acc[4 * j + 2 * h + 1], bscale * qv.y, bscale * bv.y, silu);
+            } else {
+              x0 = bias_act(acc[4 * j + 2 * h], bscale * bv.x, silu);
+              x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * bv.y, silu);
+            }
+            if constexpr (kOutE4m3) {
+              uint16_t& hw = *reinterpret_cast<uint16_t*>(pp);
+              if (has_res) {
+                const float2 f = unpack_e4m3x2(hw);
+                x0 = fmaf(p.res_scale, f.x, x0);
+                x1 = fmaf(p.res_scale, f.y, x1);
+              }
+              hw = valid[h] ? pack_e4m3x2(x0 * p.out_inv_scale, x1 * p.out_inv_scale) : uint16_t(0);
+            } else {
+              uint32_t& word = *reinterpret_cast<uint32_t*>(pp);
+              if (has_res) {
+                const float2 f = unpack_bf16x2(word);
+                x0 += f.x;
+                x1 += f.y;
+              }
+              word = valid[h] ? pack_bf16x2(x0, x1) : 0u;
+            }
+          }
+        }
+        fence_proxy_async_smem();  // the generic-proxy writes are visible to the TMA store
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&done_bar[b]);
       } else {
-        // N <= 128 tiles, the fp32 Detect heads and the FP8 launches: straight from the registers, one row at a time, so only that row's
-        // three output pointers are live beside the accumulators.  The residual may alias the output (training dgrad:
+        // The upsampling and parity-class launches, the fp32 Detect heads: straight from the registers, one row at a
+        // time, so only that row's three output pointers are live beside the accumulators.  The residual may alias the output (training dgrad:
         // res == out), so the compiler keeps every residual load behind the stores that precede it in program order.
         // Loading a whole chunk of column pairs (bias and residual) before the first store of that chunk makes it one trip
         // to memory per chunk instead of one per column pair.  Correct with res == out: a thread reads exactly the
@@ -610,8 +767,10 @@ int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
     attr_set = true;
   }
   ConvTcArgs args = plan.args;
-  const bool out_tile = C::kStaged && args.out_f32 == nullptr;  // as the kernel decides (staged_out)
-  const uint32_t reserve = out_tile ? C::kOutBytes : 0u;
+  // as the kernel decides (staged_out, pair_out)
+  const bool out_tile = C::kStaged && args.out_f32 == nullptr;
+  const bool pair = C::kPair && args.tile_tma != 0;
+  const uint32_t reserve = out_tile ? C::kOutBytes : (pair ? C::kPairBytes : 0u);
   const int b_steps = args.taps * args.kblocks;
   args.bres = plan.bres;
   args.stages = plan.bres ? C::bres_stages(b_steps, reserve) : C::ring_stages(reserve);
@@ -621,11 +780,12 @@ int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
   }
   // the 1 KB alignment of the base comes out of the allocation's slack
   if (args.stages < 2 || args.stages > C::kMaxStages ||
-      C::smem_end(args.stages, args.bres != 0, b_steps, out_tile) + 1024u > C::kSmemBytes)
-    return set_error(Y3_ERR_BAD_ARG, "conv_tc: %d ring stages (resident weights %d, output tile %d) do not fit %zu bytes of shared memory (N=%d K=%d)",
-                     args.stages, args.bres, int(out_tile), C::kSmemBytes, BLOCK_N, BLOCK_K);
+      C::smem_end(args.stages, args.bres != 0, b_steps, reserve) + 1024u > C::kSmemBytes)
+    return set_error(Y3_ERR_BAD_ARG, "conv_tc: %d ring stages (resident weights %d, output tiles %u bytes) do not fit %zu bytes of shared memory (N=%d K=%d)",
+                     args.stages, args.bres, reserve, C::kSmemBytes, BLOCK_N, BLOCK_K);
   // the kernel parks at pdl_wait() after its prologue (y3_common.cuh)
-  Y3_CHECK_CUDA(launch_pdl(kern, dim3(plan.grid), dim3(kThreads), C::kSmemBytes, stream, plan.map_a, plan.map_b, args));
+  Y3_CHECK_CUDA(launch_pdl(kern, dim3(plan.grid), dim3(kThreads), C::kSmemBytes, stream, plan.map_a, plan.map_b,
+                           plan.map_out, plan.map_res, args));
   return Y3_OK;
 }
 
@@ -866,6 +1026,41 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     const uint32_t box[2] = {static_cast<uint32_t>(kch), static_cast<uint32_t>(bn)};
     rc = select_only ? Y3_OK : encode_tensor_map(&plan->map_b, d.in_fmt, d.weight, 2, dims, strides, box, bk * 2);
     if (rc) return rc;
+  }
+  // N <= 128 tiles leave through a TMA store (and load their residual by TMA) unless they are upsampled (a 2 x 2
+  // replicated write is not one box) or one parity class of a transposed conv (every other pixel)
+  plan->map_out = CUtensorMap{};
+  plan->map_res = CUtensorMap{};
+  a.tile_tma = (!head && bn <= 128 && !d.upsample && !(extra && extra->phase)) ? 1 : 0;
+  if (a.tile_tma && !select_only) {
+    // rows of bn output elements in boxes of at most 128 bytes (the kernel's Cfg::kBoxBytes), swizzled to the box width.
+    // The channel extent ends at coff + c_out, so the store never touches the neighbouring slice of a Concat buffer.
+    const int oes = out8 ? 1 : 2;
+    const int box_bytes = bn * oes < 128 ? bn * oes : 128;
+    const uint32_t box_ch = static_cast<uint32_t>(box_bytes / oes);
+    auto encode_out = [&](CUtensorMap* m, const void* base, int ld, int coff) {
+      const uint64_t pitch = static_cast<uint64_t>(ld) * oes;
+      if (a.mode == 0) {  // flat: [rows_total, ld]; the consumers zero the halo rows
+        const uint64_t dims[2] = {static_cast<uint64_t>(coff + d.c_out), static_cast<uint64_t>(a.rows_total)};
+        const uint64_t strides[2] = {0, pitch};
+        const uint32_t box[2] = {box_ch, kBlockM};
+        return encode_tensor_map(m, plan->out_fmt, base, 2, dims, strides, box, box_bytes);
+      }
+      // patch: the interior of the padded output (from pixel (1, 1)), so that patches overhanging it are clipped
+      const uint64_t wpo = static_cast<uint64_t>(a.wo) + 2, hpo = static_cast<uint64_t>(a.ho) + 2;
+      const void* interior = static_cast<const uint8_t*>(base) + (wpo + 1) * pitch;
+      const uint64_t dims[4] = {static_cast<uint64_t>(coff + d.c_out), static_cast<uint64_t>(a.wo),
+                                static_cast<uint64_t>(a.ho), static_cast<uint64_t>(d.n)};
+      const uint64_t strides[4] = {0, pitch, wpo * pitch, hpo * wpo * pitch};
+      const uint32_t box[4] = {box_ch, static_cast<uint32_t>(a.tw), static_cast<uint32_t>(a.th), 1};
+      return encode_tensor_map(m, plan->out_fmt, interior, 4, dims, strides, box, box_bytes);
+    };
+    rc = encode_out(&plan->map_out, d.out, d.out_ld, d.out_coff);
+    if (rc) return rc;
+    if (d.res) {
+      rc = encode_out(&plan->map_res, d.res, d.res_ld, d.res_coff);
+      if (rc) return rc;
+    }
   }
   {
     // resident weights: one N tile whose (taps x k-blocks) boxes fit beside a useful A ring.  The TMA unit's row rate

@@ -73,6 +73,9 @@ struct ConvTcArgs {
   // FP8 (y3_conv_desc): per-channel dequantisation of an e4m3 input, residual scale and output scale of an e4m3 output
   const float* dq;
   float res_scale, out_inv_scale;
+  // 1: N <= 128 tile with a bf16 / e4m3 output that is neither upsampled nor a parity class: the tile is finished in
+  // shared memory and leaves through the map_out TMA store, its residual arrives through map_res (ConvTcPlan)
+  int tile_tma;
 };
 
 struct ConvTcExtra {  // host side of the above (conv_tc_prepare)
@@ -84,6 +87,7 @@ struct ConvTcExtra {  // host side of the above (conv_tc_prepare)
 
 struct ConvTcPlan {
   CUtensorMap map_a, map_b;
+  CUtensorMap map_out, map_res;  // args.tile_tma: the output and residual tiles (zero otherwise)
   int in_fmt, out_fmt;  // Y3_FMT_*: selects the kernel instance
   int halo;    // 1: stride-1 3x3 with one A box per filter row (halo reuse)
   int bres;    // 1: weights resident in shared memory (single N tile, small K)
