@@ -396,10 +396,6 @@ class Model:
     __call__ = forward
 
 
-def _out_hw(h, w, k, s, p):
-    return (h + 2 * p - k) // s + 1, (w + 2 * p - k) // s + 1
-
-
 class Engine:
     """One lowered instance of the graph for a fixed (n, h, w): buffers + prepared launches."""
 
@@ -428,16 +424,13 @@ class Engine:
             _t.DRY_RUN = False
 
     def _lower(self, model, n, h, w, in_dtype, in_div, dev, L):
-        nodes = model.nodes
+        plan = graph.lower(model.nodes, model.ch, h, w)
         W = model.packed()
         # the TMA descriptors built below hold raw device addresses of these tensors: the engine owns a reference, and
         # remembers which weight version it was lowered from (run()/replay() refuse to use stale weights)
         self._weights = W
         self.wver = model._wver
         det = model.detect
-        gs = int(max(det.stride.tolist()))
-        if h % gs or w % gs:
-            raise ValueError(f"image size {h}x{w} must be a multiple of the max stride {gs} (utils/general.py:281-292)")
         self.static_in = torch.zeros(n, model.ch, h, w, dtype=in_dtype, device=dev)
 
         # ---- precision: with FP8 every tensor a tensor-core conv writes is e4m3 with its calibrated scale (a Concat
@@ -455,80 +448,23 @@ class Engine:
         self.amax = torch.zeros(len(model.conv_specs), dtype=torch.float32, device=dev) if calib else None
         self.op_meta: dict[int, dict] = {}       # op index -> what a conv op computes (tests, inspection)
 
-        # ---- shape inference
-        shp: dict[int, tuple[int, int, int]] = {}
-        for nd in nodes[:-1]:
-            src = [(model.ch, h, w) if s < 0 else shp[s] for s in nd.srcs]
-            c0, h0, w0 = src[0]
-            if nd.type == "Conv":
-                k = nd.args[2] if len(nd.args) > 2 else 1
-                s = nd.args[3] if len(nd.args) > 3 else 1
-                ho, wo = _out_hw(h0, w0, k, s, k // 2)
-                shp[nd.i] = (nd.c_out, ho, wo)
-            elif nd.type in ("Bottleneck", "SPP"):
-                shp[nd.i] = (nd.c_out, h0, w0)
-            elif nd.type == "MaxPool2d":
-                k = nd.args[0]
-                s = nd.args[1] if len(nd.args) > 1 else k
-                p = nd.args[2] if len(nd.args) > 2 else 0
-                ho, wo = _out_hw(h0, w0, k, s, p)
-                shp[nd.i] = (c0, ho, wo)
-            elif nd.type == "ZeroPad2d":
-                l, r, t, b = nd.args[0]
-                shp[nd.i] = (c0, h0 + t + b, w0 + l + r)
-            elif nd.type == "Upsample":
-                assert nd.args[1] == 2 and nd.args[2] == "nearest" and nd.args[0] is None, "only nearest 2x upsample"
-                shp[nd.i] = (c0, h0 * 2, w0 * 2)
-            elif nd.type == "Concat":
-                assert nd.args[0] == 1 and all(s[1:] == src[0][1:] for s in src), "Concat expects dim=1, equal H,W"
-                shp[nd.i] = (sum(s[0] for s in src), h0, w0)
-
-        consumers: dict[int, list[int]] = {}
-        for nd in nodes:
-            for s in nd.srcs:
-                consumers.setdefault(s, []).append(nd.i)
-
-        # ---- destinations: producers write straight into their consumer's Concat buffer (zero-copy concat),
-        #      through a fused nearest-2x store when an Upsample sits in between (models/yolov3.yaml:43-44,51-52)
+        # ---- one buffer per Concat: its members write straight into their slices (graph.lower decides which)
         bufs: dict[int, PaddedNHWC] = {}
-        alias: dict[int, PaddedNHWC] = {}       # node -> slice of a concat buffer it must write
-        up_alias: dict[int, PaddedNHWC] = {}    # node -> slice it must write UPSAMPLED
-        virtual: set[int] = set()
         self.keep = []                          # keeps every device tensor alive
-        for nd in nodes[:-1]:
-            if nd.type != "Concat":
-                continue
-            c, hh, ww = shp[nd.i]
-            cat = PaddedNHWC.zeros(n, hh, ww, c, device=dev, dtype=adt, scale=sc(f"model.{nd.i}"))
-            bufs[nd.i] = cat
-            self.cat_members[f"model.{nd.i}"] = []
-            off = 0
-            for s in nd.srcs:
-                cs = shp[s][0]
-                sl = cat.slice(off, cs)
-                off += cs
-                prod = nodes[s]
-                if prod.type == "Upsample":
-                    v = prod.srcs[0]
-                    if consumers.get(v) != [s] or consumers.get(s) != [nd.i] or nodes[v].type != "Conv":
-                        raise NotImplementedError("Upsample is only supported as Conv -> Upsample -> Concat")
-                    up_alias[v] = sl
-                    virtual.update((v, s))
-                else:
-                    if s in alias:
-                        raise NotImplementedError("a tensor feeding two Concat layers would need a copy kernel")
-                    alias[s] = sl
-
+        for ly in plan.layers:
+            if ly.node.type == "Concat":
+                bufs[ly.node.i] = PaddedNHWC.zeros(n, ly.h, ly.w, ly.c, device=dev, dtype=adt, scale=sc(f"model.{ly.node.i}"))
+                self.cat_members[f"model.{ly.node.i}"] = []
         cat_of = {b.buf.data_ptr(): f"model.{i}" for i, b in bufs.items()}
 
-        def out_buf(i, dtype=torch.bfloat16, scale=1.0):
-            """Where node i must leave its result (a Concat slice keeps the Concat's format and scale)."""
-            if i in alias:
-                if alias[i].buf.dtype != dtype:
+        def out_buf(ly, dtype=torch.bfloat16, scale=1.0):
+            """Where a node must leave its result (a Concat slice keeps the Concat's format and scale)."""
+            if ly.dest is not None:
+                sl = bufs[ly.dest.cat].slice(ly.dest.coff, ly.dest.c)
+                if sl.buf.dtype != dtype:
                     raise NotImplementedError("a bf16 tensor feeding an e4m3 Concat buffer")
-                return alias[i]
-            c, hh, ww = shp[i]
-            b = PaddedNHWC.zeros(n, hh, ww, c, device=dev, dtype=dtype, scale=scale)
+                return sl
+            b = PaddedNHWC.zeros(n, ly.h, ly.w, ly.c, device=dev, dtype=dtype, scale=scale)
             self.keep.append(b)
             return b
 
@@ -564,126 +500,105 @@ class Engine:
                     self.amax_names.append(prefix)
                     op_list.append(a)
 
-        tens: dict[int, object] = {}  # node -> PaddedNHWC (or ("zeropad", tensor))
-        for nd in nodes[:-1]:
-            srcs = [tens[s] if s >= 0 else None for s in nd.srcs]
-            base = f"model.{nd.i}"
-            reps = [base] if nd.n == 1 else [f"{base}.{j}" for j in range(nd.n)]
+        def conv(x, b, **kw):
+            emit_conv(x, b.prefix, b.c2, b.k, b.s, ops.ACT_SILU, **kw)
+
+        tens: dict[int, PaddedNHWC | None] = {}  # node -> its output (None: virtual, or written upsampled)
+        for ly in plan.layers:
+            nd = ly.node
+            x = tens.get(nd.srcs[0])  # None for the network input
             if nd.type == "Conv":
-                c1, c2, *rest = nd.args
-                k = rest[0] if len(rest) > 0 else 1
-                s = rest[1] if len(rest) > 1 else 1
-                assert len(rest) < 3 or rest[2] is None, "explicit Conv padding is not used by the YOLOv3 YAMLs"
-                x = srcs[0]
-                for ri, r in enumerate(reps):
-                    last = ri == len(reps) - 1
-                    if x is None:  # network input -> layer 0
-                        assert c1 == 3 and k == 3 and s == 1 and c2 in (16, 32), "first layer must be Conv(3->16|32, 3, 1)"
-                        y = out_buf(nd.i) if last else PaddedNHWC.zeros(n, h, w, c2, device=dev)
+                for j, b in enumerate(ly.blocks):
+                    last = j == len(ly.blocks) - 1
+                    if b.role == graph.FIRST:
+                        if b.c2 not in (16, 32):
+                            raise NotImplementedError("conv_first writes 16 or 32 channels")
+                        y = out_buf(ly) if last else PaddedNHWC.zeros(n, h, w, b.c2, device=dev)
                         o = _lib.Op()
                         o.kind = _lib.OP_CONV_FIRST
-                        o.first = ops.first_desc(self.static_in, *W[r], c2, y, in_div)
+                        o.first = ops.first_desc(self.static_in, *W[b.prefix], b.c2, y, in_div)
                         op_list.append(o)
-                    elif last and nd.i in up_alias:
-                        emit_conv(x, r, c2, k, s, ops.ACT_SILU, out=up_alias[nd.i], upsample=True)
+                    elif last and ly.upsampled:
+                        conv(x, b, out=out_buf(ly, adt), upsample=True)
                         y = None
                     else:
-                        ho, wo = _out_hw(x.h, x.w, k, s, k // 2)
-                        y = out_buf(nd.i, adt, sc(r)) if last else PaddedNHWC.zeros(n, ho, wo, c2, device=dev, dtype=adt,
-                                                                                    scale=sc(r))
-                        emit_conv(x, r, c2, k, s, ops.ACT_SILU, out=y)
+                        y = out_buf(ly, adt, sc(b.prefix)) if last else PaddedNHWC.zeros(n, ly.h, ly.w, b.c2, device=dev,
+                                                                                          dtype=adt, scale=sc(b.prefix))
+                        conv(x, b, out=y)
                     self.keep.append(y)
                     x = y
                 tens[nd.i] = x
             elif nd.type == "Bottleneck":
-                c1, c2, *rest = nd.args
-                shortcut = rest[0] if rest else True
-                assert len(rest) < 2 or rest[1] == 1, "grouped Bottleneck is not used by the YOLOv3 YAMLs"
-                x = srcs[0]
-                c_ = int(c2 * 0.5)
-                tmp = PaddedNHWC.zeros(n, x.h, x.w, c_, device=dev, dtype=adt)
-                ping = [PaddedNHWC.zeros(n, x.h, x.w, c2, device=dev, dtype=adt)
-                        for _ in range(min(2, max(0, len(reps) - 1)))]
+                pairs = list(zip(ly.blocks[::2], ly.blocks[1::2]))  # (cv1, cv2) per repeat
+                c_ = pairs[0][0].c2
+                tmp = PaddedNHWC.zeros(n, ly.h, ly.w, c_, device=dev, dtype=adt)
+                ping = [PaddedNHWC.zeros(n, ly.h, ly.w, ly.c, device=dev, dtype=adt) for _ in range(min(2, len(pairs) - 1))]
                 self.keep += [tmp, *ping]
-                final = out_buf(nd.i, adt, sc(reps[-1] + ".cv2"))
-                for ri, r in enumerate(reps):
+                final = out_buf(ly, adt, sc(pairs[-1][1].prefix))
+                for j, (cv1, cv2) in enumerate(pairs):
                     # the shared buffers carry the scale of the conv that writes them this time
-                    t = PaddedNHWC(tmp.buf, 0, c_, sc(r + ".cv1"))
-                    y = final if ri == len(reps) - 1 else PaddedNHWC(ping[ri % 2].buf, 0, c2, sc(r + ".cv2"))
-                    add = shortcut and c1 == c2
-                    emit_conv(x, r + ".cv1", c_, 1, 1, ops.ACT_SILU, out=t)
-                    emit_conv(t, r + ".cv2", c2, 3, 1, ops.ACT_SILU, out=y, res=x if add else None)
-                    x, c1 = y, c2
+                    t = PaddedNHWC(tmp.buf, 0, c_, sc(cv1.prefix))
+                    y = final if j == len(pairs) - 1 else PaddedNHWC(ping[j % 2].buf, 0, ly.c, sc(cv2.prefix))
+                    conv(x, cv1, out=t)
+                    conv(t, cv2, out=y, res=x if cv2.shortcut else None)
+                    x = y
                 tens[nd.i] = x
             elif nd.type == "SPP":
-                c1, c2, *rest = nd.args
-                ks = tuple(rest[0]) if rest else (5, 9, 13)
-                assert ks == (5, 9, 13), "SPP kernels other than (5, 9, 13) are not used by the YOLOv3 YAMLs"
-                x = srcs[0]
-                c_ = c1 // 2
-                cat = PaddedNHWC.zeros(n, x.h, x.w, 4 * c_, device=dev, dtype=adt, scale=sc(base + ".cv1"))
+                cv1, cv2 = ly.blocks
+                if cv1.ks != (5, 9, 13):
+                    raise NotImplementedError("SPP kernels other than (5, 9, 13) are not used by the YOLOv3 YAMLs")
+                c_ = cv1.c2
+                cat = PaddedNHWC.zeros(n, ly.h, ly.w, 4 * c_, device=dev, dtype=adt, scale=sc(cv1.prefix))
                 self.keep.append(cat)
-                emit_conv(x, base + ".cv1", c_, 1, 1, ops.ACT_SILU, out=cat.slice(0, c_))
+                conv(x, cv1, out=cat.slice(0, c_))
                 for q in range(3):  # 5x5 cascade == 5/9/13 pools with -inf padding
                     o = _lib.Op()
                     o.kind = _lib.OP_MAXPOOL
                     o.pool = ops.pool_desc(cat.slice(q * c_, c_), cat.slice((q + 1) * c_, c_), 5, 1, -2, False)
                     op_list.append(o)
-                y = out_buf(nd.i, adt, sc(base + ".cv2"))
-                emit_conv(cat, base + ".cv2", c2, 1, 1, ops.ACT_SILU, out=y)
+                y = out_buf(ly, adt, sc(cv2.prefix))
+                conv(cat, cv2, out=y)
                 tens[nd.i] = y
             elif nd.type == "MaxPool2d":
-                k = nd.args[0]
-                s = nd.args[1] if len(nd.args) > 1 else k
-                p = nd.args[2] if len(nd.args) > 2 else 0
-                x = srcs[0]
-                oob_zero = False
-                if isinstance(x, tuple):  # ZeroPad2d([0,1,0,1]) feeding MaxPool2d(2,1,0)
-                    _, x, pad = x
-                    assert tuple(pad) == (0, 1, 0, 1) and (k, s, p) == (2, 1, 0), "only ZeroPad2d([0,1,0,1])+MaxPool2d(2,1,0)"
-                    oob_zero = True
-                if nd.i in alias and self.precision != "bf16":
+                p = ly.pool
+                x = tens[p.src]
+                if ly.dest is not None and self.precision != "bf16":
                     # its codes would carry the input's scale, not the Concat's, and calibration would miss it
                     raise NotImplementedError("FP8: a max-pool writing into a Concat buffer")
-                y = out_buf(nd.i, x.buf.dtype, x.scale)
+                y = out_buf(ly, x.buf.dtype, x.scale)
                 o = _lib.Op()
                 o.kind = _lib.OP_MAXPOOL
-                o.pool = ops.pool_desc(x, y, k, s, -p, oob_zero)
+                o.pool = ops.pool_desc(x, y, p.k, p.s, -p.pad, p.oob_zero)
                 op_list.append(o)
                 tens[nd.i] = y
-            elif nd.type == "ZeroPad2d":
-                assert consumers.get(nd.i, []) and all(nodes[c].type == "MaxPool2d" for c in consumers[nd.i])
-                tens[nd.i] = ("zeropad", srcs[0], nd.args[0])
-            elif nd.type == "Upsample":
-                tens[nd.i] = None  # fused into the producing conv's store
             elif nd.type == "Concat":
                 tens[nd.i] = bufs[nd.i]
+            else:  # Upsample / ZeroPad2d: folded into the producing conv's store / the pool that follows
+                tens[nd.i] = None
 
         # ---- Detect: 1x1 head convs storing fp32 pixel-major [bs*ny*nx, ld], then ONE launch that transposes them
         #      into the reference's [bs,na,ny,nx,no] logits and decodes z
-        dnode = nodes[-1]
         self.raw = []
         self.head_out = []
         head_ld = ops.cout_pad(det.na * det.no)
         dec = _lib.DecodeDesc()
         anchors_px = det.anchors * det.stride.view(-1, 1, 1)
         rows = 0
-        for j, s in enumerate(dnode.srcs):
-            x = tens[s]
-            head = torch.zeros(n * x.h * x.w, head_ld, dtype=torch.float32, device=dev)
+        for j, hd in enumerate(plan.heads):
+            head = torch.zeros(n * hd.ny * hd.nx, head_ld, dtype=torch.float32, device=dev)
             # the reference's raw map x[i] = conv(x).view(bs,na,no,ny,nx).permute(0,1,3,4,2) (models/yolo.py:96-98) IS this
             # buffer seen through strides: no second copy of 8.6 MB/image is written.  Model.forward() clones it into the
             # reference's contiguous format; Engine users get the zero-copy view.
-            raw = head.view(n, x.h, x.w, head_ld)[..., : det.na * det.no].unflatten(-1, (det.na, det.no)).permute(0, 3, 1, 2, 4)
+            raw = head.view(n, hd.ny, hd.nx, head_ld)[..., : det.na * det.no].unflatten(-1, (det.na, det.no)).permute(0, 3, 1, 2, 4)
             self.raw.append(raw)
             self.head_out.append(head)
-            emit_conv(x, f"model.{det.i}.m.{j}", det.na * det.no, 1, 1, ops.ACT_NONE, out_f32=head)
+            emit_conv(tens[hd.src], f"model.{det.i}.m.{j}", det.na * det.no, 1, 1, ops.ACT_NONE, out_f32=head)
             lv = dec.levels[j]
             lv.head, lv.head_ld, lv.raw_out = head.data_ptr(), head_ld, None
-            lv.ny, lv.nx, lv.stride = x.h, x.w, float(det.stride[j])
+            lv.ny, lv.nx, lv.stride = hd.ny, hd.nx, hd.stride
             for a in range(det.na):
                 lv.anchor_w[a], lv.anchor_h[a] = float(anchors_px[j, a, 0]), float(anchors_px[j, a, 1])
-            rows += det.na * x.h * x.w
+            rows += det.na * hd.ny * hd.nx
         self.z = torch.zeros(n, rows, det.no, dtype=torch.float32, device=dev)
         dec.nl, dec.bs, dec.na, dec.no, dec.z = det.nl, n, det.na, det.no, self.z.data_ptr()
         o = _lib.Op()

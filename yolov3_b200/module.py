@@ -82,36 +82,31 @@ class DetectionModel(nn.Module):
         self.yaml, self.save, self.stride, self.names, self.nc = core.yaml, core.save, core.stride, core.names, core.nc
         self.inplace, self.hyp = core.inplace, None
         store = core.store()
+        blocks = {}  # node -> its Conv+BN blocks, decoded once by graph.conv_specs
+        for b in core.conv_specs:
+            blocks.setdefault(b.node, []).append(b)
         layers = []
         for nd in core.nodes:
-            t, a = nd.type, nd.args
+            t, a, bl = nd.type, nd.args, blocks.get(nd.i)
             if t == "Conv":
-                mk = lambda a=a: Conv(a[0], a[1], a[2] if len(a) > 2 else 1, a[3] if len(a) > 3 else 1)  # noqa: E731
+                mods = [Conv(b.c1, b.c2, b.k, b.s) for b in bl]
             elif t == "Bottleneck":
-                mk = None
+                mods = [Bottleneck(cv1.c1, cv2.c2, cv2.shortcut) for cv1, cv2 in zip(bl[::2], bl[1::2])]
             elif t == "SPP":
-                mk = lambda a=a: SPP(a[0], a[1], tuple(a[2]) if len(a) > 2 else (5, 9, 13))  # noqa: E731
+                mods = [SPP(bl[0].c1, bl[1].c2, bl[0].ks)]
             elif t == "Upsample":
-                mk = lambda a=a: nn.Upsample(a[0], a[1], a[2])  # noqa: E731
+                mods = [nn.Upsample(a[0], a[1], a[2]) for _ in range(nd.n)]
             elif t == "Concat":
-                mk = lambda a=a: Concat(a[0])  # noqa: E731
+                mods = [Concat(a[0]) for _ in range(nd.n)]
             elif t == "MaxPool2d":
-                mk = lambda a=a: nn.MaxPool2d(*a)  # noqa: E731
+                mods = [nn.MaxPool2d(*a) for _ in range(nd.n)]
             elif t == "ZeroPad2d":
-                mk = lambda a=a: nn.ZeroPad2d(*a)  # noqa: E731
+                mods = [nn.ZeroPad2d(*a) for _ in range(nd.n)]
             elif t == "Detect":
-                mk = lambda a=a: Detect(core.detect, a[2])  # noqa: E731
+                mods = [Detect(core.detect, a[2]) for _ in range(nd.n)]
             else:
                 raise NotImplementedError(t)
-            if t == "Bottleneck":
-                c1, c2, *rest = a
-                blocks = []
-                for _ in range(nd.n):
-                    blocks.append(Bottleneck(c1, c2, rest[0] if rest else True))
-                    c1 = c2
-                m_ = nn.Sequential(*blocks) if nd.n > 1 else blocks[0]
-            else:
-                m_ = nn.Sequential(*(mk() for _ in range(nd.n))) if nd.n > 1 else mk()
+            m_ = nn.Sequential(*mods) if nd.n > 1 else mods[0]
             m_.i, m_.f, m_.type = nd.i, nd.f, f"models.common.{t}" if t not in ("Upsample", "MaxPool2d", "ZeroPad2d") else f"torch.nn.{t}"
             layers.append(m_)
         self.model = nn.Sequential(*layers)

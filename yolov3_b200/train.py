@@ -20,7 +20,8 @@ with a fixed summation order — no floating-point atomics — except the split-
 
 ``TrainEngine.forward/backward`` are wrapped in one ``torch.autograd.Function`` so that the reference's
 ``loss.backward(); optimizer.step()`` work unchanged on the fp32 master parameters (``Model.parameters()``).
-Supported layer types in train mode: Conv, Bottleneck, SPP, nn.Upsample, Concat, Detect (= yolov3.yaml, yolov3-spp.yaml).
+The graph is lowered by ``graph.lower``, the same plan the inference engine builds from: both engines accept the same
+graphs and write every tensor to the same place.
 """
 from __future__ import annotations
 
@@ -29,7 +30,7 @@ import ctypes as C
 import torch
 import torch.distributed as dist
 
-from . import _lib, ops
+from . import _lib, graph, ops
 from . import train_ops as T
 from .tensors import PaddedNHWC, _stream
 
@@ -57,14 +58,8 @@ class TrainEngine:
         dev = model.device
         self.model, self.n, self.h, self.w = model, n, h, w
         det = model.detect
-        nodes = model.nodes
-        gs = int(max(det.stride.tolist()))
-        if h % gs or w % gs:  # same rule as the inference Engine (utils/general.py:281-292 check_img_size)
-            raise ValueError(f"image size {h}x{w} must be a multiple of the max stride {gs}")
+        plan = graph.lower(model.nodes, model.ch, h, w)
         self.fwd_gen = 0  # activations live in this engine's buffers: a backward must belong to the LAST forward
-        for nd in nodes[:-1]:
-            if nd.type not in ("Conv", "Bottleneck", "Upsample", "Concat", "SPP", "MaxPool2d", "ZeroPad2d"):
-                raise NotImplementedError(f"training-mode {nd.type} is not built")
         store = model.store()
         self.store = store
         self.P = model.device_params()
@@ -92,8 +87,10 @@ class TrainEngine:
             self.keep.append(t)
             return t
 
-        def new_block(prefix, c1, c2, k, s, x, a, res=None, upsample=False, first=False):
+        def new_block(cb, x, a, res=None, upsample=False):
             nonlocal max_partial
+            prefix, c2, first = cb.prefix, cb.c2, cb.role == graph.FIRST
+            c1, k, s = (32, 1, 1) if first else (cb.c1, cb.k, cb.s)  # layer 0 = 1x1 conv over the im2col
             b = _Block()
             b.prefix, b.c1, b.c2, b.k, b.s, b.x, b.a, b.res, b.upsample, b.first = prefix, c1, c2, k, s, x, a, res, upsample, first
             ho, wo = x.h // s, x.w // s
@@ -114,140 +111,71 @@ class TrainEngine:
             self.blocks.append(b)
             return b
 
-        # ---- shapes and concat destinations (same zero-copy concat / fused upsample layout as the inference engine)
-        shp = {}
-        for nd in nodes[:-1]:
-            src = [(model.ch, h, w) if s < 0 else shp[s] for s in nd.srcs]
-            c0, h0, w0 = src[0]
-            if nd.type == "Conv":
-                s_ = nd.args[3] if len(nd.args) > 3 else 1
-                shp[nd.i] = (nd.c_out, h0 // s_, w0 // s_)
-            elif nd.type in ("Bottleneck", "SPP"):
-                shp[nd.i] = (nd.c_out, h0, w0)
-            elif nd.type == "Upsample":
-                shp[nd.i] = (c0, h0 * 2, w0 * 2)
-            elif nd.type == "Concat":
-                shp[nd.i] = (sum(s[0] for s in src), h0, w0)
-            elif nd.type == "ZeroPad2d":
-                shp[nd.i] = (c0, h0, w0)  # virtual: folded into the MaxPool2d(2,1,0) that follows (out-of-bounds = 0)
-            elif nd.type == "MaxPool2d":
-                k_, s2_ = nd.args[0], (nd.args[1] if len(nd.args) > 1 else nd.args[0])
-                shp[nd.i] = (c0, h0, w0) if (k_, s2_) == (2, 1) else (c0, h0 // s2_, w0 // s2_)
-        consumers = {}
-        for nd in nodes:
-            for s in nd.srcs:
-                consumers.setdefault(s, []).append(nd.i)
-        cat_buf, alias, up_alias = {}, {}, {}
-        for nd in nodes[:-1]:
-            if nd.type != "Concat":
-                continue
-            c, hh, ww = shp[nd.i]
-            cat = buf(c, hh, ww)
-            cat_buf[nd.i] = cat
-            off = 0
-            for s in nd.srcs:
-                cs = shp[s][0]
-                sl = cat.slice(off, cs)
-                off += cs
-                if nodes[s].type == "Upsample":
-                    v = nodes[s].srcs[0]
-                    assert consumers.get(v) == [s] and consumers.get(s) == [nd.i] and nodes[v].type == "Conv"
-                    up_alias[v] = sl
-                else:
-                    alias[s] = sl
+        # ---- Concat destinations (the same zero-copy concat / fused upsample layout as the inference engine)
+        cat_buf = {ly.node.i: buf(ly.c, ly.h, ly.w) for ly in plan.layers if ly.node.type == "Concat"}
 
-        def out_of(i):
-            if i in alias:
-                return alias[i]
-            c, hh, ww = shp[i]
-            return buf(c, hh, ww)
+        def out_of(ly):
+            if ly.dest is not None:
+                return cat_buf[ly.dest.cat].slice(ly.dest.coff, ly.dest.c)
+            return buf(ly.c, ly.h, ly.w)
 
         # ---- lower the graph into Conv blocks
         self.im2col = buf(32, h, w)
         tens = {}
-        for nd in nodes[:-1]:
-            srcs = [tens[s] if s >= 0 else None for s in nd.srcs]
-            base = f"model.{nd.i}"
-            reps = [base] if nd.n == 1 else [f"{base}.{j}" for j in range(nd.n)]
+        for ly in plan.layers:
+            nd = ly.node
+            x = self.im2col if nd.srcs[0] < 0 else tens.get(nd.srcs[0])
             if nd.type == "Conv":
-                c1, c2, *rest = nd.args
-                k = rest[0] if len(rest) > 0 else 1
-                s_ = rest[1] if len(rest) > 1 else 1
-                x = srcs[0]
-                for ri, r in enumerate(reps):
-                    last = ri == len(reps) - 1
-                    if x is None:
-                        assert c1 == 3 and k == 3 and s_ == 1
-                        a = out_of(nd.i) if last else buf(c2, h, w)
-                        new_block(r, 32, c2, 1, 1, self.im2col, a, first=True)  # layer 0 = 1x1 conv over the im2col
-                    elif last and nd.i in up_alias:
-                        a = up_alias[nd.i]
-                        new_block(r, c1, c2, k, s_, x, a, upsample=True)
-                    else:
-                        a = out_of(nd.i) if last else buf(c2, x.h // s_, x.w // s_)
-                        new_block(r, c1, c2, k, s_, x, a)
+                for j, cb in enumerate(ly.blocks):
+                    last = j == len(ly.blocks) - 1
+                    a = out_of(ly) if last else buf(cb.c2, ly.h, ly.w)
+                    new_block(cb, x, a, upsample=last and ly.upsampled)
                     x = a
                 tens[nd.i] = x
             elif nd.type == "Bottleneck":
-                c1, c2, *rest = nd.args
-                shortcut = rest[0] if rest else True
-                x = srcs[0]
-                c_ = int(c2 * 0.5)
-                for ri, r in enumerate(reps):
-                    yb = out_of(nd.i) if ri == len(reps) - 1 else buf(c2, x.h, x.w)
-                    t = buf(c_, x.h, x.w)
-                    new_block(r + ".cv1", c1, c_, 1, 1, x, t)
-                    new_block(r + ".cv2", c_, c2, 3, 1, t, yb, res=x if (shortcut and c1 == c2) else None)
-                    x, c1 = yb, c2
+                for cv1, cv2 in zip(ly.blocks[::2], ly.blocks[1::2]):
+                    yb = out_of(ly) if cv2 is ly.blocks[-1] else buf(cv2.c2, ly.h, ly.w)
+                    t = buf(cv1.c2, ly.h, ly.w)
+                    new_block(cv1, x, t)
+                    new_block(cv2, t, yb, res=x if cv2.shortcut else None)
+                    x = yb
                 tens[nd.i] = x
             elif nd.type == "SPP":
                 # models/common.py:281-290: cv2(cat[x, mp5(x), mp9(x), mp13(x)]) with x = cv1(input); each pool reads x
-                c1, c2, *rest = nd.args
-                ks = tuple(rest[0]) if rest else (5, 9, 13)
-                x = srcs[0]
-                c_ = c1 // 2
-                cat = buf((len(ks) + 1) * c_, x.h, x.w)
-                b1 = new_block(base + ".cv1", c1, c_, 1, 1, x, cat.slice(0, c_))
-                for q, k in enumerate(ks):
-                    idx = torch.zeros(n * x.h * x.w * c_, dtype=torch.uint8, device=dev)
+                cv1, cv2 = ly.blocks
+                c_ = cv1.c2
+                cat = buf(cv2.c1, ly.h, ly.w)
+                b1 = new_block(cv1, x, cat.slice(0, c_))
+                for q, k in enumerate(cv1.ks):
+                    idx = torch.zeros(n * ly.h * ly.w * c_, dtype=torch.uint8, device=dev)
                     self.keep.append(idx)
                     src, dst = cat.slice(0, c_), cat.slice((q + 1) * c_, c_)
                     b1.post_fwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_train_fwd(src, dst, k, idx))
                     b1.pre_bwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_bwd(self.grad_of(dst), self.grad_of(src),
                                                                                         k, idx, accumulate=True))
-                y = out_of(nd.i)
-                new_block(base + ".cv2", (len(ks) + 1) * c_, c2, 1, 1, cat, y)
+                y = out_of(ly)
+                new_block(cv2, cat, y)
                 tens[nd.i] = y
-            elif nd.type == "Upsample":
-                tens[nd.i] = None
             elif nd.type == "Concat":
                 tens[nd.i] = cat_buf[nd.i]
-            elif nd.type == "ZeroPad2d":  # yolov3-tiny.yaml:29: nn.ZeroPad2d([0,1,0,1]) feeding nn.MaxPool2d(2,1,0)
-                assert tuple(nd.args[0]) == (0, 1, 0, 1) and all(nodes[c].type == "MaxPool2d" for c in consumers.get(nd.i, []))
-                tens[nd.i] = ("zeropad", srcs[0])
             elif nd.type == "MaxPool2d":
-                k = nd.args[0]
-                s_ = nd.args[1] if len(nd.args) > 1 else k
-                pd = nd.args[2] if len(nd.args) > 2 else 0
-                x, oob_zero = srcs[0], False
-                if isinstance(x, tuple):
-                    assert (k, s_, pd) == (2, 1, 0), "only ZeroPad2d([0,1,0,1]) + MaxPool2d(2,1,0)"
-                    x, oob_zero = x[1], True
-                y = out_of(nd.i)
+                p = ly.pool
+                x = tens[p.src]
+                y = out_of(ly)
                 idx = torch.zeros(n * y.h * y.w * x.c, dtype=torch.uint8, device=dev)
                 self.keep.append(idx)
                 host = self.blocks[-1]  # the pool runs after the latest block's forward and before that block's backward
-                host.post_fwd.append(lambda x=x, y=y, k=k, s_=s_, pd=pd, idx=idx, oz=oob_zero:
-                                     T.maxpool_train_fwd(x, y, k, idx, stride=s_, off=-pd, oob_zero=oz))
-                host.pre_bwd.append(lambda x=x, y=y, k=k, s_=s_, pd=pd, idx=idx: self._pool_backward(x, y, k, s_, -pd, idx))
+                host.post_fwd.append(lambda x=x, y=y, p=p, idx=idx:
+                                     T.maxpool_train_fwd(x, y, p.k, idx, stride=p.s, off=-p.pad, oob_zero=p.oob_zero))
+                host.pre_bwd.append(lambda x=x, y=y, p=p, idx=idx: self._pool_backward(x, y, p.k, p.s, -p.pad, idx))
                 tens[nd.i] = y
 
         # ---- Detect heads
         self.heads = []
         head_ld = ops.cout_pad(det.na * det.no)
         dec = _lib.DecodeDesc()
-        for j, s in enumerate(nodes[-1].srcs):
-            x = tens[s]
+        for j, ph in enumerate(plan.heads):
+            x = tens[ph.src]
             wname, bname = f"model.{det.i}.m.{j}.weight", f"model.{det.i}.m.{j}.bias"
             hd = dict(x=x, c1=x.c, j=j, wname=wname, bname=bname)
             hd["out"] = torch.zeros(n * x.h * x.w, head_ld, dtype=torch.float32, device=dev)
@@ -263,7 +191,7 @@ class TrainEngine:
             self.heads.append(hd)
             lv = dec.levels[j]
             lv.head, lv.head_ld, lv.raw_out = hd["out"].data_ptr(), head_ld, hd["raw"].data_ptr()
-            lv.ny, lv.nx, lv.stride = x.h, x.w, float(det.stride[j])
+            lv.ny, lv.nx, lv.stride = ph.ny, ph.nx, ph.stride
         dec.nl, dec.bs, dec.na, dec.no, dec.z = det.nl, n, det.na, det.no, None
         self.dec = dec
         self.err = torch.zeros(1, dtype=torch.int32, device=dev)
