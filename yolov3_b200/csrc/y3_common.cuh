@@ -87,6 +87,12 @@ __device__ __forceinline__ void tma_load_5d(void* dst, const CUtensorMap* m, uin
       "r"(c4)
       : "memory");
 }
+// 1-D bulk copy of `bytes` contiguous bytes (a multiple of 16; both addresses 16-byte aligned), credited to `bar`
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
 
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
@@ -108,6 +114,27 @@ __device__ __forceinline__ void bulk_wait_read_1() { asm volatile("cp.async.bulk
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+__device__ __forceinline__ uint32_t lds32(uint32_t saddr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(saddr));
+  return v;
+}
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory");
+}
+__device__ __forceinline__ float2 lds_f32x2(uint32_t saddr) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(saddr));
+  return v;
+}
+__device__ __forceinline__ uint16_t lds16(uint32_t saddr) {
+  uint16_t v;
+  asm volatile("ld.shared.b16 %0, [%1];" : "=h"(v) : "r"(saddr));
+  return v;
+}
+__device__ __forceinline__ void sts16(uint32_t saddr, uint16_t v) {
+  asm volatile("st.shared.b16 [%0], %1;" ::"r"(saddr), "h"(v) : "memory");
 }
 __device__ __forceinline__ uint4 lds128(uint32_t saddr) {
   uint4 v;

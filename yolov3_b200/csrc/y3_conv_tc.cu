@@ -13,28 +13,24 @@
 // Warp roles (320 threads, 1 CTA/SM, persistent over tiles): warp 8 = TMA producer (the whole warp runs the loop, one elected
 // lane issues); warpgroups 0 and 1 (warps 0-7) = consumers, each owning 64 of the tile's 128 rows: it issues the
 // m64 x BLOCK_N wgmma of its rows for every stage of the smem ring and releases a stage as soon as the MMAs that read it
-// have completed; warp 9 = store warp (N = 256 bf16-output launches).  Per tile of such a launch:
-//   1. stage: during the tile's main loop the store warp copies the tile's residual into a 128 x BLOCK_N bf16 shared-memory
-//      tile and the BLOCK_N bias floats beside it (cp.async), then arrives on `staged`;
+// have completed; warp 9 = store warp.  Launches with a bf16 / e4m3 output (ConvTcArgs::tile_tma) keep Cfg::kBufs output
+// tile buffers in the swizzled layout of their TMA maps, and the store warp's lane 0 moves whole tiles with the bulk-copy
+// engine.  Tile i of a CTA uses buffer i % kBufs:
+//   1. stage: the store warp loads the tile's residual into the buffer by TMA (N = 256: also the tile's bias, and an e4m3
+//      input's dq, by bulk copy beside it), all credited to `staged`, while the consumers still run earlier tiles;
 //   2. finish: after the last k-block the consumers wait on `staged`, apply bias, SiLU and residual from their registers,
-//      write the bf16 pairs back into the same words, arrive on `done` and go straight on to the next tile's MMAs;
-//   3. drain: the store warp waits on `done` and writes the tile out with 16-byte stores (halo and out-of-range rows
-//      skipped, concat offset, nearest-2x upsample), then stages the next tile into the same buffer.
-// N <= 128 launches with a bf16 / e4m3 output (Cfg::kPair, ConvTcArgs::tile_tma) run the same three steps with TWO tile
-// buffers in the swizzled layout of their TMA maps, and the store warp's lane 0 moves whole tiles with the bulk-copy engine:
-// it loads tile i's residual into buffer i & 1 by TMA (one tile ahead), the consumers finish the tile in place and fence
-// it for the async proxy, and the store warp writes it out with one TMA store per 128-byte-wide box (the maps clip pixels
-// outside the output and channels past c_out; flat-mode halo rows carry zeros), then restages the buffer for tile i + 2
-// once that store has read it.
+//      write the pairs into the buffer in place (flat-mode halo rows get zeros), fence it for the async proxy, arrive on
+//      `done` and go straight on to the next tile's MMAs;
+//   3. store: the store warp waits on `done` and writes the tile out with one TMA store per 128-byte-wide box (the maps
+//      clip pixels outside the output and channels past c_out), then restages the buffer for tile i + kBufs once that
+//      store has read it.
 // The fp32 Detect-head launches (a 128 x 256 fp32 tile does not fit beside the ring), the upsampling launches (a 2 x 2
 // replicated write is not one box) and the parity classes of the transposed stride-2 conv store straight from the
 // consumers' registers.  While the consumers finish a tile the producer already fills the ring for their next one.
 // FP8 (IN_FMT / OUT_FMT = Y3_FMT_E4M3): an e4m3 k-block of 2 * BLOCK_K channels has the byte geometry of a bf16 k-block of
 // BLOCK_K channels (same swizzled rows, descriptors and halo offsets) and one k32 e4m3 wgmma consumes the 32 bytes of one
 // k16 bf16 step, so ring, halo / patch modes and the producer's addressing are shared; BLOCK_K counts bf16-equivalent
-// columns (half a row's bytes).  The epilogue dequantises with dq[n] = s_in * s_w[n] and stores sat_e4m3(y / s_out).  The
-// N = 256 e4m3-output launches keep the store warp: their tile is 128 x 256 bytes in channel order (16-byte chunks of 16
-// channels), the residual is staged as e4m3, and an e4m3 input stages its dq floats beside the bias.
+// columns (half a row's bytes).  The epilogue dequantises with dq[n] = s_in * s_w[n] and stores sat_e4m3(y / s_out).
 #include <cuda_bf16.h>
 
 #include <type_traits>
@@ -60,7 +56,7 @@ constexpr int kSmemBudget = 221 * 1024;  // ring (+ resident weights); alignment
 // so the descriptor's base offset stays 0).  A rows fetched per k-block drop from 9*128 to 3*130 and the producer runs a
 // third of the pipeline stages.
 // STAGE_ES: bytes per element of the staged output tile (2 bf16, 1 e4m3; 0: never staged, the fp32-only head instances).
-// STAGE_DQ: an e4m3 input, whose BLOCK_N dq floats are staged beside the bias.
+// STAGE_DQ: an e4m3 input, whose BLOCK_N dq floats are staged beside the bias (N = 256).
 template <int BLOCK_N, int BLOCK_K, bool HALO, int STAGE_ES = 2, bool STAGE_DQ = false>
 struct Cfg {
   static constexpr uint32_t kARows = HALO ? kBlockM + 2 : kBlockM;
@@ -71,22 +67,22 @@ struct Cfg {
   static constexpr uint32_t kStageBytes = kABytes + kTaps * kBBytes;
   static constexpr int kMaxStages = 8;
   static constexpr uint32_t kBarBytes = 256;  // mbarriers
-  // N = 256 bf16-output launches hand the finished tile to the store warp: they keep the output tile (128 x BLOCK_N bf16)
-  // and the tile's BLOCK_N bias floats beside the ring, and those bytes come out of the ring's budget (`reserve`).
-  // Thinner tiles run only a few microseconds each: one warp's 16-byte copies cannot drain and restage them in that time,
-  // so they use two buffers and the bulk-copy engine instead (kPair below).
-  static constexpr bool kStaged = BLOCK_N == 256 && STAGE_ES > 0;
-  static constexpr uint32_t kTileBytes = kBlockM * BLOCK_N * (STAGE_ES > 0 ? STAGE_ES : 2);
-  static constexpr uint32_t kOutBytes = kTileBytes + BLOCK_N * 4 * (STAGE_DQ ? 2 : 1);
-  // N <= 128 launches whose tile leaves by TMA (ConvTcArgs::tile_tma) keep two output tiles, 1 KB aligned after the
-  // barriers, in the TMA maps' swizzled layout: each row is split into boxes of kBoxBytes (at most 128, the widest
-  // swizzle), box k of all 128 rows is one region of 128 x kBoxBytes, and 16-byte chunk c of row m sits at chunk
-  // c ^ ((m * kBoxBytes / 128) mod (kBoxBytes / 16)) of that row (the TMA swizzle of that width)
-  static constexpr bool kPair = BLOCK_N <= 128 && STAGE_ES > 0;
+  // Launches whose tile leaves by TMA (ConvTcArgs::tile_tma) keep kBufs output tiles, 1 KB aligned after the barriers,
+  // in the TMA maps' swizzled layout: each row is split into boxes of kBoxBytes (at most 128, the widest swizzle), box k
+  // of all 128 rows is one region of 128 x kBoxBytes, and 16-byte chunk c of row m sits at chunk
+  // c ^ ((m * kBoxBytes / 128) mod (kBoxBytes / 16)) of that row (the TMA swizzle of that width).  Those bytes come out
+  // of the ring's budget (`reserve` = kTileReserve).  Two buffers let a tile's residual arrive while the previous tile
+  // is still being stored; a 64 KB bf16 N = 256 tile gets one, as two would leave a single ring stage beside them.
   static constexpr uint32_t kRowBytes = BLOCK_N * (STAGE_ES > 0 ? STAGE_ES : 2);
+  static constexpr uint32_t kTileBytes = kBlockM * kRowBytes;
   static constexpr uint32_t kBoxBytes = kRowBytes < 128 ? kRowBytes : 128;
   static constexpr uint32_t kBoxes = kRowBytes / kBoxBytes;
-  static constexpr uint32_t kPairBytes = 1024 - kBarBytes + 2 * kTileBytes;
+  static constexpr int kBufs = STAGE_ES == 0 ? 0 : (kTileBytes > 32 * 1024 ? 1 : 2);
+  // N = 256: the tile's BLOCK_N bias floats (and an e4m3 input's dq floats) are staged after the kBufs tiles, one set per
+  // buffer: the consumers hold 128 accumulators and have no registers for batched loads of them
+  static constexpr bool kSBias = BLOCK_N == 256 && kBufs > 0;
+  static constexpr uint32_t kBiasBytes = kSBias ? BLOCK_N * 4 * (STAGE_DQ ? 2 : 1) : 0;
+  static constexpr uint32_t kTileReserve = 1024 - kBarBytes + kBufs * (kTileBytes + kBiasBytes);
   __host__ __device__ static constexpr int ring_stages(uint32_t reserve) {
     const int s = int(kSmemBudget - reserve) / int(kStageBytes);
     return s > kMaxStages ? kMaxStages : s;
@@ -100,9 +96,8 @@ struct Cfg {
   static constexpr uint32_t kSwizzleBytes = BLOCK_K * 2;  // 32 / 64 / 128: one smem row of an operand tile
   static constexpr uint32_t kSbo = 8 * kSwizzleBytes;
   // Shared-memory layout from the 1 KB-aligned base, as conv_tc_kernel lays it out: A ring, then B ring or resident
-  // weights, then the mbarriers (bar_offset), then `reserve` bytes: the output tile and the bias (kStaged launches,
-  // kOutBytes) or the two TMA output tiles (kPairBytes).  launch_cfg checks smem_end() against the allocation before
-  // every launch.
+  // weights, then the mbarriers (bar_offset), then `reserve` bytes: the output tiles, bias and dq of a tile_tma launch
+  // (kTileReserve).  launch_cfg checks smem_end() against the allocation before every launch.
   __host__ __device__ static constexpr uint32_t bar_offset(int stages, bool bres, int b_steps) {
     return uint32_t(stages) * kABytes + (bres ? bres_bytes(b_steps) : uint32_t(stages) * kTaps * kBBytes);
   }
@@ -110,7 +105,7 @@ struct Cfg {
     return bar_offset(stages, bres, b_steps) + kBarBytes + reserve;
   }
   static constexpr size_t kSmemBytes = size_t(kSmemBudget) + 1024 /*align*/ + kBarBytes;
-  static_assert(ring_stages(kStaged ? kOutBytes : (kPair ? kPairBytes : 0u)) >= 2, "pipeline needs at least two stages");
+  static_assert(ring_stages(kTileReserve) >= 2, "pipeline needs at least two stages");
   static_assert(!HALO || BLOCK_K >= 32, "halo reuse: rows of 64 or 128 bytes");
 };
 
@@ -132,11 +127,6 @@ __device__ __forceinline__ float bias_act_dq(float a, float s, float b, bool sil
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(h));
   return fmaf(h, t, h);
 }
-
-__device__ __forceinline__ void cp_async16(uint32_t saddr, const void* gptr) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(saddr), "l"(gptr) : "memory");
-}
-__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
 // exact n / d for any 32-bit n with a precomputed (multiplier, shift) pair (host: fast_div_for)
 __device__ __forceinline__ uint32_t fast_div(uint32_t n, uint32_t mul, uint32_t shr) {
@@ -221,20 +211,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_b + (bres ? C::bres_bytes(b_steps) : uint32_t(STAGES) * kBStage));
   uint64_t* empty_bar = full_bar + C::kMaxStages;
   uint64_t* bres_bar = empty_bar + C::kMaxStages;
-  // [b]: output tile buffer b (kPair launches use two, kStaged launches buffer 0)
+  // [b]: output tile buffer b (at most two)
   uint64_t* staged_bar = bres_bar + 1;  // store warp -> consumers: the tile's residual (and bias) are in shared memory
   uint64_t* done_bar = bres_bar + 3;    // consumers -> store warp: the finished tile is in shared memory
-  // output tile: word (h * BLOCK_N / 8 + j) * 256 + t holds consumer thread t's column pair j of its row m0 + 8 h (the
-  // residual pair before the consumers finish the tile, the output pair after).  Lanes 4 r .. 4 r + 3 of a consumer warp
-  // hold 8 consecutive columns of one row, so 16 bytes at word (h * BLOCK_N / 8 + j) * 256 + 32 w + 4 r are 8 channels of
-  // one row of warp w
-  uint32_t* stile = reinterpret_cast<uint32_t*>(reinterpret_cast<uint8_t*>(full_bar) + C::kBarBytes);
-  float* sbias = reinterpret_cast<float*>(stile + C::kTileBytes / 4);
-  float* sdq = sbias + BLOCK_N;  // e4m3 input (Cfg STAGE_DQ)
-  const bool staged_out = C::kStaged && p.out_f32 == nullptr;
-  // two output tiles (Cfg::kPair), 1 KB aligned for the 128-byte swizzle
-  uint8_t* ptile = reinterpret_cast<uint8_t*>(full_bar) + 1024;
-  const bool pair_out = C::kPair && p.tile_tma != 0;
+  // Cfg::kBufs output tiles, 1 KB aligned for the 128-byte swizzle, then (Cfg::kSBias) buffer b's bias floats at
+  // otile + kBufs * kTileBytes + b * kBiasBytes, followed by its dq floats (e4m3 input)
+  uint8_t* otile = reinterpret_cast<uint8_t*>(full_bar) + 1024;
+  const bool tile_out = C::kBufs > 0 && p.tile_tma != 0;
+  constexpr int kBufs = C::kBufs > 0 ? C::kBufs : 1;  // buffer cycle of tile_out launches (the divisor, never 0)
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -242,7 +226,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    if (pair_out) {
+    if (tile_out) {
       tma_prefetch_desc(&map_out);
       if (p.res) tma_prefetch_desc(&map_res);
     }
@@ -252,9 +236,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     }
     mbar_init(bres_bar, 1);
     for (int b = 0; b < 2; ++b) {
-      // kStaged: every store-warp lane, after its own copies have landed; kPair: the store warp's one TMA issuing lane
-      mbar_init(&staged_bar[b], pair_out ? 1 : 32);
-      mbar_init(&done_bar[b], 8);  // one arrival per consumer warp
+      mbar_init(&staged_bar[b], 1);  // the store warp's one TMA issuing lane
+      mbar_init(&done_bar[b], 8);    // one arrival per consumer warp
     }
     fence_mbar_init();
   }
@@ -353,11 +336,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       run(std::integral_constant<int, 1>{});
   } else if (warp == kStoreWarp) {
     // ------------------------------------------------------------------ store warp
-    if (pair_out) {
-      // N <= 128 (kPair): lane 0 moves whole tiles with the bulk-copy engine.  Tile i of this CTA uses buffer i & 1: its
-      // residual is loaded while the consumers run tile i - 1 or i - 2, and the buffer is restaged for tile i + 2 as soon
-      // as tile i's store has finished reading it.  With res == out (training dgrad) a tile's residual is loaded before
-      // that tile is stored, and tiles are disjoint.
+    if (tile_out) {
+      // Lane 0 moves whole tiles with the bulk-copy engine.  Tile i of this CTA uses buffer i % kBufs: its residual (and
+      // bias) is loaded while the consumers run the earlier tiles, and the buffer is restaged for tile i + kBufs as soon as
+      // tile i's store has finished reading it.  With one buffer that is after `done` of tile i, so the consumers have
+      // also read tile i's bias before the next tile's overwrites it.  With res == out (training dgrad) a tile's residual
+      // is loaded before that tile is stored, and tiles are disjoint.
       if (lane != 0) return;
       const uint32_t res_tx = uint32_t(p.mode == 0 ? kBlockM : p.tw * p.th) * C::kRowBytes;  // out-of-range parts count
       constexpr int kBoxCh = C::kBoxBytes / kOes;
@@ -374,7 +358,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
 #pragma unroll
         for (uint32_t k = 0; k < C::kBoxes; ++k) {
-          uint8_t* s = ptile + b * C::kTileBytes + k * kBlockM * C::kBoxBytes;
+          uint8_t* s = otile + b * C::kTileBytes + k * kBlockM * C::kBoxBytes;
           const int c0 = (load ? p.res_coff : p.out_coff) + n0 + int(k) * kBoxCh;
           if (load) {
             if (p.mode == 0) tma_load_2d(s, &map_res, &staged_bar[b], c0, c1);
@@ -386,126 +370,38 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         }
       };
       auto stage = [&](int tile, int b) {
-        if (p.res) {
-          mbar_expect_tx(&staged_bar[b], res_tx);
-          move(tile, b, true);
-        } else {
+        // N = 256: the bias (and dq) floats of the tile's channels below c_out, a multiple of 32 floats
+        const int n0 = (tile % p.n_tiles) * BLOCK_N;
+        const uint32_t bias_tx = C::kSBias ? uint32_t(min(BLOCK_N, p.cout - n0)) * 4u : 0u;
+        const uint32_t tx = (p.res ? res_tx : 0u) + bias_tx * (kInE4m3 ? 2u : 1u);
+        if (tx == 0) {
           mbar_arrive(&staged_bar[b]);
+          return;
+        }
+        mbar_expect_tx(&staged_bar[b], tx);
+        if (p.res) move(tile, b, true);
+        if constexpr (C::kSBias) {
+          uint8_t* sb = otile + C::kBufs * C::kTileBytes + b * C::kBiasBytes;
+          bulk_load(sb, p.bias + n0, bias_tx, &staged_bar[b]);
+          if (kInE4m3) bulk_load(sb + BLOCK_N * 4, p.dq + n0, bias_tx, &staged_bar[b]);
         }
       };
       const int step = int(gridDim.x);
-      if (int(blockIdx.x) < total_tiles) stage(blockIdx.x, 0);
-      if (int(blockIdx.x) + step < total_tiles) stage(blockIdx.x + step, 1);
+#pragma unroll
+      for (int i = 0; i < kBufs; ++i)
+        if (int(blockIdx.x) + i * step < total_tiles) stage(blockIdx.x + i * step, i);
       for (int tile = blockIdx.x, i = 0; tile < total_tiles; tile += step, ++i) {
-        const int b = i & 1;
-        mbar_wait(&done_bar[b], uint32_t(i >> 1) & 1u, p.err, 9);  // the consumers have finished tile i in buffer b
+        const int b = i % kBufs;
+        // the consumers have finished tile i in buffer b
+        mbar_wait(&done_bar[b], uint32_t(i / kBufs) & 1u, p.err, 9);
         move(tile, b, false);
         bulk_commit_group();
-        if (tile + 2 * step < total_tiles) {
+        if (tile + kBufs * step < total_tiles) {
           bulk_wait_read_all();  // the store has read buffer b
-          stage(tile + 2 * step, b);
+          stage(tile + kBufs * step, b);
         }
       }
       bulk_wait_all();  // the output is in global memory before the grid completes (the next grid's griddepcontrol.wait)
-      return;
-    }
-    if (!staged_out) return;
-    // lane = 8 c + r: row r of 8 rows of one consumer warp's block, chunk c of 4 consecutive 16-byte chunks.  Each quarter
-    // warp reads 128 contiguous bytes of the tile (no bank conflict) and each row gets a 64-byte global segment.
-    const int r = lane & 7, c = lane >> 3;
-    const uint32_t stile_s = smem_u32(stile);
-    // The destinations of a tile's 128 rows are computed once, four per lane (rows lane + 32 q), before the tile is
-    // finished; the drain and the staging fetch them by shuffle.  Row (w >> 2) * 64 + (w & 3) * 16 + 8 h + r of the
-    // (h, w) loops below sits in slot q = 2 (w >> 2) + ((w & 3) >> 1) of lane 16 (w & 1) + 8 h + r.
-    struct Rows {
-      __nv_bfloat16* out[4];
-      const __nv_bfloat16* res[4];
-    };
-    auto rows_of = [&](int tile, Rows& R) {
-      const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BLOCK_N;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const RowOut ro = row_out<kOes>(p, mt, n0, 32 * q + lane);
-        R.out[q] = ro.out;
-        R.res[q] = ro.res;
-      }
-    };
-    // 16-byte chunk j of a row: channels [kCh j, kCh j + kCh)
-    constexpr int kCh = 16 / kOes, kRowChunks = BLOCK_N / kCh;
-    auto chunk = [&](int h, int w, int j) { return uint32_t((h * kRowChunks + j) * 64 + w * 8 + r); };  // 16-byte index
-    auto src_lane = [&](int h, int w) { return (w & 1) * 16 + 8 * h + r; };
-    auto stage_bias = [&](int tile) {
-      const int n0 = (tile % p.n_tiles) * BLOCK_N;
-      for (int i = lane; i < BLOCK_N / 4; i += 32)
-        if (n0 + 4 * i < p.cout) {
-          cp_async16(smem_u32(sbias + 4 * i), p.bias + n0 + 4 * i);
-          if (kInE4m3) cp_async16(smem_u32(sdq + 4 * i), p.dq + n0 + 4 * i);
-        }
-    };
-    // With res == out (training dgrad) a tile's residual is read before that tile is written, and tiles are disjoint.
-    // c_out % 32 == 0: a group of 4 chunks is either inside c_out or outside.
-    auto stage_res = [&](int tile, const Rows& R) {
-      const int n0 = (tile % p.n_tiles) * BLOCK_N;
-      if (p.res) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int w = 0; w < 8; ++w) {
-            const auto* res = reinterpret_cast<const __nv_bfloat16*>(
-                __shfl_sync(~0u, reinterpret_cast<unsigned long long>(R.res[2 * (w >> 2) + ((w & 3) >> 1)]), src_lane(h, w)));
-            if (!res) continue;
-#pragma unroll 1
-            for (int jg = 0; jg < kRowChunks / 4; ++jg) {
-              const int j = 4 * jg + c;
-              // bf16: a group of 4 chunks (32 channels) is inside c_out or outside; e4m3: each chunk of 16 is
-              if (kOutE4m3 ? n0 + kCh * j < p.cout : n0 + 32 * jg < p.cout)
-                cp_async16(stile_s + 16u * chunk(h, w, j), elem_ptr<kOes>(res, kCh * j));
-            }
-          }
-      }
-      cp_async_wait_all();
-      mbar_arrive(staged_bar);
-    };
-    auto drain = [&](int tile, const Rows& R) {
-      const int n0 = (tile % p.n_tiles) * BLOCK_N;
-      const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
-      const int reps = p.upsample ? 4 : 1;
-      const uint4* tile16 = reinterpret_cast<const uint4*>(stile);
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int w = 0; w < 8; ++w) {
-          auto* out = reinterpret_cast<__nv_bfloat16*>(
-              __shfl_sync(~0u, reinterpret_cast<unsigned long long>(R.out[2 * (w >> 2) + ((w & 3) >> 1)]), src_lane(h, w)));
-          if (!out) continue;
-#pragma unroll 2
-          for (int jg = 0; jg < kRowChunks / 4; ++jg) {
-            const int j = 4 * jg + c;
-            if (kOutE4m3 ? n0 + kCh * j >= p.cout : n0 + 32 * jg >= p.cout) break;
-            const uint4 v = tile16[chunk(h, w, j)];
-            for (int rep = 0; rep < reps; ++rep)
-              *reinterpret_cast<uint4*>(elem_ptr<kOes>(out, (rep >> 1) * up_row_stride + (rep & 1) * p.out_ld + kCh * j)) = v;
-          }
-        }
-    };
-    uint32_t tphase = 0;
-    Rows cur, nxt;
-    if (int(blockIdx.x) < total_tiles) {
-      rows_of(blockIdx.x, cur);
-      stage_bias(blockIdx.x);
-      stage_res(blockIdx.x, cur);
-    }
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      const int next = tile + int(gridDim.x);
-      if (next < total_tiles) rows_of(next, nxt);  // while the consumers run the tile's main loop
-      mbar_wait(done_bar, tphase, p.err, 7);      // the consumers have finished the tile
-      tphase ^= 1u;
-      if (next < total_tiles) stage_bias(next);   // the consumers have read this tile's bias; lands during the drain
-      drain(tile, cur);
-      // each lane overwrites only chunks it has just read into registers, and the consumers wait on `staged` before
-      // they write the next tile
-      if (next < total_tiles) stage_res(next, nxt);
-      cur = nxt;
     }
   } else {
     // ------------------------------------------------------------------ consumers: wgmma + epilogue (warpgroups 0, 1)
@@ -515,9 +411,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     constexpr uint32_t kDescHi = wgmma_desc_hi(C::kSbo, C::kSwizzleBytes);
     const uint32_t a_base = smem_u32(smem_a) + uint32_t(wg) * 64u * C::kSwizzleBytes;
     const uint32_t b_base = smem_u32(smem_b);
-    uint32_t stage = 0, phase = 0, tphase = 0;
+    uint32_t stage = 0, phase = 0;
     if (bres && int(blockIdx.x) < total_tiles) mbar_wait(bres_bar, 0, p.err, 6);  // resident weights have landed
-    for (int tile = blockIdx.x, ti = 0; tile < total_tiles; tile += gridDim.x, ++ti) {
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       float acc[BLOCK_N / 2];
       uint32_t prev = 0;
       for (int it = 0; it < k_iters; ++it) {
@@ -553,88 +449,36 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       // the main loop)
       const bool silu = p.act == Y3_ACT_SILU;
       const float bscale = silu ? 0.5f : 1.0f;
-      if (staged_out) {
-        // Every column pair of every row goes through the tile: the store warp drops halo rows and columns past c_out
-        // (their bias and residual words were never staged).
-        mbar_wait(staged_bar, tphase, p.err, 8);  // the tile's residual and bias have landed
-        tphase ^= 1u;
-        const bool has_res = p.res != nullptr;
-        if constexpr (kOutE4m3) {
-          // this thread's column pair j of row m0 + 8 h: bytes (j & 1) * 8 + cq of 16-byte chunk j / 2 of that row (the
-          // residual pair before, the output pair after; channel order, as the store warp copies it)
-          uint8_t* tb = reinterpret_cast<uint8_t*>(stile) + ((warp * 8 + (lane >> 2)) * 16 + cq);
-#pragma unroll
-          for (int j = 0; j < BLOCK_N / 8; ++j) {
-            const float2 b = *reinterpret_cast<const float2*>(sbias + 8 * j + cq);
-            float2 q = b;
-            if (kInE4m3) q = *reinterpret_cast<const float2*>(sdq + 8 * j + cq);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              uint16_t& hw = *reinterpret_cast<uint16_t*>(tb + (h * BLOCK_N / 16 + j / 2) * 64 * 16 + (j & 1) * 8);
-              float x0, x1;
-              if (kInE4m3) {
-                x0 = bias_act_dq(acc[4 * j + 2 * h], bscale * q.x, bscale * b.x, silu);
-                x1 = bias_act_dq(acc[4 * j + 2 * h + 1], bscale * q.y, bscale * b.y, silu);
-              } else {
-                x0 = bias_act(acc[4 * j + 2 * h], bscale * b.x, silu);
-                x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b.y, silu);
-              }
-              if (has_res) {
-                const float2 f = unpack_e4m3x2(hw);
-                x0 = fmaf(p.res_scale, f.x, x0);
-                x1 = fmaf(p.res_scale, f.y, x1);
-              }
-              hw = pack_e4m3x2(x0 * p.out_inv_scale, x1 * p.out_inv_scale);
-            }
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(done_bar);
-          continue;
-        }
-        uint32_t* words = stile + threadIdx.x;
-#pragma unroll
-        for (int j = 0; j < BLOCK_N / 8; ++j) {
-          const float2 b = *reinterpret_cast<const float2*>(sbias + 8 * j + cq);
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            uint32_t& word = words[(h * BLOCK_N / 8 + j) * 256];
-            float x0 = bias_act(acc[4 * j + 2 * h], bscale * b.x, silu);
-            float x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * b.y, silu);
-            if (has_res) {
-              const float2 f = unpack_bf16x2(word);
-              x0 += f.x;
-              x1 += f.y;
-            }
-            word = pack_bf16x2(x0, x1);
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(done_bar);
-      } else if (pair_out) {
-        // N <= 128 (kPair): finish the tile in buffer ti & 1, in place over its residual, with the arithmetic of the
-        // register epilogue below.  Every column pair is written; the TMA store clips columns past c_out and pixels outside
-        // the output.  Flat mode: halo rows get zeros, so the halo stays zero.
+      if (tile_out) {
+        // Finish the tile in buffer ti % kBufs, in place over its residual, with the arithmetic of the register epilogue
+        // below.  Every column pair is written; the TMA store clips columns past c_out and pixels outside the output.
+        // Flat mode: halo rows get zeros, so the halo stays zero.
         // Bank conflicts: a warp's 32 lanes access rows m0 .. m0 + 7 (m0 % 8 == 0) at lanes 4 r .. 4 r + 3, each quad a
         // contiguous 8 (bf16) or 4 (e4m3) bytes inside one 16-byte chunk of its row.  128-byte boxes: the 8 rows are 8
         // different 128-byte lines, i.e. the same 32 banks, and the swizzle puts row r's chunk at c ^ r: 8 different
         // chunks, 32 different banks (e4m3: 16 banks, two lanes per word).  64-byte boxes: rows 2 s and 2 s + 1 share a
         // line at byte 64 (r & 1) and the chunk is c ^ (r >> 1): again 8 different 16-byte bank groups.  32-byte boxes
         // (e4m3 N = 32): rows r and r + 4 share bank group 8 (r & 3) and differ in the chunk (c ^ (r >> 2)).
-        const int b = ti & 1;
-        mbar_wait(&staged_bar[b], uint32_t(ti >> 1) & 1u, p.err, 10);  // the tile's residual has landed, the buffer is free
-        uint8_t* tb = ptile + b * C::kTileBytes;
+        // this CTA's tile index, derived here rather than kept in a register through the main loop (N = 256 has none)
+        const int ti = (tile - int(blockIdx.x)) / int(gridDim.x);
+        const int b = ti % kBufs;
+        // the tile's residual (and bias) has landed, the buffer is free
+        mbar_wait(&staged_bar[b], uint32_t(ti / kBufs) & 1u, p.err, 10);
         const int n0 = (tile % p.n_tiles) * BLOCK_N;
         const bool has_res = p.res != nullptr;
-        uint32_t rowoff[2], sw[2];
-        bool valid[2];
+        // Rows m0 and m0 + 8 lie 8 x kBoxBytes apart and share the swizzle term: (m * kBoxBytes / 128) mod (kBoxBytes / 16)
+        // changes by 8 kBoxBytes / 128 = kBoxBytes / 16, i.e. not at all.  The term and the in-box chunk offsets occupy
+        // address bits [4, log2 kBoxBytes), which are zero in the row's base and untouched by the region and row offsets,
+        // so the term is XOR-ed into the base once and each column group XORs its chunk offset into that (the buffer
+        // offset, a multiple of 1 KB, is added after: the XOR-ed base is then the same for every tile).
+        const uint32_t sw = ((uint32_t(m0) * C::kBoxBytes >> 7) & (C::kBoxBytes / 16 - 1)) << 4;
+        const uint32_t row_s = ((smem_u32(otile) + uint32_t(m0) * C::kBoxBytes + cq * kOes) ^ sw) + b * C::kTileBytes;
+        const uint32_t bias_s = smem_u32(otile) + C::kBufs * C::kTileBytes + b * C::kBiasBytes + cq * 4;  // Cfg::kSBias
+        bool valid[2] = {true, true};
+        if (p.mode == 0) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int m = m0 + 8 * h;
-          rowoff[h] = uint32_t(m) * C::kBoxBytes;
-          sw[h] = ((rowoff[h] >> 7) & (C::kBoxBytes / 16 - 1)) << 4;
-          valid[h] = true;
-          if (p.mode == 0) {
-            const int row = (tile / p.n_tiles) * kBlockM + m;
+          for (int h = 0; h < 2; ++h) {
+            const int row = (tile / p.n_tiles) * kBlockM + m0 + 8 * h;
             const int img = static_cast<int>(fast_div(static_cast<uint32_t>(row), p.plane_mul, p.plane_shr));
             const int rem = row - img * (p.hp * p.wp);
             const int yp = static_cast<int>(fast_div(static_cast<uint32_t>(rem), p.wp_mul, p.wp_shr)), xp = rem - yp * p.wp;
@@ -644,15 +488,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 #pragma unroll
         for (int j = 0; j < BLOCK_N / 8; ++j) {
           const int c = 8 * j + cq;
-          const bool in = n0 + c < p.cout;  // c_out % 32 == 0: a column pair is either inside or outside
-          const float2 bv = in ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
-          float2 qv = bv;
-          if (kInE4m3) qv = in ? __ldg(reinterpret_cast<const float2*>(p.dq + n0 + c)) : make_float2(0.f, 0.f);
+          float2 bv, qv;
+          if constexpr (C::kSBias) {  // staged beside the buffer (entries past c_out are stale: their columns are clipped)
+            bv = lds_f32x2(bias_s + 32 * j);
+            qv = kInE4m3 ? lds_f32x2(bias_s + 4 * BLOCK_N + 32 * j) : bv;
+          } else {
+            const bool in = n0 + c < p.cout;  // c_out % 32 == 0: a column pair is either inside or outside
+            bv = in ? __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c)) : make_float2(0.f, 0.f);
+            qv = bv;
+            if (kInE4m3) qv = in ? __ldg(reinterpret_cast<const float2*>(p.dq + n0 + c)) : make_float2(0.f, 0.f);
+          }
           const uint32_t xb = uint32_t(8 * j * kOes);  // byte of column 8 j in the row
           const uint32_t region = xb / C::kBoxBytes * (kBlockM * C::kBoxBytes), xin = xb % C::kBoxBytes;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            uint8_t* pp = tb + region + rowoff[h] + (xin ^ sw[h]) + cq * kOes;
+            const uint32_t pp = (row_s ^ xin) + region + 8 * h * C::kBoxBytes;
             float x0, x1;
             if (kInE4m3) {
               x0 = bias_act_dq(acc[4 * j + 2 * h], bscale * qv.x, bscale * bv.x, silu);
@@ -662,21 +512,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
               x1 = bias_act(acc[4 * j + 2 * h + 1], bscale * bv.y, silu);
             }
             if constexpr (kOutE4m3) {
-              uint16_t& hw = *reinterpret_cast<uint16_t*>(pp);
               if (has_res) {
-                const float2 f = unpack_e4m3x2(hw);
+                const float2 f = unpack_e4m3x2(lds16(pp));
                 x0 = fmaf(p.res_scale, f.x, x0);
                 x1 = fmaf(p.res_scale, f.y, x1);
               }
-              hw = valid[h] ? pack_e4m3x2(x0 * p.out_inv_scale, x1 * p.out_inv_scale) : uint16_t(0);
+              sts16(pp, valid[h] ? pack_e4m3x2(x0 * p.out_inv_scale, x1 * p.out_inv_scale) : uint16_t(0));
             } else {
-              uint32_t& word = *reinterpret_cast<uint32_t*>(pp);
               if (has_res) {
-                const float2 f = unpack_bf16x2(word);
+                const float2 f = unpack_bf16x2(lds32(pp));
                 x0 += f.x;
                 x1 += f.y;
               }
-              word = valid[h] ? pack_bf16x2(x0, x1) : 0u;
+              sts32(pp, valid[h] ? pack_bf16x2(x0, x1) : 0u);
             }
           }
         }
@@ -689,17 +537,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         // res == out), so the compiler keeps every residual load behind the stores that precede it in program order.
         // Loading a whole chunk of column pairs (bias and residual) before the first store of that chunk makes it one trip
         // to memory per chunk instead of one per column pair.  Correct with res == out: a thread reads exactly the
-        // elements it then overwrites, and tiles are disjoint.  (N = 256 only comes here for the fp32 heads, which have no
-        // residual, and has no registers left for a chunk.)
+        // elements it then overwrites, and tiles are disjoint.  (N = 256 has no registers left for a chunk.)
         const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BLOCK_N;
-        const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
-        const int reps = p.upsample ? 4 : 1;
         // column pairs per batch (an e4m3 input also holds the batch's dq pairs: half the batch at N = 128 keeps 0 spills)
         constexpr int kChunk = BLOCK_N == 256 ? 1 : (kInE4m3 && BLOCK_N == 128 ? 8 : (BLOCK_N / 8 < 16 ? BLOCK_N / 8 : 16));
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const RowOut ro = row_out<kOes>(p, mt, n0, m0 + 8 * h);
           if (!ro.f32 && !ro.out) continue;
+          // per row: nothing but the accumulators and the row's pointers stays live from one row to the next
+          const long long up_row_stride = static_cast<long long>(2 * (p.mode == 0 ? p.wp - 2 : p.wo) + 2) * p.out_ld;
+          const int reps = p.upsample ? 4 : 1;
 #pragma unroll
           for (int j0 = 0; j0 < BLOCK_N / 8; j0 += kChunk) {
             float2 b[kChunk], q[kChunk];
@@ -767,10 +615,8 @@ int launch_cfg(const ConvTcPlan& plan, cudaStream_t stream) {
     attr_set = true;
   }
   ConvTcArgs args = plan.args;
-  // as the kernel decides (staged_out, pair_out)
-  const bool out_tile = C::kStaged && args.out_f32 == nullptr;
-  const bool pair = C::kPair && args.tile_tma != 0;
-  const uint32_t reserve = out_tile ? C::kOutBytes : (pair ? C::kPairBytes : 0u);
+  // as the kernel decides (tile_out)
+  const uint32_t reserve = (C::kBufs > 0 && args.tile_tma != 0) ? C::kTileReserve : 0u;
   const int b_steps = args.taps * args.kblocks;
   args.bres = plan.bres;
   args.stages = plan.bres ? C::bres_stages(b_steps, reserve) : C::ring_stages(reserve);
@@ -883,7 +729,8 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
   }
   if (out8) {
     Y3_REQUIRE(d.out_inv_scale > 0.f, "conv: an e4m3 output needs out_inv_scale > 0");
-    // the N = 256 store warp moves 16-byte chunks of 16 e4m3 channels (output and staged residual)
+    // the output and residual tiles move by TMA, whose row pitches are multiples of 16 bytes; the channel offsets keep the
+    // same 16-channel grain
     Y3_REQUIRE(d.out_ld % 16 == 0 && d.out_coff % 16 == 0, "conv: an e4m3 output needs out_ld and out_coff %% 16 == 0");
     if (d.res)
       Y3_REQUIRE(d.res_ld % 16 == 0 && d.res_coff % 16 == 0 && d.res_scale > 0.f,
@@ -1027,11 +874,11 @@ int conv_tc_prepare(const y3_conv_desc& d, ConvTcPlan* plan, bool select_only, c
     rc = select_only ? Y3_OK : encode_tensor_map(&plan->map_b, d.in_fmt, d.weight, 2, dims, strides, box, bk * 2);
     if (rc) return rc;
   }
-  // N <= 128 tiles leave through a TMA store (and load their residual by TMA) unless they are upsampled (a 2 x 2
+  // bf16 / e4m3 output tiles leave through a TMA store (and load their residual by TMA) unless they are upsampled (a 2 x 2
   // replicated write is not one box) or one parity class of a transposed conv (every other pixel)
   plan->map_out = CUtensorMap{};
   plan->map_res = CUtensorMap{};
-  a.tile_tma = (!head && bn <= 128 && !d.upsample && !(extra && extra->phase)) ? 1 : 0;
+  a.tile_tma = (!head && !d.upsample && !(extra && extra->phase)) ? 1 : 0;
   if (a.tile_tma && !select_only) {
     // rows of bn output elements in boxes of at most 128 bytes (the kernel's Cfg::kBoxBytes), swizzled to the box width.
     // The channel extent ends at coff + c_out, so the store never touches the neighbouring slice of a Concat buffer.

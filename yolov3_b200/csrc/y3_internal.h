@@ -73,7 +73,7 @@ struct ConvTcArgs {
   // FP8 (y3_conv_desc): per-channel dequantisation of an e4m3 input, residual scale and output scale of an e4m3 output
   const float* dq;
   float res_scale, out_inv_scale;
-  // 1: N <= 128 tile with a bf16 / e4m3 output that is neither upsampled nor a parity class: the tile is finished in
+  // 1: a tile with a bf16 / e4m3 output that is neither upsampled nor a parity class: the tile is finished in
   // shared memory and leaves through the map_out TMA store, its residual arrives through map_res (ConvTcPlan)
   int tile_tma;
 };
