@@ -189,7 +189,10 @@ typedef struct y3_decode_desc {
   float* z;                         /* [bs, sum_l na*ny*nx, no] or NULL (training: logits only) */
 } y3_decode_desc;
 /* Fused head transpose + decode used by the graph executor: one pass from the head convs' pixel-major fp32 output to
- * z and to the reference-layout logits. */
+ * z and to the reference-layout logits.  no = nc + 5 may be 5..Y3_MAX_DECODE_NO (nc <= 1024, the NMS limit): rows of up
+ * to 256 elements go through register-array kernels that walk 4 z rows per warp, wider rows through a kernel that walks
+ * one z row per warp. */
+#define Y3_MAX_DECODE_NO 1029
 int y3_detect_head_decode_fwd(const y3_decode_desc* d, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
@@ -317,8 +320,9 @@ typedef struct y3_pack_item {
 int y3_pack_dgrad_batched(const y3_pack_item* items_dev, int32_t n_items, const void* wbf, int32_t total_tiles,
                           y3_stream_t stream);
 /* Detect-head gradient: g = dL/draw fp32 [n, na, ny, nx, no] (ComputeLoss output) -> dy bf16 padded NHWC channel a*no+o
- * (the head conv's output order; channels >= na*no zeroed) and partial[y3_bn_partial_blocks(n, ny, 0, 0)][256] column sums
- * (bias gradient = y3_colreduce_f32 over them). */
+ * (the head conv's output order; channels >= na*no zeroed) and partial[y3_bn_partial_blocks(n, ny, 0, 0)][W256] column sums
+ * (bias gradient = y3_colreduce_f32 over them), W = dy_ld - dy_coff >= na*no, W256 = W rounded up to a multiple of 256
+ * (256 for every head of at most 80 classes and 3 anchors). */
 int y3_head_grad_pack(const float* g, int32_t n, int32_t na, int32_t ny, int32_t nx, int32_t no, void* dy, int32_t dy_ld,
                       int32_t dy_coff, float* partial, y3_stream_t stream);
 /* dy of a stride-2 conv scattered onto the even positions of a zeroed [n, 2ho+2, 2wo+2, dst_ld] buffer */
@@ -357,7 +361,7 @@ int y3_add_nhwc(const void* src, int32_t src_ld, int32_t src_coff, void* dst, in
  * NHWC buffer, column (c*3+kh)*3+kw; lets training run layer 0 as a 1x1 conv with the generic kernels */
 int y3_im2col_first(const void* in, int32_t in_dtype, float in_div, int32_t n, int32_t h, int32_t w, void* out,
                     int32_t out_ld, int32_t out_coff, y3_stream_t stream);
-/* out[c] += sum over rows of g[row, c] (fp32 pixel-major; Detect-head bias gradients) */
+/* out[c] += sum over rows of g[row, c] (fp32 pixel-major; Detect-head bias gradients), any c (256 columns per block) */
 int y3_colsum_f32(const float* g, int32_t ld, int32_t c, int64_t rows, float* out, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------

@@ -198,6 +198,61 @@ __global__ void __launch_bounds__(256, NITER <= 3 ? 3 : 1) head_decode_kernel(co
   }
 }
 
+// Rows wider than 256 elements (no > 256: more than 251 classes, e.g. Objects365's 365).  The register arrays of
+// head_decode_kernel would need NITER > 8; here one warp walks one z row instead: every load and store instruction moves 32
+// consecutive floats of the row, kWideUnroll loads per lane are issued before the first is used, and the row descriptor
+// (image, level, anchor, cell) is warp-uniform integer work paid once per row of 257..1029 elements.
+constexpr int kWideUnroll = 8;
+
+__global__ void __launch_bounds__(256) head_decode_wide_kernel(const HeadDecodeArgs p) {
+  pdl_entry();
+  const int lane = threadIdx.x & 31;
+  const int rows_per_img = p.row_off[p.nl];
+  const int total = rows_per_img * p.bs;  // < 2^31 (checked by the launcher)
+  const int nwarps = (gridDim.x * blockDim.x) >> 5;
+  const int no = p.no;
+  for (int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; w < total; w += nwarps) {
+    const int b = w / rows_per_img;
+    const int row = w - b * rows_per_img;
+    int l = 0;
+    while (l + 1 < p.nl && row >= p.row_off[l + 1]) ++l;
+    const int r = row - p.row_off[l];
+    const int nx = p.nx[l], plane = p.ny[l] * nx;
+    const int a = r / plane, cell = r - a * plane;
+    const int y = cell / nx, x = cell - y * nx;
+    const float* src = p.head[l] + (static_cast<long long>(b) * plane + cell) * p.head_ld[l] + a * no;
+    float* raw = p.raw[l] ? p.raw[l] + ((static_cast<long long>(b) * p.na + a) * plane + cell) * no : nullptr;
+    float* dst = p.z ? p.z + static_cast<long long>(w) * no : nullptr;
+    const float stride = p.stride[l], aw = p.anchor_w[l][a], ah = p.anchor_h[l][a];
+    for (int k0 = 0; k0 < no; k0 += 32 * kWideUnroll) {
+      float v[kWideUnroll];
+#pragma unroll
+      for (int u = 0; u < kWideUnroll; ++u) {
+        const int k = k0 + u * 32 + lane;
+        v[u] = k < no ? __ldg(src + k) : 0.f;
+      }
+#pragma unroll
+      for (int u = 0; u < kWideUnroll; ++u) {
+        const int k = k0 + u * 32 + lane;
+        if (k >= no) continue;
+        if (raw) raw[k] = v[u];
+        if (dst) {
+          const float s = sigmoid_fast(v[u]);
+          float o = s;
+          if (k < 4) {
+            const float t2 = s * 2.0f;
+            if (k < 2)
+              o = (t2 + (static_cast<float>(k == 0 ? x : y) - 0.5f)) * stride;
+            else
+              o = (t2 * t2) * (k == 2 ? aw : ah);
+          }
+          dst[k] = o;
+        }
+      }
+    }
+  }
+}
+
 }  // namespace
 }  // namespace y3
 
@@ -239,9 +294,23 @@ extern "C" int y3_detect_head_decode_fwd(const y3_decode_desc* d, y3_stream_t st
                "head_decode: level %d too large", l);
   }
   Y3_REQUIRE(d->na <= 8 && d->nl <= 8, "head_decode: na/nl > 8");
-  const int niter = (y3::kDecodeRows * d->no + 127) / 128;
-  Y3_REQUIRE(niter <= 8, "head_decode: no=%d > 256 is not supported", d->no);
+  Y3_REQUIRE(d->no <= Y3_MAX_DECODE_NO, "head_decode: no=%d > %d (nc > 1024) is not supported", d->no, Y3_MAX_DECODE_NO);
   const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int niter = (y3::kDecodeRows * d->no + 127) / 128;
+  if (niter > 8) {  // no > 256: one warp per z row; the grid is one resident wave that walks the rows
+    static int per_sm = 0;  // benign race: every thread computes the same value
+    if (per_sm == 0) {
+      Y3_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, y3::head_decode_wide_kernel, 256, 0));
+      if (per_sm < 1) per_sm = 1;
+    }
+    const long long rows = static_cast<long long>(off) * d->bs;
+    long long wblocks = (rows + 7) / 8;
+    const long long wcap = static_cast<long long>(y3::num_sms()) * per_sm;
+    if (wblocks > wcap) wblocks = wcap;
+    Y3_CHECK_CUDA(::y3::launch_pdl(y3::head_decode_wide_kernel, dim3(static_cast<unsigned>(wblocks)), dim3(256), 0, st, a));
+    Y3_CHECK_CUDA(cudaGetLastError());
+    return Y3_OK;
+  }
   const unsigned g = static_cast<unsigned>(blocks);
   switch (niter) {
     case 1: Y3_CHECK_CUDA(::y3::launch_pdl(y3::head_decode_kernel<1>, dim3(g), dim3(256), 0, st, a)); break;

@@ -670,11 +670,13 @@ __global__ void __launch_bounds__(128) wgrad_kernel(const WgradArgs p) {
 }
 
 // ---------------------------------------------------------------------------------------------- bias_grad (fp32 head grads)
-// g: fp32 pixel-major [rows, ld]; db[c] += sum_rows g[row, c]
+// g: fp32 pixel-major [rows, ld]; db[c] += sum_rows g[row, c].  Column block blockIdx.y covers columns
+// [256*blockIdx.y, 256*blockIdx.y + cb), cb = min(256, c - 256*blockIdx.y); its threads split into 256/cb row lanes.
 __global__ void __launch_bounds__(256) colsum_f32_kernel(const float* __restrict__ g, int ld, int c, long long rows,
                                                          int rows_per_block, float* __restrict__ db) {
   pdl_entry();
-  const int col = threadIdx.x % c, rl = threadIdx.x / c, nrl = blockDim.x / c;
+  const int c0 = blockIdx.y * 256, cb = min(256, c - c0);
+  const int col = c0 + threadIdx.x % cb, rl = threadIdx.x / cb, nrl = blockDim.x / cb;
   const long long r0 = static_cast<long long>(blockIdx.x) * rows_per_block;
   const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
   float s = 0.f;
@@ -810,11 +812,13 @@ __global__ void __launch_bounds__(256) pack_dgrad_batched_kernel(const y3_pack_i
 // ---------------------------------------------------------------------------------------------- Detect-head gradient
 // g: dL/draw fp32 [n, na, ny, nx, no] (the loss kernel's output) -> dy bf16 padded NHWC [n, ny+2, nx+2, ld], channel a*no+o
 // (the head conv's output order), plus per-block partial column sums (bias gradient; second stage = colreduce_kernel).
-// Thread t owns channel t: consecutive threads read consecutive o of one anchor (coalesced) and write consecutive channels.
+// Thread t of column block blockIdx.y owns channel blockIdx.y*256 + t: consecutive threads read consecutive o of one anchor
+// (coalesced) and write consecutive channels.  W = dy.ld - dy.coff channels are written (zero beyond na*no); partial is
+// [gridDim.x][gridDim.y*256] = [blocks][round_up(W, 256)].
 __global__ void __launch_bounds__(256) head_grad_pack_kernel(const float* __restrict__ g, int n, int na, int ny, int nx, int no,
                                                              SliceW dy, float* __restrict__ partial) {
   pdl_entry();
-  const int ch = threadIdx.x, co = na * no;
+  const int ch = blockIdx.y * 256 + threadIdx.x, co = na * no;
   const int a = ch / no, o = ch - a * no;
   float acc = 0.f;
   const int rows = n * ny;
@@ -829,7 +833,7 @@ __global__ void __launch_bounds__(256) head_grad_pack_kernel(const float* __rest
       if (ch < dy.ld - dy.coff) dy.p[(drow + x) * dy.ld + dy.coff + ch] = __float2bfloat16(v);
     }
   }
-  partial[static_cast<long long>(blockIdx.x) * 256 + ch] = acc;
+  partial[static_cast<long long>(blockIdx.x) * gridDim.y * 256 + ch] = acc;
 }
 
 int grid_for(long long total, int per_block = 256, int cap_mult = 32) {
@@ -1014,10 +1018,11 @@ extern "C" int y3_pack_dgrad_batched(const y3_pack_item* items_dev, int32_t n_it
 
 extern "C" int y3_head_grad_pack(const float* g, int32_t n, int32_t na, int32_t ny, int32_t nx, int32_t no, void* dy,
                                  int32_t dy_ld, int32_t dy_coff, float* partial, y3_stream_t stream) {
-  Y3_REQUIRE(g && dy && partial && n > 0 && na > 0 && ny > 0 && nx > 0 && no > 0 && na * no <= 256 && dy_ld - dy_coff <= 256,
-             "head_grad_pack: bad arguments (na*no <= 256)");
+  Y3_REQUIRE(g && dy && partial && n > 0 && na > 0 && ny > 0 && nx > 0 && no > 0 && dy_coff >= 0 && na * no <= dy_ld - dy_coff,
+             "head_grad_pack: bad arguments (the dy slice must hold all na*no channels)");
   const int nblk = y3_bn_partial_blocks(n, ny, 0, 0);
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::head_grad_pack_kernel, dim3(nblk), dim3(256), 0, static_cast<cudaStream_t>(stream), g, n, na, ny, nx, no, SliceW{static_cast<__nv_bfloat16*>(dy), dy_ld, dy_coff}, partial));
+  const int col_blocks = (dy_ld - dy_coff + 255) / 256;  // partial rows are round_up(dy_ld - dy_coff, 256) wide
+  Y3_CHECK_CUDA(::y3::launch_pdl(y3::head_grad_pack_kernel, dim3(nblk, col_blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), g, n, na, ny, nx, no, SliceW{static_cast<__nv_bfloat16*>(dy), dy_ld, dy_coff}, partial));
   Y3_CHECK_CUDA(cudaGetLastError());
   return Y3_OK;
 }
@@ -1087,10 +1092,11 @@ extern "C" int y3_conv_wgrad_s2_supported(int32_t h, int32_t w) { return y3::wgr
 extern "C" int y3_conv_wgrad_tap_major(int32_t c_in) { return c_in % 32 == 0 ? 1 : 0; }
 
 extern "C" int y3_colsum_f32(const float* g, int32_t ld, int32_t c, int64_t rows, float* out, y3_stream_t stream) {
-  Y3_REQUIRE(g && out && c > 0 && c <= 256 && rows > 0, "colsum: bad arguments");
+  Y3_REQUIRE(g && out && c > 0 && rows > 0, "colsum: bad arguments");
   const int rows_per_block = 1024;
   const long long blocks = (rows + rows_per_block - 1) / rows_per_block;
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::colsum_f32_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, static_cast<cudaStream_t>(stream), g, ld, c, rows, rows_per_block, out));
+  const dim3 grid(static_cast<unsigned>(blocks), static_cast<unsigned>((c + 255) / 256));
+  Y3_CHECK_CUDA(::y3::launch_pdl(y3::colsum_f32_kernel, grid, dim3(256), 0, static_cast<cudaStream_t>(stream), g, ld, c, rows, rows_per_block, out));
   Y3_CHECK_CUDA(cudaGetLastError());
   return Y3_OK;
 }

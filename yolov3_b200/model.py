@@ -26,6 +26,7 @@ from .tensors import PaddedNHWC, _stream
 
 BN_EPS = 1e-3       # ultralytics initialize_weights (called models/yolo.py:229)
 BN_MOMENTUM = 0.03
+MAX_NC = 1024       # class-count limit of the whole path: NMS (y3_nms.cu nms_bucket_kernel), decode (Y3_MAX_DECODE_NO = 1029)
 
 
 class Detect:
@@ -63,6 +64,10 @@ class Model:
             self.yaml["nc"] = nc  # models/yolo.py:207-209
         if anchors:
             self.yaml["anchors"] = round(anchors)  # models/yolo.py:210-212
+        nc_ = self.yaml["nc"]
+        if not (isinstance(nc_, int) and 1 <= nc_ <= MAX_NC):
+            raise ValueError(f"nc={nc_!r}: yolov3_b200 supports 1 <= nc <= {MAX_NC} classes (the NMS bucket kernel keeps one "
+                             f"per-class histogram slot per thread of its {MAX_NC}-thread block)")
         self.nodes, self.save = graph.parse(self.yaml, ch)
         self.ch = ch
         self.nc = self.yaml["nc"]

@@ -180,14 +180,16 @@ class TrainEngine:
             hd = dict(x=x, c1=x.c, j=j, wname=wname, bname=bname)
             hd["out"] = torch.zeros(n * x.h * x.w, head_ld, dtype=torch.float32, device=dev)
             hd["raw"] = torch.zeros(n, det.na, x.h, x.w, det.no, dtype=torch.float32, device=dev)
-            hd["wf"] = store.weight_rows_bf16(wname)                   # [256, c1]: row 255 is the zero pad row of the slot
+            hd["wf"] = store.weight_rows_bf16(wname)                   # [head_ld, c1]: rows >= na*no are the slot's zero pad rows
             hd["wd"] = torch.zeros(ops.cout_pad(x.c), head_ld, dtype=torch.bfloat16, device=dev)
             hd["bias"] = store.flat(bname, padded=True)[:head_ld]      # fp32 master bias read in place (pad entry = 0)
             hd["dy"] = buf(head_ld, x.h, x.w)
-            hd["dw"] = store.grad_rows(wname)                          # [256, 1, c1]
-            hd["db"] = store.flat(bname, grad=True, padded=True)[:head_ld]
+            hd["dw"] = store.grad_rows(wname)                          # [head_ld, 1, c1]
             hd["nblk"] = T.partial_blocks(n, x.h)
-            max_partial = max(max_partial, hd["nblk"] * 256)
+            hd["pw"] = T.head_grad_width(hd["dy"])                    # partial-row width: head_ld rounded up to 256
+            hd["db"] = store.flat(bname, grad=True, padded=True)       # the whole slot: pw entries, zero beyond na*no
+            assert hd["db"].numel() == hd["pw"]
+            max_partial = max(max_partial, hd["nblk"] * hd["pw"])
             self.heads.append(hd)
             lv = dec.levels[j]
             lv.head, lv.head_ld, lv.raw_out = hd["out"].data_ptr(), head_ld, hd["raw"].data_ptr()
@@ -406,7 +408,7 @@ class TrainEngine:
             for hd, g in zip(self.heads, graws):
                 x = hd["x"]
                 T.head_grad_pack(g, hd["dy"], self.partial)
-                T.colreduce(self.partial, hd["nblk"], 256, hd["db"], accumulate=True)
+                T.colreduce(self.partial, hd["nblk"], hd["pw"], hd["db"], accumulate=True)
                 T.conv_wgrad(hd["dy"], x, hd["dw"], 1, layout=_lib.DW_OHWI, accumulate=True, deterministic=det_flag)
                 self._contribute_conv(hd["dy"], hd["wd"], hd["c1"], 1, x)
         for b in seg:

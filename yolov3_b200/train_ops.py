@@ -90,12 +90,18 @@ def pack_dgrad_batched(items_dev: torch.Tensor, n_items: int, wbf: torch.Tensor,
 
 
 def head_grad_pack(g: torch.Tensor, dy: PaddedNHWC, partial: torch.Tensor):
-    """dL/draw fp32 [n,na,ny,nx,no] -> dy (bf16 padded NHWC, channel a*no+o) + first-stage column sums partial[blocks][256]."""
+    """dL/draw fp32 [n,na,ny,nx,no] -> dy (bf16 padded NHWC, channel a*no+o) + first-stage column sums
+    partial[blocks][head_grad_width(dy)]."""
     assert g.dtype == torch.float32 and g.is_contiguous() and g.dim() == 5
     n, na, ny, nx, no = g.shape
-    assert (dy.n, dy.h, dy.w) == (n, ny, nx) and partial.numel() >= partial_blocks(n, ny) * 256
+    assert (dy.n, dy.h, dy.w) == (n, ny, nx) and partial.numel() >= partial_blocks(n, ny) * head_grad_width(dy)
     _lib.check(_lib.lib().y3_head_grad_pack(g.data_ptr(), n, na, ny, nx, no, dy.ptr, dy.ld, dy.coff, partial.data_ptr(), _stream()),
                "y3_head_grad_pack")
+
+
+def head_grad_width(dy: PaddedNHWC) -> int:
+    """Row width of ``head_grad_pack``'s partial sums: the dy slice's channel count rounded up to 256 (256 up to 80 classes)."""
+    return (dy.ld - dy.coff + 255) // 256 * 256
 
 
 def pack_weights(w: torch.Tensor, fwd: torch.Tensor | None, dgrad: torch.Tensor | None):
