@@ -86,7 +86,7 @@ typedef struct y3_conv_desc {
 int y3_conv_bn_act_fwd(const y3_conv_desc* d, y3_stream_t stream);
 /* Input gradient of a STRIDE-2 3x3 conv (training; autograd of Conv.forward, models/common.py:71-75) as four parity-class
  * convolutions of the un-stuffed output gradient: `in` = dy, padded NHWC [n, h+2, w+2, in_ld] on the conv's OUTPUT grid (h, w =
- * output size), `weight` = the dgrad pack [c_in_pad rows = dx channels, 9 * c_dy] (taps flipped, y3_pack_weights), `out` = dx, padded
+ * output size), `weight` = the dgrad pack [c_in_pad rows = dx channels, 9 * c_dy] (taps flipped, y3_pack_dgrad_batched), `out` = dx, padded
  * [n, 2h+2, 2w+2, out_ld]; `res` (optional, dx geometry) is added — pass `out` itself to accumulate.  ksize = 3, stride = 1 and
  * act = Y3_ACT_NONE in the descriptor (it describes the transposed conv on dy's grid). */
 int y3_conv_dgrad_s2(const y3_conv_desc* d, y3_stream_t stream);
@@ -300,10 +300,7 @@ typedef struct y3_bn_bwd_desc {
   float count;     /* pixels behind the sums used by the apply phase (all ranks); 0 = this rank's n*h*w */
 } y3_bn_bwd_desc;
 int y3_bn_act_bwd(const y3_bn_bwd_desc* d, y3_stream_t stream);
-/* fp32 master weights [co, ci, k, k] -> bf16 forward pack [co_pad, k*k*ci] and/or dgrad pack [ci_pad, k*k*co] (taps
- * flipped, channels swapped); pad rows must already be zero */
-int y3_pack_weights(const float* w, int32_t co, int32_t ci, int32_t k, void* fwd, void* dgrad, y3_stream_t stream);
-/* Batched form used by the training engine: the fp32 masters live in ONE flat buffer with every conv weight stored
+/* Weight packs of the training engine: the fp32 masters live in ONE flat buffer with every conv weight stored
  * [co][kh][kw][ci] (channels_last strides of the [co,ci,k,k] parameter == the forward pack's order), so
  *   y3_f32_to_bf16        converts the whole buffer once per step (forward packs are views of the copy), and
  *   y3_pack_dgrad_batched transposes every layer of a device-resident table into its dgrad pack in one launch. */
@@ -325,35 +322,21 @@ int y3_pack_dgrad_batched(const y3_pack_item* items_dev, int32_t n_items, const 
  * (256 for every head of at most 80 classes and 3 anchors). */
 int y3_head_grad_pack(const float* g, int32_t n, int32_t na, int32_t ny, int32_t nx, int32_t no, void* dy, int32_t dy_ld,
                       int32_t dy_coff, float* partial, y3_stream_t stream);
-/* dy of a stride-2 conv scattered onto the even positions of a zeroed [n, 2ho+2, 2wo+2, dst_ld] buffer */
-int y3_zero_stuff(const void* src, int32_t src_ld, int32_t src_coff, void* dst, int32_t dst_ld, int32_t dst_coff, int32_t n,
-                  int32_t ho, int32_t wo, int32_t c, y3_stream_t stream);
-/* dW[co, ci, kh, kw] += sum_p dy[p, co] * x[p + shift(kh,kw), ci] on the stride-1 padded grid [n, h+2, w+2]; dw is fp32,
- * zeroed by the caller; co, ci multiples of 8.  dw_layout Y3_DW_OIHW: PyTorch's [co, ci, k, k].  Y3_DW_TAP_MAJOR:
- * [k*k, co, ci] — every (tap, co) row is contiguous in ci, so the tensor-core kernel accumulates with 16-byte vector
- * reductions instead of one 4-byte atomic per element (the scattered atomics, ~45 G/s, were all of its time); the caller
- * permutes once when it hands the gradient to the optimizer.  Needs c_in % 32 == 0 (y3_conv_wgrad_tap_major tells). */
-#define Y3_DW_OIHW 0
-#define Y3_DW_TAP_MAJOR 1
-#define Y3_DW_OHWI 2       /* [co, k*k, ci] == the channels_last strides of a [co, ci, k, k] tensor: the training engine's
-                              flat gradient buffer (the gradient IS the parameter's .grad view, no permute) */
+/* dW[co, kh*k+kw, ci] += sum_p dy[p, co] * x[p + shift(kh,kw), ci] on the stride-1 padded grid [n, h+2, w+2], with the
+ * wgmma kernel.  dw is fp32 [co, k*k, ci]: the channels_last strides of a [co, ci, k, k] tensor, i.e. the training engine's
+ * flat gradient buffer (the gradient IS the parameter's .grad view, no permute); each (co, tap) row is contiguous in ci,
+ * so the kernel adds with 8-byte vector reductions.  co, ci multiples of 8; dy and x 16-byte aligned, dw 8-byte aligned. */
 typedef struct y3_wgrad_desc {
   const void* dy; int32_t dy_ld, dy_coff;
   const void* x;  int32_t x_ld, x_coff;
   float* dw;
   int32_t co, ci, ksize, n, h, w;
-  int32_t dw_layout;
   int32_t accumulate;     /* 1: dw holds earlier contributions that must be kept (always reduce, never plain-store) */
   int32_t deterministic;  /* 1: no split over pixels — one CTA per dW tile, bit-reproducible, slower on the early layers */
-  int32_t stride;         /* 0/1: dy on x's grid (a stride-2 conv passes the zero-stuffed dy).  2: DIRECT stride-2 — dy is the
-                             conv's own [n, h/2+2, w/2+2, dy_ld] output-grid gradient, x is read through its row/column parity view;
-                             3x3 only, needs y3_conv_wgrad_s2_supported(h, w) and c_in % 32 == 0 */
+  int32_t stride;         /* 0/1: dy on x's grid.  2: a stride-2 conv — dy is the conv's own [n, h/2+2, w/2+2, dy_ld]
+                             output-grid gradient, x is read through its row/column parity view; 3x3 and even h, w only */
 } y3_wgrad_desc;
 int y3_conv_wgrad(const y3_wgrad_desc* d, y3_stream_t stream);
-/* 1 if the direct stride-2 form (stride = 2) can tile an input of h x w (an 80-pixel tw x th patch must divide the output) */
-int y3_conv_wgrad_s2_supported(int32_t h, int32_t w);
-/* 1 if y3_conv_wgrad accepts Y3_DW_TAP_MAJOR for this c_in (the wgmma kernel is in use), else 0 */
-int y3_conv_wgrad_tap_major(int32_t c_in);
 /* dst (+)= src over the interior pixels of two padded NHWC bf16 slices of equal [n,h,w,c] (gradient fan-in) */
 int y3_add_nhwc(const void* src, int32_t src_ld, int32_t src_coff, void* dst, int32_t dst_ld, int32_t dst_coff, int32_t n,
                 int32_t h, int32_t w, int32_t c, int32_t accumulate, y3_stream_t stream);
@@ -361,8 +344,6 @@ int y3_add_nhwc(const void* src, int32_t src_ld, int32_t src_coff, void* dst, in
  * NHWC buffer, column (c*3+kh)*3+kw; lets training run layer 0 as a 1x1 conv with the generic kernels */
 int y3_im2col_first(const void* in, int32_t in_dtype, float in_div, int32_t n, int32_t h, int32_t w, void* out,
                     int32_t out_ld, int32_t out_coff, y3_stream_t stream);
-/* out[c] += sum over rows of g[row, c] (fp32 pixel-major; Detect-head bias gradients), any c (256 columns per block) */
-int y3_colsum_f32(const float* g, int32_t ld, int32_t c, int64_t rows, float* out, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Image pre-processing on the device (SURVEY §8(f) row f1): letterbox (utils/augmentations.py:104-134: cv2.resize

@@ -219,7 +219,7 @@ def test_loss_vs_oracle(nc):
 
 
 # ------------------------------------------------------------------------------------------------ head gradient
-@pytest.mark.parametrize("no", [6, 85, 370, 1029])
+@pytest.mark.parametrize("no", [6, 85, 370, 1029, 25, 86, 170, 600])  # 86, 170: na*no just past / below a 256-column block
 def test_head_grad_pack_and_colreduce(no):
     from yolov3_b200 import ops
     from yolov3_b200 import train_ops as T
@@ -247,10 +247,8 @@ def test_head_grad_pack_and_colreduce(no):
     assert partial[nblk * w256:].isnan().all() and not partial[: nblk * w256].isnan().any()
     assert torch.allclose(db[:co] - 1, g.sum(dim=(0, 2, 3)).reshape(co), rtol=1e-5, atol=1e-4)
     assert torch.equal(db[co:], torch.ones(w256 - co, device="cuda"))
-    # the same bias gradient straight from the fp32 rows (y3_colsum_f32, any column count)
-    out = torch.zeros(co, device="cuda")
-    T.colsum_f32(ref.reshape(-1, co).contiguous(), co, out)
-    assert torch.allclose(out, g.sum(dim=(0, 2, 3)).reshape(co), rtol=1e-4, atol=1e-3)
+    # the same bias gradient against a float64 sum of the fp32 rows
+    assert torch.allclose((db[:co] - 1).double(), ref.double().reshape(-1, co).sum(0), rtol=1e-4, atol=1e-3)
 
 
 # ------------------------------------------------------------------------------------------------ training
@@ -311,17 +309,11 @@ def test_train_heads_vs_autograd_and_bit_reproducible(name, nc):
             if not e <= 2e-2:
                 bad.append((hd["wname"], tag, e))
     assert not bad, bad
-    # deterministic mode: every gradient bit for bit, except the weight gradients of convs with c_in % 32 != 0 (yolov3-tiny's
-    # 16-channel inputs), whose warp-level wgrad kernel adds its pixel chunks with atomics whatever the class count
+    # deterministic mode: every gradient bit for bit (yolov3-tiny's 16-channel convs included)
     st = m.store()
-    keep = torch.ones(st.n_train, dtype=torch.bool, device=st.G.device)
-    for s in st.slots.values():
-        if s.rows and s.ci % 32:
-            keep[s.offset:s.offset + s.numel] = False
     G1, P1 = st.G.clone(), st.P.clone()
     m2, _, loss2, _ = _step(name, nc, 128, 4)
-    assert loss == loss2 and torch.equal(G1[keep], m2.store().G[keep]) and torch.equal(P1, m2.store().P)
-    assert keep.all() or name == "yolov3-tiny"
+    assert loss == loss2 and torch.equal(G1, m2.store().G) and torch.equal(P1, m2.store().P)
 
 
 # ------------------------------------------------------------------------------------------------ AutoAnchor seam

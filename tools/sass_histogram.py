@@ -5,7 +5,7 @@
 Runs `cuobjdump -sass` on yolov3_b200/libyolov3_b200.so (no GPU needed) and counts, for every kernel, the instructions that
 prove which hardware path it takes: HGMMA (wgmma), WARPGROUP (wgmma fences / waits), UTMALDG / UTMASTG (TMA load / store),
 SYNCS (mbarrier), ACQBULK / PREEXIT (griddepcontrol.wait / launch_dependents: programmatic
-dependent launch), HMMA / IMMA (legacy mma.sync: only the 3-channel stem conv and the fallback wgrad), MUFU, REDUX, ATOM/ATOMS/RED,
+dependent launch), HMMA / IMMA (legacy mma.sync: only the 3-channel stem conv), MUFU, REDUX, ATOM/ATOMS/RED,
 LDGSTS (cp.async: the shared-memory ring of the BatchNorm backward passes).
 """
 import collections

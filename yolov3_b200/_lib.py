@@ -153,10 +153,7 @@ class WgradDesc(C.Structure):
                 ("x", C.c_void_p), ("x_ld", C.c_int32), ("x_coff", C.c_int32),
                 ("dw", C.c_void_p),
                 ("co", C.c_int32), ("ci", C.c_int32), ("ksize", C.c_int32), ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32),
-                ("dw_layout", C.c_int32), ("accumulate", C.c_int32), ("deterministic", C.c_int32), ("stride", C.c_int32)]
-
-
-DW_OIHW, DW_TAP_MAJOR, DW_OHWI = 0, 1, 2
+                ("accumulate", C.c_int32), ("deterministic", C.c_int32), ("stride", C.c_int32)]
 
 
 class LetterboxDesc(C.Structure):
@@ -209,15 +206,10 @@ def _declare(lib):
         "y3_sgd_step": ([vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp], C.c_int),
         "y3_bn_act_fwd": ([C.POINTER(BnActDesc), vp], C.c_int),
         "y3_bn_act_bwd": ([C.POINTER(BnBwdDesc), vp], C.c_int),
-        "y3_pack_weights": ([vp, i32, i32, i32, vp, vp, vp], C.c_int),
-        "y3_zero_stuff": ([vp, i32, i32, vp, i32, i32, i32, i32, i32, i32, vp], C.c_int),
         "y3_scale_boxes": ([vp, C.c_int64, i32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, vp], C.c_int),
         "y3_conv_wgrad": ([C.POINTER(WgradDesc), vp], C.c_int),
-        "y3_conv_wgrad_tap_major": ([i32], C.c_int),
-        "y3_conv_wgrad_s2_supported": ([i32, i32], C.c_int),
         "y3_add_nhwc": ([vp, i32, i32, vp, i32, i32, i32, i32, i32, i32, i32, vp], C.c_int),
         "y3_im2col_first": ([vp, i32, C.c_float, i32, i32, i32, vp, i32, i32, vp], C.c_int),
-        "y3_colsum_f32": ([vp, i32, i32, C.c_int64, vp, vp], C.c_int),
         "y3_box_iou": ([vp, i32, vp, i32, C.c_float, vp, vp], C.c_int),
         "y3_loss_workspace_bytes": ([C.POINTER(LossDesc)], C.c_int64),
         "y3_loss_fwd_bwd": ([C.POINTER(LossDesc), vp, C.c_int64, vp, vp], C.c_int),

@@ -100,7 +100,6 @@ int conv_tc_launch(const ConvTcPlan& plan, cudaStream_t stream);
 int pool_launch(const y3_pool_desc& d, cudaStream_t stream);
 int amax_launch(const y3_amax_desc& d, cudaStream_t stream);
 int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream);
-int wgrad_tc_s2_supported(int h, int w);
 int pool_train_fwd(const y3_pool_desc& d, uint8_t* idx, cudaStream_t stream);
 int pool_bwd(const y3_pool_desc& d, const uint8_t* idx, int accumulate, cudaStream_t stream);
 

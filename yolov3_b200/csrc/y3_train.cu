@@ -9,12 +9,6 @@
 //                   apply pass:  dy = scale * (dz - mean(dz) - yhat * mean(dz*yhat))               (input of dgrad / wgrad)
 //                   through a per-thread cp.async shared-memory ring; the 2x-upsample layers sum four da replicas per
 //                   item in registers instead
-//   pack_weights    fp32 master weights [co,ci,k,k] -> bf16 forward pack [co_pad, tap*ci+c] and dgrad pack
-//                   [ci_pad, tap'*co+o] (taps flipped), every optimizer step
-//   zero_stuff      dy of a stride-2 conv scattered onto the even positions of a zero 2x grid (its dgrad is then a
-//                   stride-1 conv with flipped weights)
-//   wgrad           dW[co, tap, ci] = sum_p dy[p, co] * x[p + shift(tap), ci]  (warp-level bf16 MMA, split over pixels)
-//   bias_grad       Detect heads: db[co] = sum_p dy[p, co]
 #include "y3_common.cuh"
 #include "y3_internal.h"
 
@@ -504,187 +498,6 @@ __global__ void __launch_bounds__(256, 3) bn_act_bwd_async_kernel(const BnBwdArg
   }
 }
 
-// ---------------------------------------------------------------------------------------------- pack_weights
-// w: fp32 [co, ci, k, k] (PyTorch layout).  fwd: bf16 [co_pad, (kh*k+kw)*ci + c];  dgrad: bf16 [ci_pad, (kh'*k+kw')*co + o]
-// with (kh', kw') = (k-1-kh, k-1-kw).  Rows beyond co / ci stay zero (buffers are zero-initialised once).
-__global__ void __launch_bounds__(256) pack_weights_kernel(const float* __restrict__ w, int co, int ci, int k,
-                                                           __nv_bfloat16* __restrict__ fwd, __nv_bfloat16* __restrict__ dgr) {
-  pdl_entry();
-  const long long total = static_cast<long long>(co) * ci * k * k;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int kw = static_cast<int>(i % k);
-    long long t = i / k;
-    const int kh = static_cast<int>(t % k);
-    t /= k;
-    const int c = static_cast<int>(t % ci);
-    const int o = static_cast<int>(t / ci);
-    const __nv_bfloat16 v = __float2bfloat16(w[i]);
-    if (fwd) fwd[static_cast<long long>(o) * k * k * ci + (kh * k + kw) * ci + c] = v;
-    if (dgr) dgr[static_cast<long long>(c) * k * k * co + ((k - 1 - kh) * k + (k - 1 - kw)) * co + o] = v;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------- zero_stuff
-// src: dy of a stride-2 conv, padded NHWC [n, ho+2, wo+2, ld]; dst: zero-initialised padded [n, 2ho+2, 2wo+2, c]:
-// dst(2*oy, 2*ox) = src(oy, ox)  (unpadded coordinates).  Only the even positions are ever written.
-__global__ void __launch_bounds__(256) zero_stuff_kernel(Slice src, SliceW dst, int n, int ho, int wo, int c8) {
-  pdl_entry();
-  const long long total = static_cast<long long>(n) * ho * wo * c8;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const int cg = static_cast<int>(i % c8);
-    long long t = i / c8;
-    const int x = static_cast<int>(t % wo);
-    t /= wo;
-    const int y = static_cast<int>(t % ho);
-    const int b = static_cast<int>(t / ho);
-    const long long rs = (static_cast<long long>(b) * (ho + 2) + y + 1) * (wo + 2) + x + 1;
-    const long long rd = (static_cast<long long>(b) * (2 * ho + 2) + 2 * y + 1) * (2 * wo + 2) + 2 * x + 1;
-    *reinterpret_cast<uint4*>(dst.p + rd * dst.ld + dst.coff + cg * 8) =
-        __ldg(reinterpret_cast<const uint4*>(src.p + rs * src.ld + src.coff + cg * 8));
-  }
-}
-
-// ---------------------------------------------------------------------------------------------- wgrad
-// dW[co, tap, ci] += sum over a chunk of padded pixels p of dy[p, co] * x[p + shift(tap), ci]   (stride-1 geometry;
-// for a stride-2 conv the caller passes the zero-stuffed dy so that the same relation holds on the input grid).
-// CTA tile: 64 (co) x 64 (ci) for one tap; K = pixels, consumed 32 at a time.  Both operands are "K-rows" in memory
-// (pixel-major, channels contiguous), i.e. exactly the col-major A / row... fragments of mma.m16n8k16 after a transposed
-// shared-memory read (ldmatrix.trans).  fp32 partial sums are reduced with atomics into the fp32 gradient.
-constexpr int kWgPix = 32;    // pixels per smem stage
-constexpr int kWgTile = 64;   // channels per tile side
-
-__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t (&r)[4], uint32_t saddr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(saddr));
-}
-__device__ __forceinline__ void mma16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
-struct WgradArgs {
-  Slice dy;   // [rows, ld] padded pixel list, channels [coff, coff+co)
-  Slice x;    // input activation, same padded geometry
-  float* dw;  // fp32 [co, ci, taps] == PyTorch's [co, ci, k, k], or (ohwi) [co, taps, ci]
-  int ohwi;
-  int co, ci, taps, wp;
-  long long rows;
-  int rows_per_cta;
-};
-
-// grid: (pixel chunks, co/64 * ci/64, taps); block 128 threads (4 warps: 2x2 over the 64x64 tile, 32x32 each)
-__global__ void __launch_bounds__(128) wgrad_kernel(const WgradArgs p) {
-  pdl_entry();
-  __shared__ __align__(16) __nv_bfloat16 s_a[kWgPix][kWgTile + 8];  // dy chunk  [pixel][co]   (+8: conflict-free ldmatrix)
-  __shared__ __align__(16) __nv_bfloat16 s_b[kWgPix][kWgTile + 8];  // x chunk   [pixel][ci]
-  const int tiles_ci = (p.ci + kWgTile - 1) / kWgTile;
-  const int co0 = (blockIdx.y / tiles_ci) * kWgTile, ci0 = (blockIdx.y % tiles_ci) * kWgTile;
-  const int tap = blockIdx.z;
-  const int shift = p.taps == 9 ? (tap / 3 - 1) * p.wp + (tap % 3 - 1) : 0;
-  const long long r0 = static_cast<long long>(blockIdx.x) * p.rows_per_cta;
-  const long long r1 = r0 + p.rows_per_cta < p.rows ? r0 + p.rows_per_cta : p.rows;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int wm = (warp >> 1) * 32, wn = (warp & 1) * 32;  // warp's 32x32 sub-tile (co, ci)
-  float acc[2][4][4];
-#pragma unroll
-  for (int i = 0; i < 2; ++i)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[i][j][0] = acc[i][j][1] = acc[i][j][2] = acc[i][j][3] = 0.f;
-
-  for (long long r = r0; r < r1; r += kWgPix) {
-    // stage 32 pixels x 64 channels of dy and of (shifted) x: 128 threads x 2 x 16 B each
-#pragma unroll
-    for (int it = 0; it < 2; ++it) {
-      const int idx = threadIdx.x + it * 128;  // 0..255 = 32 pixels x 8 chunks
-      const int px = idx >> 3, ch = (idx & 7) * 8;
-      const long long ra = r + px, rb = r + px + shift;
-      uint4 va = make_uint4(0, 0, 0, 0), vb = make_uint4(0, 0, 0, 0);
-      if (ra < r1 && co0 + ch < p.co) va = __ldg(reinterpret_cast<const uint4*>(p.dy.p + ra * p.dy.ld + p.dy.coff + co0 + ch));
-      if (ra < r1 && rb >= 0 && rb < p.rows && ci0 + ch < p.ci)
-        vb = __ldg(reinterpret_cast<const uint4*>(p.x.p + rb * p.x.ld + p.x.coff + ci0 + ch));
-      *reinterpret_cast<uint4*>(&s_a[px][ch]) = va;
-      *reinterpret_cast<uint4*>(&s_b[px][ch]) = vb;
-    }
-    __syncthreads();
-#pragma unroll
-    for (int ks = 0; ks < kWgPix / 16; ++ks) {
-      // A fragments (16 co x 16 pixels, row-major A[m][k] = dy[pixel k][co m]): transposed 8x8 loads from [pixel][co]
-      uint32_t af[2][4];
-#pragma unroll
-      for (int mi = 0; mi < 2; ++mi) {
-        // matrices: (m0-7,k0-7) (m8-15,k0-7) (m0-7,k8-15) (m8-15,k8-15); smem rows are pixels (k), 8 consecutive co per row
-        const int mat = lane >> 3, rr = lane & 7;
-        const int kk = ks * 16 + (mat >> 1) * 8 + rr;
-        const int mm = wm + mi * 16 + (mat & 1) * 8;
-        ldmatrix_x4_trans(af[mi], smem_u32(&s_a[kk][mm]));
-      }
-      // B fragments (16 pixels x 8 ci, "col" operand B[k][n] = x[pixel k][ci n]): b0 = (k 2t..2t+1, n g), b1 = k+8
-      uint32_t bf[4][2];
-#pragma unroll
-      for (int nj = 0; nj < 2; ++nj) {
-        // one x4.trans covers two n8 tiles: matrices (k0-7,n0-7) (k8-15,n0-7) (k0-7,n8-15) (k8-15,n8-15)
-        uint32_t t4[4];
-        const int mat = lane >> 3, rr = lane & 7;
-        const int kk = ks * 16 + (mat & 1) * 8 + rr;
-        const int nn = wn + nj * 16 + (mat >> 1) * 8;
-        ldmatrix_x4_trans(t4, smem_u32(&s_b[kk][nn]));
-        bf[nj * 2 + 0][0] = t4[0];
-        bf[nj * 2 + 0][1] = t4[1];
-        bf[nj * 2 + 1][0] = t4[2];
-        bf[nj * 2 + 1][1] = t4[3];
-      }
-#pragma unroll
-      for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-        for (int nj = 0; nj < 4; ++nj) mma16816(acc[mi][nj], af[mi], bf[nj][0], bf[nj][1]);
-    }
-    __syncthreads();
-  }
-  // C fragment: c0,c1 = (row g, cols 2t,2t+1), c2,c3 = (row g+8, same cols)
-  const int g = lane >> 2, t = lane & 3;
-#pragma unroll
-  for (int mi = 0; mi < 2; ++mi)
-#pragma unroll
-    for (int nj = 0; nj < 4; ++nj) {
-      const int co = co0 + wm + mi * 16 + g, ci = ci0 + wn + nj * 8 + t * 2;
-      if (ci >= p.ci) continue;  // ci is a multiple of 8, so ci+1 is in range with ci
-      const long long step = p.ohwi ? 1 : p.taps;  // distance between ci and ci + 1
-      if (co < p.co) {
-        float* d0 = p.ohwi ? p.dw + (static_cast<long long>(co) * p.taps + tap) * p.ci + ci
-                           : p.dw + (static_cast<long long>(co) * p.ci + ci) * p.taps + tap;
-        atomicAdd(d0, acc[mi][nj][0]);
-        atomicAdd(d0 + step, acc[mi][nj][1]);
-      }
-      if (co + 8 < p.co) {
-        float* d1 = p.ohwi ? p.dw + (static_cast<long long>(co + 8) * p.taps + tap) * p.ci + ci
-                           : p.dw + (static_cast<long long>(co + 8) * p.ci + ci) * p.taps + tap;
-        atomicAdd(d1, acc[mi][nj][2]);
-        atomicAdd(d1 + step, acc[mi][nj][3]);
-      }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------- bias_grad (fp32 head grads)
-// g: fp32 pixel-major [rows, ld]; db[c] += sum_rows g[row, c].  Column block blockIdx.y covers columns
-// [256*blockIdx.y, 256*blockIdx.y + cb), cb = min(256, c - 256*blockIdx.y); its threads split into 256/cb row lanes.
-__global__ void __launch_bounds__(256) colsum_f32_kernel(const float* __restrict__ g, int ld, int c, long long rows,
-                                                         int rows_per_block, float* __restrict__ db) {
-  pdl_entry();
-  const int c0 = blockIdx.y * 256, cb = min(256, c - c0);
-  const int col = c0 + threadIdx.x % cb, rl = threadIdx.x / cb, nrl = blockDim.x / cb;
-  const long long r0 = static_cast<long long>(blockIdx.x) * rows_per_block;
-  const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
-  float s = 0.f;
-  if (rl < nrl)
-    for (long long r = r0 + rl; r < r1; r += nrl) s += g[r * ld + col];
-  if (rl < nrl) atomicAdd(db + col, s);
-}
-
 // ---------------------------------------------------------------------------------------------- add / copy
 // dst (+)= src over the interior pixels of two padded NHWC slices with the same [n,h,w,c] (gradient fan-in:
 // Bottleneck shortcut, tensors with several consumers)
@@ -1027,78 +840,16 @@ extern "C" int y3_head_grad_pack(const float* g, int32_t n, int32_t na, int32_t 
   return Y3_OK;
 }
 
-extern "C" int y3_pack_weights(const float* w, int32_t co, int32_t ci, int32_t k, void* fwd, void* dgrad,
-                               y3_stream_t stream) {
-  Y3_REQUIRE(w && (fwd || dgrad) && co > 0 && ci > 0 && (k == 1 || k == 3), "pack_weights: bad arguments");
-  const long long total = static_cast<long long>(co) * ci * k * k;
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::pack_weights_kernel, dim3(y3::grid_for(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), w, co, ci, k, static_cast<__nv_bfloat16*>(fwd), static_cast<__nv_bfloat16*>(dgrad)));
-  Y3_CHECK_CUDA(cudaGetLastError());
-  return Y3_OK;
-}
-
-extern "C" int y3_zero_stuff(const void* src, int32_t src_ld, int32_t src_coff, void* dst, int32_t dst_ld, int32_t dst_coff,
-                             int32_t n, int32_t ho, int32_t wo, int32_t c, y3_stream_t stream) {
-  Y3_REQUIRE(src && dst && c % 8 == 0 && n > 0 && ho > 0 && wo > 0, "zero_stuff: bad arguments");
-  const long long total = static_cast<long long>(n) * ho * wo * (c / 8);
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::zero_stuff_kernel, dim3(y3::grid_for(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), Slice{static_cast<const __nv_bfloat16*>(src), src_ld, src_coff}, SliceW{static_cast<__nv_bfloat16*>(dst), dst_ld, dst_coff}, n,
-      ho, wo, c / 8));
-  Y3_CHECK_CUDA(cudaGetLastError());
-  return Y3_OK;
-}
-
 extern "C" int y3_conv_wgrad(const y3_wgrad_desc* d, y3_stream_t stream) {
   Y3_REQUIRE(d && d->dy && d->x && d->dw, "wgrad: null pointer");
   Y3_REQUIRE(d->co % 8 == 0 && d->ci % 8 == 0 && (d->ksize == 1 || d->ksize == 3) && d->n > 0 && d->h > 0 && d->w > 0,
              "wgrad: c_out/c_in must be multiples of 8 (got %d/%d), ksize 1|3", d->co, d->ci);
   Y3_REQUIRE(d->dy_ld % 8 == 0 && d->dy_coff % 8 == 0 && d->x_ld % 8 == 0 && d->x_coff % 8 == 0, "wgrad: bad slices");
-  Y3_REQUIRE(d->stride == 0 || d->stride == 1 || (d->stride == 2 && d->ci % 32 == 0),
-             "wgrad: stride must be 1, or 2 with the tensor-core kernel (c_in % 32 == 0)");
-  // wgmma kernel (csrc/y3_wgrad_tc.cu) whenever its tiling fits; the warp-level MMA kernel below otherwise
-  if (d->ci % 32 == 0 && (reinterpret_cast<uintptr_t>(d->dy) & 15) == 0 &&
-      (reinterpret_cast<uintptr_t>(d->x) & 15) == 0)
-    return y3::wgrad_tc(*d, static_cast<cudaStream_t>(stream));
-  Y3_REQUIRE(d->dw_layout == Y3_DW_OIHW || d->dw_layout == Y3_DW_OHWI,
-             "wgrad: the tap-major accumulation layout needs the tensor-core kernel (c_in % 32 == 0)");
-  Y3_REQUIRE(d->stride != 2, "wgrad: the direct stride-2 form needs the tensor-core kernel (c_in % 32 == 0)");
-  y3::WgradArgs a;
-  a.ohwi = d->dw_layout == Y3_DW_OHWI ? 1 : 0;
-  a.dy = Slice{static_cast<const __nv_bfloat16*>(d->dy), d->dy_ld, d->dy_coff};
-  a.x = Slice{static_cast<const __nv_bfloat16*>(d->x), d->x_ld, d->x_coff};
-  a.dw = d->dw;
-  a.co = d->co;
-  a.ci = d->ci;
-  a.taps = d->ksize * d->ksize;
-  a.wp = d->w + 2;
-  a.rows = static_cast<long long>(d->n) * (d->h + 2) * (d->w + 2);
-  // split the pixel dimension so that the grid fills the machine ~4x
-  const int t_co = (d->co + 63) / 64, t_ci = (d->ci + 63) / 64;
-  const long long tiles = static_cast<long long>(t_co) * t_ci * a.taps;
-  long long chunks = (4ll * y3::num_sms() + tiles - 1) / tiles;
-  const long long max_chunks = (a.rows + 1023) / 1024;
-  if (chunks > max_chunks) chunks = max_chunks;
-  if (chunks < 1) chunks = 1;
-  long long rpc = (a.rows + chunks - 1) / chunks;
-  rpc = (rpc + y3::kWgPix - 1) / y3::kWgPix * y3::kWgPix;
-  chunks = (a.rows + rpc - 1) / rpc;
-  a.rows_per_cta = static_cast<int>(rpc);
-  const dim3 grid(static_cast<unsigned>(chunks), static_cast<unsigned>(t_co * t_ci), a.taps);
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::wgrad_kernel, dim3(grid), dim3(128), 0, static_cast<cudaStream_t>(stream), a));
-  Y3_CHECK_CUDA(cudaGetLastError());
-  return Y3_OK;
-}
-
-extern "C" int y3_conv_wgrad_s2_supported(int32_t h, int32_t w) { return y3::wgrad_tc_s2_supported(h, w); }
-
-extern "C" int y3_conv_wgrad_tap_major(int32_t c_in) { return c_in % 32 == 0 ? 1 : 0; }
-
-extern "C" int y3_colsum_f32(const float* g, int32_t ld, int32_t c, int64_t rows, float* out, y3_stream_t stream) {
-  Y3_REQUIRE(g && out && c > 0 && rows > 0, "colsum: bad arguments");
-  const int rows_per_block = 1024;
-  const long long blocks = (rows + rows_per_block - 1) / rows_per_block;
-  const dim3 grid(static_cast<unsigned>(blocks), static_cast<unsigned>((c + 255) / 256));
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::colsum_f32_kernel, grid, dim3(256), 0, static_cast<cudaStream_t>(stream), g, ld, c, rows, rows_per_block, out));
-  Y3_CHECK_CUDA(cudaGetLastError());
-  return Y3_OK;
+  Y3_REQUIRE(d->stride == 0 || d->stride == 1 || d->stride == 2, "wgrad: stride must be 1 or 2");
+  Y3_REQUIRE((reinterpret_cast<uintptr_t>(d->dy) & 15) == 0 && (reinterpret_cast<uintptr_t>(d->x) & 15) == 0 &&
+                 (reinterpret_cast<uintptr_t>(d->dw) & 7) == 0,
+             "wgrad: dy and x must be 16-byte aligned (TMA), dw 8-byte aligned");
+  return y3::wgrad_tc(*d, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int y3_add_nhwc(const void* src, int32_t src_ld, int32_t src_coff, void* dst, int32_t dst_ld, int32_t dst_coff,

@@ -1,13 +1,13 @@
-// yolov3_b200 — weight gradient of a conv on the Hopper tensor cores (wgmma).
-//   dW[co, ci, tap] += sum over padded pixels p of dy[p, co] * x[p + shift(tap), ci]
+// yolov3_b200 — weight gradient of a conv on the Hopper tensor cores (wgmma); every training conv runs it.
+//   dW[co, tap, ci] += sum over padded pixels p of dy[p, co] * x[p + shift(tap), ci]
 // is a GEMM whose K dimension is the PIXEL index: both operands sit in memory pixel-major with channels contiguous, i.e.
 // "MN-major" (transposed) wgmma operands: shared-memory descriptors of the canonical MN-major swizzled layout — 64
 // channels (128 B) contiguous, 8 pixel rows per swizzle atom, SBO = bytes between 8-row groups, LBO = bytes between
 // 64-channel blocks.  The same TMA boxes as the forward conv ([64 pixels x 64 channels], the x box shifted by the tap)
 // land in exactly that layout — no transposition anywhere.
 // One CTA = one (128-co block, N-ci block, tap) output tile over a range of pixels (split-K): warp 8 streams the boxes,
-// warpgroups 0 and 1 accumulate co rows [0, 64) and [64, 128) in registers and finish with fp32 atomics into
-// PyTorch-layout dW.  Replaces the mma.sync kernel of y3_train.cu behind the same y3_conv_wgrad entry point
+// warpgroups 0 and 1 accumulate co rows [0, 64) and [64, 128) in registers and finish with 8-byte fp32 vector reductions
+// (or plain stores) into dW laid out [co][taps][ci], the flat gradient buffer's order
 // (reference: autograd of Conv.forward, models/common.py:71-75).
 #include <cuda_bf16.h>
 
@@ -28,8 +28,7 @@ struct WgTcArgs {
   int kblocks_total;    // ceil(rows / 64)
   int kblocks_per_cta;  // pixel blocks one CTA accumulates (split-K)
   int dy_coff, x_coff;
-  float* dw;
-  int layout;           // Y3_DW_OIHW [co][ci][taps] | Y3_DW_TAP_MAJOR [taps][co][ci] | Y3_DW_OHWI [co][taps][ci] (vector reductions)
+  float* dw;            // [co][taps][ci]
   int single;           // 1: this CTA is the only contributor to its dW tile AND dw need not be accumulated into (plain stores)
   int* err;
   uint32_t lbo_a, lbo_b, sbo_a, sbo_b;  // descriptor strides in bytes
@@ -151,31 +150,24 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap map_dy, const __grid_constan
     wgmma_wait<0>();
     wgmma_fence_regs(acc);
 
-    // epilogue: accumulator row = co, column = ci; fp32 atomics (or plain stores) into dW
-    const bool rows_contig = p.layout != Y3_DW_OIHW || p.taps == 1;  // this thread's ci run is contiguous in memory
+    // epilogue: accumulator row = co, column = ci; fp32 vector reductions (or plain stores) into dW.  ci and this thread's
+    // column c are even, so ci0 + c < ci puts both columns of the pair inside the row; columns past ci are discarded.
     const int cq = 2 * (lane & 3);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int co = co0 + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
       if (co >= p.co) continue;
-      float* dst = p.layout == Y3_DW_OHWI ? p.dw + (static_cast<long long>(co) * p.taps + tap) * p.ci + ci0
-                   : rows_contig          ? p.dw + (static_cast<long long>(tap) * p.co + co) * p.ci + ci0
-                                          : p.dw + (static_cast<long long>(co) * p.ci + ci0) * p.taps + tap;
+      float* dst = p.dw + (static_cast<long long>(co) * p.taps + tap) * p.ci + ci0;
 #pragma unroll
       for (int j = 0; j < N / 8; ++j) {
         const int c = 8 * j + cq;
+        if (ci0 + c >= p.ci) continue;
         const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-        if (rows_contig && ci0 + c + 2 <= p.ci) {
-          float* q = dst + c;  // two contiguous floats: 8-byte vector reduction (or a plain store when nobody else adds)
-          if (p.single)
-            *reinterpret_cast<float2*>(q) = make_float2(v0, v1);
-          else
-            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(q), "f"(v0), "f"(v1) : "memory");
-        } else {
-          const long long step = rows_contig ? 1 : p.taps;
-          if (ci0 + c < p.ci) atomicAdd(dst + c * step, v0);
-          if (ci0 + c + 1 < p.ci) atomicAdd(dst + (c + 1) * step, v1);
-        }
+        float* q = dst + c;
+        if (p.single)  // this CTA is the only contributor: plain 8-byte store
+          *reinterpret_cast<float2*>(q) = make_float2(v0, v1);
+        else
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(q), "f"(v0), "f"(v1) : "memory");
       }
     }
   }
@@ -196,33 +188,34 @@ int wgrad_tc_launch(const CUtensorMap& mdy, const CUtensorMap& mx, const WgTcArg
 
 }  // namespace
 
-// (tw, th) with tw * th == 80, tw | wo, th | ho for the stride-2 patch mode; false: no such tiling (caller zero-stuffs)
-static bool s2_patch(int ho, int wo, int* tw, int* th) {
+// (tw, th) with tw * th == 80 for the stride-2 patch mode: the fewest tw x th patches over the ho x wo output, ties to the
+// smallest th.  An exact tiling, when one exists, is the unique minimum (ceil(ho/th) * ceil(wo/tw) >= ho * wo / 80, with
+// equality only when both divide), so it is the one chosen.
+static void s2_patch(int ho, int wo, int* tw, int* th) {
+  long long best = -1;
   for (int cand_th = 1; cand_th <= 80; ++cand_th) {
     if (80 % cand_th) continue;
     const int cand_tw = 80 / cand_th;
-    if (cand_tw <= 256 && wo % cand_tw == 0 && ho % cand_th == 0) {
+    const long long patches = static_cast<long long>((ho + cand_th - 1) / cand_th) * ((wo + cand_tw - 1) / cand_tw);
+    if (best < 0 || patches < best) {
+      best = patches;
       *tw = cand_tw;
       *th = cand_th;
-      return true;
     }
   }
-  return false;
-}
-
-int wgrad_tc_s2_supported(int h, int w) {
-  int tw, th;
-  return (h % 2 == 0 && w % 2 == 0 && s2_patch(h / 2, w / 2, &tw, &th)) ? 1 : 0;
 }
 
 static int wgrad_tc_s2(const y3_wgrad_desc& d, cudaStream_t stream) {
   // dW[co, tap, ci] += sum over OUTPUT pixels p of dy[p, co] * x[2p + tap, ci]: no zero-stuffed copy of dy, a quarter of the
-  // K extent of the stride-1 formulation on the input grid (which multiplied 75 % zeros)
+  // K extent of the stride-1 formulation on the input grid (which multiplied 75 % zeros).
+  // A patch that overhangs the output reads dy's zero halo (column wo + 1, row ho + 1) and past it the map's out-of-bounds
+  // zero fill, so its extra pixels add exactly 0.  The x map's channel extent is 2 * x_ld (the parity view), so B columns
+  // past ci read neighbouring channels: column n of the product depends only on column n of B, and the epilogue discards
+  // those columns.
+  Y3_REQUIRE(d.ksize == 3 && d.h % 2 == 0 && d.w % 2 == 0, "wgrad: the stride-2 form needs a 3x3 conv and even h, w");
   const int ho = d.h / 2, wo = d.w / 2;
   int tw = 0, th = 0;
-  Y3_REQUIRE(d.ksize == 3 && d.h % 2 == 0 && d.w % 2 == 0 && s2_patch(ho, wo, &tw, &th),
-             "wgrad: no 80-pixel patch tiling for a %dx%d stride-2 output (ask y3_conv_wgrad_s2_supported first)", ho, wo);
-  Y3_REQUIRE(d.ci % 32 == 0, "wgrad_tc: c_in=%d must be a multiple of 32", d.ci);
+  s2_patch(ho, wo, &tw, &th);
   const int n_tile = d.ci >= 128 ? 128 : (d.ci >= 64 ? 64 : 32);
   const uint32_t bcols = n_tile >= 64 ? 64 : n_tile;
   CUtensorMap mdy, mx;
@@ -254,8 +247,8 @@ static int wgrad_tc_s2(const y3_wgrad_desc& d, cudaStream_t stream) {
   a.s2 = 1;
   a.tw = tw;
   a.th = th;
-  a.tiles_w = wo / tw;
-  a.tiles_per_img = (wo / tw) * (ho / th);
+  a.tiles_w = (wo + tw - 1) / tw;
+  a.tiles_per_img = a.tiles_w * ((ho + th - 1) / th);
   a.x_ld = d.x_ld;
   a.kblocks_total = d.n * a.tiles_per_img;
   a.dy_coff = d.dy_coff;
@@ -275,7 +268,6 @@ static int wgrad_tc_s2(const y3_wgrad_desc& d, cudaStream_t stream) {
   if (want < 1 || d.deterministic) want = 1;
   a.kblocks_per_cta = static_cast<int>((a.kblocks_total + want - 1) / want);
   const unsigned splits = static_cast<unsigned>((a.kblocks_total + a.kblocks_per_cta - 1) / a.kblocks_per_cta);
-  a.layout = d.dw_layout;
   a.single = (splits == 1 && !d.accumulate) ? 1 : 0;
   const dim3 grid(splits, static_cast<unsigned>(tiles), 9u);
   switch (n_tile) {
@@ -291,7 +283,6 @@ int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream) {
   const long long rows = static_cast<long long>(d.n) * (d.h + 2) * (d.w + 2);
   Y3_REQUIRE(rows < (1ll << 31) - 4096, "wgrad: too many pixels");
   const int n_tile = d.ci >= 128 ? 128 : (d.ci >= 64 ? 64 : 32);
-  Y3_REQUIRE(d.ci % 32 == 0 || d.ci < 32, "wgrad_tc: c_in=%d must be a multiple of 32", d.ci);
   CUtensorMap mdy, mx;
   {
     const uint64_t dims[2] = {static_cast<uint64_t>(d.dy_coff + d.co), static_cast<uint64_t>(rows)};
@@ -302,6 +293,7 @@ int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream) {
   }
   const uint32_t bcols = n_tile >= 64 ? 64 : n_tile;
   {
+    // the extent x_coff + ci clips the last ci tile: its B columns past ci are zero-filled
     const uint64_t dims[2] = {static_cast<uint64_t>(d.x_coff + d.ci), static_cast<uint64_t>(rows)};
     const uint64_t strides[2] = {0, static_cast<uint64_t>(d.x_ld) * 2};
     const uint32_t box[2] = {bcols, static_cast<uint32_t>(kWgK)};
@@ -333,7 +325,6 @@ int wgrad_tc(const y3_wgrad_desc& d, cudaStream_t stream) {
   if (d.deterministic) want = 1;  // one CTA per dW tile: a single adder per address, bit-reproducible (slow on early layers)
   a.kblocks_per_cta = static_cast<int>((a.kblocks_total + want - 1) / want);
   const unsigned splits = static_cast<unsigned>((a.kblocks_total + a.kblocks_per_cta - 1) / a.kblocks_per_cta);
-  a.layout = d.dw_layout;
   a.single = (splits == 1 && !d.accumulate) ? 1 : 0;
   const dim3 grid(splits, static_cast<unsigned>(tiles), static_cast<unsigned>(taps));
   switch (n_tile) {

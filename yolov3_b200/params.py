@@ -124,7 +124,7 @@ class ParamStore:
         return self.Wbf[s.offset:s.offset + s.rows * s.taps * s.ci].view(s.rows, s.taps * s.ci)
 
     def grad_rows(self, name) -> torch.Tensor:
-        """fp32 [rows, taps, ci] view of a conv weight's gradient slot (Y3_DW_OHWI: what the wgrad kernel accumulates into)."""
+        """fp32 [rows, taps, ci] view of a conv weight's gradient slot (the [co, k*k, ci] layout the wgrad kernel accumulates into)."""
         s = self.slots[name]
         return self.G[s.offset:s.offset + s.rows * s.taps * s.ci].view(s.rows, s.taps, s.ci)
 

@@ -7,10 +7,11 @@ statistics, eps 1e-3 / momentum 0.03; ``Detect`` returning the raw ``[bs,na,ny,n
   forward  per Conv block:  conv (wgmma implicit GEMM, identity epilogue) -> bn_stats (per-block partial sums)
                             -> bn_finalize (fixed-order second stage, running statistics) -> bn_act_fwd
   backward per Conv block:  bn_act_bwd (partial sums -> dgamma/dbeta accumulated into the flat gradient buffer -> dy)
-                            -> wgrad (wgmma, accumulating straight into the parameter's .grad view)
+                            -> wgrad (wgmma, accumulating straight into the parameter's .grad view; stride-2 layers
+                               read dy on their own output grid)
                             -> dgrad, which is the SAME conv kernel run on dy with the transposed, tap-flipped weight pack
-                               (stride-2 layers: on the zero-stuffed dy), accumulating into the input's gradient through
-                               the residual port (the Bottleneck shortcut's gradient rides on that port too).
+                               (stride-2 layers: four parity-class convs of dy), accumulating into the input's gradient
+                               through the residual port (the Bottleneck shortcut's gradient rides on that port too).
 
 Parameters, gradients and the bf16 weight copy live in ONE flat buffer each (``params.ParamStore``): the forward re-packs
 all weights with two launches, the backward writes every gradient in place, and the data-parallel exchange all-reduces
@@ -44,7 +45,7 @@ class _Block:
     """One Conv+BN+SiLU block (models/common.py:57-81) with everything its forward and backward need."""
 
     __slots__ = ("prefix", "c1", "c2", "k", "s", "x", "y", "a", "res", "upsample", "wf", "wd", "st", "dw", "first", "dy",
-                 "dy_up", "post_fwd", "pre_bwd", "gamma", "beta", "rmean", "rvar", "dgamma", "dbeta", "nblk")
+                 "post_fwd", "pre_bwd", "gamma", "beta", "rmean", "rvar", "dgamma", "dbeta", "nblk")
 
 
 class TrainEngine:
@@ -106,7 +107,6 @@ class TrainEngine:
             b.nblk = T.partial_blocks(n, ho, wo, c2)
             max_partial = max(max_partial, b.nblk * 2 * c2)
             b.dy = buf(c2, ho, wo) if keep_all else self._scratch(c2, ho, wo, dev)
-            b.dy_up = self._scratch(c2, x.h, x.w, dev, tag="up") if s == 2 else None
             b.post_fwd, b.pre_bwd = [], []  # extra launches after this block's forward / before its backward (SPP pools)
             self.blocks.append(b)
             return b
@@ -237,8 +237,8 @@ class TrainEngine:
         self._graphs: dict = {}
 
     # ------------------------------------------------------------------------------------------------ helpers
-    def _scratch(self, c, hh, ww, dev, tag=""):
-        key = (c, hh, ww, tag)
+    def _scratch(self, c, hh, ww, dev):
+        key = (c, hh, ww)
         if key not in self.scratch:
             self.scratch[key] = PaddedNHWC.zeros(self.n, hh, ww, c, device=dev)
         return self.scratch[key]
@@ -409,7 +409,7 @@ class TrainEngine:
                 x = hd["x"]
                 T.head_grad_pack(g, hd["dy"], self.partial)
                 T.colreduce(self.partial, hd["nblk"], hd["pw"], hd["db"], accumulate=True)
-                T.conv_wgrad(hd["dy"], x, hd["dw"], 1, layout=_lib.DW_OHWI, accumulate=True, deterministic=det_flag)
+                T.conv_wgrad(hd["dy"], x, hd["dw"], 1, accumulate=True, deterministic=det_flag)
                 self._contribute_conv(hd["dy"], hd["wd"], hd["c1"], 1, x)
         for b in seg:
             st = b.st
@@ -425,13 +425,7 @@ class TrainEngine:
                              count=self.n * b.y.h * b.y.w * self.world)
             else:
                 T.bn_act_bwd(b.y, da, b.dy, st, st["sums"], self.partial, b.dbeta, b.dgamma, b.upsample)
-            if b.s == 2 and T.wgrad_s2_supported(b.x.h, b.x.w):
-                # wgrad straight from the un-stuffed dy (x through its parity view): a quarter of the pixels, no zeros multiplied
-                T.conv_wgrad(b.dy, b.x, b.dw, b.k, layout=_lib.DW_OHWI, accumulate=True, deterministic=det_flag, stride=2)
-            else:
-                # a stride-2 input the direct form cannot tile: stride-1 wgrad on the zero-stuffed dy
-                src = T.zero_stuff(b.dy, b.dy_up) if b.s == 2 else b.dy
-                T.conv_wgrad(src, b.x, b.dw, b.k, layout=_lib.DW_OHWI, accumulate=True, deterministic=det_flag)
+            T.conv_wgrad(b.dy, b.x, b.dw, b.k, accumulate=True, deterministic=det_flag, stride=b.s)
             if b.res is not None:
                 # Bottleneck shortcut: the block output's gradient also flows to its input.  It is folded into the next
                 # dgrad into that tensor (cv1 of the same Bottleneck: the very next block) through the residual port, or

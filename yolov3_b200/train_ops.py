@@ -1,5 +1,5 @@
 """Adapters for the training-mode entry points of the C ABI (csrc/y3_train.cu): BatchNorm statistics / apply / backward,
-weight packing, zero-stuffing, wgrad.  Like ops.py they only marshal pointers; all arithmetic is in the library."""
+weight packing, wgrad.  Like ops.py they only marshal pointers; all arithmetic is in the library."""
 from __future__ import annotations
 
 import ctypes as C
@@ -104,40 +104,14 @@ def head_grad_width(dy: PaddedNHWC) -> int:
     return (dy.ld - dy.coff + 255) // 256 * 256
 
 
-def pack_weights(w: torch.Tensor, fwd: torch.Tensor | None, dgrad: torch.Tensor | None):
-    """w fp32 [co,ci,k,k] (device) -> bf16 forward pack [co_pad, k*k*ci] / dgrad pack [ci_pad, k*k*co] (pad rows pre-zeroed)."""
-    co, ci, k, _ = w.shape
-    assert w.is_cuda and w.dtype == torch.float32 and w.is_contiguous()
-    _lib.check(_lib.lib().y3_pack_weights(w.data_ptr(), co, ci, k, fwd.data_ptr() if fwd is not None else None,
-                                          dgrad.data_ptr() if dgrad is not None else None, _stream()), "y3_pack_weights")
-
-
-def zero_stuff(src: PaddedNHWC, dst: PaddedNHWC):
-    assert dst.h == 2 * src.h and dst.w == 2 * src.w and dst.c == src.c
-    _lib.check(_lib.lib().y3_zero_stuff(src.ptr, src.ld, src.coff, dst.ptr, dst.ld, dst.coff, src.n, src.h, src.w, src.c,
-                                        _stream()), "y3_zero_stuff")
-    return dst
-
-
-def wgrad_tap_major(ci: int) -> bool:
-    """True when y3_conv_wgrad takes the [k*k, co, ci] accumulation layout for this c_in (wgmma kernel in use)."""
-    return bool(_lib.lib().y3_conv_wgrad_tap_major(int(ci)))
-
-
-def wgrad_s2_supported(h: int, w: int) -> bool:
-    """True when the direct stride-2 wgrad (no zero-stuffed dy) can tile an h x w input (y3_conv_wgrad_s2_supported)."""
-    return bool(_lib.lib().y3_conv_wgrad_s2_supported(int(h), int(w)))
-
-
-def conv_wgrad(dy: PaddedNHWC, x: PaddedNHWC, dw: torch.Tensor, ksize: int, tap_major: bool = False, layout: int | None = None,
-               accumulate: bool = False, deterministic: int = 0, stride: int = 1):
-    """dw (fp32, accumulated into) from dy and x on the same stride-1 padded grid.  Layouts: [co,ci,k,k] (default),
-    tap_major [k*k,co,ci], or ``layout=_lib.DW_OHWI`` [co,k*k,ci] (the flat gradient buffer's).  ``accumulate``: dw already holds
-    gradient that must be kept; ``deterministic``: no split over pixels (bit-reproducible)."""
+def conv_wgrad(dy: PaddedNHWC, x: PaddedNHWC, dw: torch.Tensor, ksize: int, accumulate: bool = False, deterministic: int = 0,
+               stride: int = 1):
+    """dw (fp32 [co, k*k, ci], the flat gradient buffer's layout, added to) from dy on the conv's output grid and x.
+    ``accumulate``: dw already holds gradient that must be kept; ``deterministic``: no split over pixels (bit-reproducible)."""
     assert dy.n == x.n and dy.h * stride == x.h and dy.w * stride == x.w and dw.dtype == torch.float32 and dw.is_contiguous()
+    assert dw.numel() >= dy.c * ksize * ksize * x.c
     d = _lib.WgradDesc()
     d.stride = int(stride)
-    d.dw_layout = layout if layout is not None else (1 if tap_major else 0)
     d.accumulate, d.deterministic = int(bool(accumulate)), int(deterministic)
     d.dy, d.dy_ld, d.dy_coff = dy.ptr, dy.ld, dy.coff
     d.x, d.x_ld, d.x_coff = x.ptr, x.ld, x.coff
@@ -145,12 +119,6 @@ def conv_wgrad(dy: PaddedNHWC, x: PaddedNHWC, dw: torch.Tensor, ksize: int, tap_
     d.n, d.h, d.w = x.n, x.h, x.w
     _lib.check(_lib.lib().y3_conv_wgrad(C.byref(d), _stream()), "y3_conv_wgrad")
     return dw
-
-
-def colsum_f32(g: torch.Tensor, c: int, out: torch.Tensor):
-    assert g.dtype == torch.float32 and g.dim() == 2 and g.is_contiguous()
-    _lib.check(_lib.lib().y3_colsum_f32(g.data_ptr(), g.shape[1], c, g.shape[0], out.data_ptr(), _stream()), "y3_colsum_f32")
-    return out
 
 
 def add_nhwc(src: PaddedNHWC, dst: PaddedNHWC, accumulate: bool):
