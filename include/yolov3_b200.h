@@ -388,6 +388,43 @@ int y3_val_match(const float* det, const int32_t* det_count, int32_t bs, int32_t
                  int32_t* overflow, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
+ * Validation metrics (val.py:379-429, utils/metrics.py:22-178) — csrc/y3_metrics.cu.  Caller-owned buffers, no allocation,
+ * no synchronisation: every entry point is graph-capturable.
+ *
+ * y3_val_prepare: one batch of the validation loop in native image space (val.py:394-403).
+ *   det [bs, max_det, 6] + det_count[bs] (the nms_batched output); img_params [bs, 5] = (gain, pad_x, pad_y, h0, w0) of each
+ *   image's ratio_pad / original shape; targets [nt, 6] = (image, cls, x, y, w, h) normalised, image index inside the batch;
+ *   img_w, img_h = the letterboxed batch's width and height.
+ *   det_native [bs, max_det, 6]: rows scaled by scale_boxes (y3_scale_boxes' arithmetic), class 0 when single_cls, zero rows
+ *   past the count; labels_native [nt, 6] = (image, cls, xyxy): x (w, h, w, h), xywh2xyxy, scale_boxes.
+ *   acc_conf / acc_cls [bs * max_det], acc_count [bs] = min(det_count, max_det), acc_tcls [nt] = int(cls): the accumulator's
+ *   slices of this batch.  y3_val_match(det_native, acc_count, ..., labels_native) then writes the batch's correct rows.
+ * y3_confusion_update: ConfusionMatrix(nc, conf_thres, iou_thres).process_batch(predn, labelsn) for every image of a batch
+ *   that has labels (val.py:390,406), added to matrix [(nc+1), (nc+1)] (row = predicted class, column = true class, index nc =
+ *   background) with integer atomics.  IoU as y3_val_match (eps 1e-7); a bit-equal IoU goes to the lower label / detection
+ *   index.  At most 1024 labels per image.
+ * y3_ap_per_class: ap_per_class(tp, conf, pred_cls, target_cls) (utils/metrics.py:22-91) over n_images * stride rows
+ *   (conf, cls fp32, tp [rows, niou] bytes; row d of image i counts when d < counts[i], counts NULL = all) and n_labels label
+ *   classes tcls.  Classes are integers in [0, nc), nc <= 1024; a prediction of another class value is ignored.  px [1000]
+ *   and xap [101] are np.linspace(0, 1, 1000) / (0, 1, 101).  Outputs are indexed by class id (a class without labels has
+ *   no meaning there): npred [nc + 1], nt [nc], info [2] = (max-F1 index, 1 if any tp byte is set), ap [nc, niou],
+ *   curves [3, nc, 1000] = p, r, f1 (ap_per_class's p / r / f1 before the max-F1 selection), best [5, nc] = p, r, f1, tp, fp
+ *   at the max-F1 index.  Confidence ties keep row order (stable), where the reference's argsort is unstable.
+ *   Workspace: y3_ap_workspace_bytes(n_images * stride, nc, niou) bytes (-1: unsupported shape). */
+int y3_val_prepare(const float* det, const int32_t* det_count, int32_t bs, int32_t max_det, const float* img_params,
+                   int32_t single_cls, const float* targets, int32_t nt, float img_w, float img_h, float* det_native,
+                   float* labels_native, float* acc_conf, float* acc_cls, int32_t* acc_count, int32_t* acc_tcls,
+                   y3_stream_t stream);
+int y3_confusion_update(const float* det, const int32_t* det_count, int32_t bs, int32_t max_det, const float* labels,
+                        int32_t nl, int32_t nc, float conf_thres, float iou_thres, float eps, unsigned long long* matrix,
+                        y3_stream_t stream);
+int64_t y3_ap_workspace_bytes(int32_t n_rows, int32_t nc, int32_t niou);
+int y3_ap_per_class(const float* conf, const float* cls, const uint8_t* tp, const int32_t* counts, int32_t n_images,
+                    int32_t stride, int32_t niou, const int32_t* tcls, int32_t n_labels, int32_t nc, const double* px,
+                    const double* xap, void* workspace, int64_t workspace_bytes, int32_t* npred, int32_t* nt, int32_t* info,
+                    double* ap, double* curves, double* best, y3_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
  * Optimizer step over ONE flat fp32 parameter buffer (train.py:411-421: clip_grad_norm_(10.0), SGD-nesterov with the three
  * parameter groups of smart_optimizer utils/torch_utils.py:207-237, ModelEMA.update) — csrc/y3_optim.cu.
  * Layout contract: every parameter occupies a slot whose length is a multiple of 256 elements; group[i] is the group of

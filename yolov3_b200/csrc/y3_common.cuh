@@ -459,6 +459,18 @@ __device__ __forceinline__ void pdl_entry() {
 
 int pdl_enabled();  // y3_runtime.cu
 
+// ---- box_iou(labels, detections) of one (label, detection) pair (ultralytics box_iou, reference utils/metrics.py:10):
+// inter / (area_label + area_det - inter + eps), separately rounded fp32 operations in the reference's order.  Only the
+// EXACT_SOURCES of build.py (no fast math, no FMA contraction) call it.
+__device__ __forceinline__ float iou_ld(const float4& a, const float4& b, float eps) {  // a = label box, b = detection box
+  const float w = fmaxf(__fsub_rn(fminf(a.z, b.z), fmaxf(a.x, b.x)), 0.0f);
+  const float h = fmaxf(__fsub_rn(fminf(a.w, b.w), fmaxf(a.y, b.y)), 0.0f);
+  const float inter = __fmul_rn(w, h);
+  const float a1 = __fmul_rn(__fsub_rn(a.z, a.x), __fsub_rn(a.w, a.y));
+  const float a2 = __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y));
+  return __fdiv_rn(inter, __fadd_rn(__fsub_rn(__fadd_rn(a1, a2), inter), eps));
+}
+
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
