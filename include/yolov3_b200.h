@@ -40,7 +40,7 @@ int y3_device_check(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror definitions:
  * 0 y3_conv_desc, 1 y3_first_desc, 2 y3_pool_desc, 3 y3_detect_level, 4 y3_decode_desc, 5 y3_op, 6 y3_nms_params,
  * 7 y3_loss_desc, 8 y3_bn_act_desc, 9 y3_bn_bwd_desc, 10 y3_wgrad_desc, 11 y3_pack_item, 12 y3_letterbox_desc,
- * 13 y3_amax_desc. */
+ * 13 y3_amax_desc, 14 y3_resize_item, 15 y3_augment_desc. */
 int64_t y3_abi_sizeof(int32_t which);
 /* Programmatic dependent launch between consecutive kernels of a stream (on by default; env Y3_PDL=0 or on=0 turns it off).
  * Results are identical either way — only the launch boundaries overlap.  Returns the previous setting.  A tuning switch with
@@ -361,6 +361,47 @@ typedef struct y3_letterbox_desc {
   uint8_t pad[4];
 } y3_letterbox_desc;
 int y3_letterbox_u8(const y3_letterbox_desc* d, y3_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Training augmentation on the device (LoadImagesAndLabels.__getitem__ with augment=True, utils/dataloaders.py:659-822;
+ * utils/augmentations.py:57-73,137-216,270-275) — csrc/y3_augment.cu.  Caller-owned buffers, no allocation, no
+ * synchronisation: both entry points are graph-capturable.  The descriptor arrays live in DEVICE memory.
+ *
+ * y3_resize_u8_batched: load_image's cv2.resize (INTER_LINEAR; dst = ceil(w0 r) x ceil(h0 r)) of every item in one launch,
+ *   the rule of y3_letterbox_u8.  src / dst are uint8 HWC BGR [h, w, 3] with row pitches in bytes; max_h / max_w bound the
+ *   items' dst sizes (the grid).
+ * y3_augment_u8: one output image per descriptor into out [n, 3, out_h, out_w] (uint8 CHW RGB: a TrainEngine input).  Per
+ *   output pixel: the affine warp of cv2.warpAffine (INTER_LINEAR, border 114; inv = the inverted M as
+ *   cv::invertAffineTransform computes it: A11, A12, b1, A21, A22, b2) of a VIRTUAL canvas — up to 4 placements of resized
+ *   sources (canvas rectangle [x0, x1) x [y0, y1), canvas pixel (X, Y) = source pixel (X - off_x, Y - off_y)), 114 elsewhere
+ *   (load_mosaic's img4 or letterbox's border, never materialised); with mixup, the same of canvas[1] blended as
+ *   trunc(a r + b (1 - r)) in double; with hsv, cv2's BGR2HSV, the three LUTs and HSV2BGR (augment_hsv); then flipud /
+ *   fliplr and the HWC BGR -> CHW RGB store. */
+typedef struct y3_resize_item {
+  const void* src; int32_t src_h, src_w, src_pitch;
+  void* dst;       int32_t dst_h, dst_w, dst_pitch;
+} y3_resize_item;
+int y3_resize_u8_batched(const y3_resize_item* items, int32_t n_items, int32_t max_h, int32_t max_w, y3_stream_t stream);
+
+#define Y3_AUG_MAX_PLACE 4
+typedef struct y3_aug_place {
+  const void* src;              /* uint8 HWC BGR, row pitch `pitch` bytes */
+  int32_t pitch;
+  int32_t x0, y0, x1, y1;       /* canvas rectangle */
+  int32_t off_x, off_y;         /* canvas - source coordinates */
+} y3_aug_place;
+typedef struct y3_aug_canvas {
+  y3_aug_place place[Y3_AUG_MAX_PLACE];
+  int32_t n_place;
+  double inv[6];                /* A11, A12, b1, A21, A22, b2 */
+} y3_aug_canvas;
+typedef struct y3_augment_desc {
+  y3_aug_canvas canvas[2];      /* canvas[1] is read only with mixup */
+  int32_t mixup, hsv, flipud, fliplr;
+  double mix_r;                 /* np.random.beta(32, 32) */
+  uint8_t lut[3][256];          /* hue, saturation, value */
+} y3_augment_desc;
+int y3_augment_u8(const y3_augment_desc* descs, int32_t n, int32_t out_h, int32_t out_w, void* out, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Test-time augmentation (Model._forward_augment, models/yolo.py:239-280).

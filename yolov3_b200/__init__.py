@@ -16,6 +16,7 @@ the C ABI in ``include/yolov3_b200.h``; there is no CPU or PyTorch fallback.
     DDP, scale_loss, convert_sync_batchnorm   utils/torch_utils.py:60-72, train.py:405-406, :270-272
     SGD, ModelEMA              utils/torch_utils.py:207-237 + train.py:411-421 (fused clip + SGD-nesterov + EMA)
     Pipeline                   detect.py:185-200 loop body
+    DeviceLoader, plan_item    utils/dataloaders.py:659-822 (LoadImagesAndLabels.__getitem__ with augment=True + collate_fn)
 """
 import importlib
 
@@ -27,6 +28,7 @@ _EXPORTS = {
     "ComputeLoss": "loss", "process_batch": "val", "process_batch_batched": "val", "letterbox": "preprocess",
     "forward_augment": "tta", "Ensemble": "tta", "attempt_load": "tta", "DDP": "parallel",
     "scale_loss": "parallel", "convert_sync_batchnorm": "parallel", "SGD": "optim", "ModelEMA": "optim", "Pipeline": "pipeline",
+    "DeviceLoader": "augment", "plan_item": "augment",
 }
 __all__ = sorted(_EXPORTS)
 

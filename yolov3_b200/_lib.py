@@ -165,6 +165,36 @@ class LetterboxDesc(C.Structure):
                 ("out_chw", C.c_int32), ("swap_rb", C.c_int32), ("pad", C.c_uint8 * 4)]
 
 
+class ResizeItem(C.Structure):
+    """struct y3_resize_item."""
+
+    _fields_ = [("src", C.c_void_p), ("src_h", C.c_int32), ("src_w", C.c_int32), ("src_pitch", C.c_int32),
+                ("dst", C.c_void_p), ("dst_h", C.c_int32), ("dst_w", C.c_int32), ("dst_pitch", C.c_int32)]
+
+
+AUG_MAX_PLACE = 4
+
+
+class AugPlace(C.Structure):
+    """struct y3_aug_place."""
+
+    _fields_ = [("src", C.c_void_p), ("pitch", C.c_int32), ("x0", C.c_int32), ("y0", C.c_int32), ("x1", C.c_int32),
+                ("y1", C.c_int32), ("off_x", C.c_int32), ("off_y", C.c_int32)]
+
+
+class AugCanvas(C.Structure):
+    """struct y3_aug_canvas."""
+
+    _fields_ = [("place", AugPlace * AUG_MAX_PLACE), ("n_place", C.c_int32), ("inv", C.c_double * 6)]
+
+
+class AugmentDesc(C.Structure):
+    """struct y3_augment_desc."""
+
+    _fields_ = [("canvas", AugCanvas * 2), ("mixup", C.c_int32), ("hsv", C.c_int32), ("flipud", C.c_int32),
+                ("fliplr", C.c_int32), ("mix_r", C.c_double), ("lut", (C.c_uint8 * 256) * 3)]
+
+
 class PackItem(C.Structure):
     """struct y3_pack_item."""
 
@@ -198,6 +228,8 @@ def _declare(lib):
         "y3_pack_dgrad_batched": ([vp, i32, vp, i32, vp], C.c_int),
         "y3_head_grad_pack": ([vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, vp], C.c_int),
         "y3_letterbox_u8": ([C.POINTER(LetterboxDesc), vp], C.c_int),
+        "y3_resize_u8_batched": ([vp, i32, i32, i32, vp], C.c_int),
+        "y3_augment_u8": ([vp, i32, i32, i32, vp, vp], C.c_int),
         "y3_scale_img_f32": ([vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, C.c_float, vp, vp], C.c_int),
         "y3_tta_merge": ([vp, i32, i32, i32, i32, i32, C.c_float, i32, C.c_float, vp, i32, i32, vp], C.c_int),
         "y3_val_match": ([vp, vp, i32, i32, i32, vp, i32, vp, i32, C.c_float, vp, vp, vp], C.c_int),
@@ -252,7 +284,8 @@ def lib():
         _lib = C.CDLL(str(_LIB_PATH))
         SYMBOLS.update(_declare(_lib))
         for which, st in enumerate((ConvDesc, FirstDesc, PoolDesc, DetectLevel, DecodeDesc, Op, NmsParams, LossDesc, BnActDesc,
-                                    BnBwdDesc, WgradDesc, PackItem, LetterboxDesc, AmaxDesc)):
+                                    BnBwdDesc, WgradDesc, PackItem, LetterboxDesc, AmaxDesc, ResizeItem,
+                                    AugmentDesc)):
             if _lib.y3_abi_sizeof(which) != C.sizeof(st):
                 raise Y3Error(f"ABI mismatch: sizeof({st.__name__}) is {C.sizeof(st)} here, "
                               f"{_lib.y3_abi_sizeof(which)} in {_LIB_PATH.name}; rebuild the library")

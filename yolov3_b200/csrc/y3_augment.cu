@@ -1,0 +1,196 @@
+// yolov3_b200 — the training augmentation of LoadImagesAndLabels on the device (SURVEY §8(f)).  Replaces the image arithmetic of
+//   load_image's cv2.resize                   utils/dataloaders.py:737-756   -> y3_resize_u8_batched (every source of a batch)
+//   load_mosaic's img4 / letterbox's border   utils/dataloaders.py:764-822, utils/augmentations.py:104-134
+//   random_perspective's cv2.warpAffine       utils/augmentations.py:137-216
+//   mixup                                     utils/augmentations.py:270-275
+//   augment_hsv                               utils/augmentations.py:57-73
+//   flipud / fliplr, HWC->CHW, BGR->RGB       utils/dataloaders.py:711-733   -> y3_augment_u8 (one launch per batch)
+// The mosaic canvas is virtual: every warp tap looks its pixel up in the item's placement table (114 where no source is placed),
+// so the 2s x 2s img4 is never written.  The random draws, the geometry and the labels stay on the host (yolov3_b200/augment.py).
+//
+// OpenCV's 8-bit rules restated bit for bit (opencv-python 4.13; pinned against cv2 by tests/test_augment_cpu.py):
+//  * warpAffine INTER_LINEAR: coordinates (A11 x) 1024 per column and (A12 y + b1) 1024 per row, each rounded half-even in
+//    double, + 16, >> 5; source pixel = >> 5, fraction index (Y & 31) 32 + (X & 31); 16-bit weights (units of 2^15) from float
+//    products of the k/32 fractions, which are exact, so the four always sum to 2^15; (sum + 2^14) >> 15.
+//  * BGR2HSV: max / min, the 12-bit division tables sdiv = rint((255 << 12) / i), hdiv = rint((180 << 12) / (6 i)).
+//  * HSV2BGR: float32, q = v fma(-s, f, 1), t = v fma(-s, 1 - f, 1), truncation of x * 255.
+// Compiled without fast-math / FMA contraction (build.py EXACT_SOURCES); the two fused multiply-adds OpenCV's compiler makes are
+// written as __fmaf_rn.
+#include "y3_common.cuh"
+#include "y3_internal.h"
+#include "y3_resize.cuh"
+
+namespace y3 {
+namespace {
+
+constexpr int kAugThreads = 256;
+constexpr int kAugRows = 4;  // output rows per block: the shared weight table and descriptor are set up once per 1024 pixels
+
+__global__ void __launch_bounds__(256) resize_batched_kernel(const y3_resize_item* __restrict__ items) {
+  pdl_entry();
+  const y3_resize_item it = items[blockIdx.z];
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= it.dst_w || y >= it.dst_h) return;
+  ResizeGeom g;
+  g.src = static_cast<const uint8_t*>(it.src);
+  g.src_h = it.src_h;
+  g.src_w = it.src_w;
+  g.src_pitch = it.src_pitch;
+  g.new_h = it.dst_h;
+  g.new_w = it.dst_w;
+  resize_setup(g);
+  int v[3];
+  resize_pixel(g, x, y, v);
+  uint8_t* o = static_cast<uint8_t*>(it.dst) + static_cast<size_t>(y) * it.dst_pitch + x * 3;
+  o[0] = static_cast<uint8_t>(v[0]);
+  o[1] = static_cast<uint8_t>(v[1]);
+  o[2] = static_cast<uint8_t>(v[2]);
+}
+
+// one canvas pixel: a placed source pixel, else the 114 of img4 / the letterbox border / warpAffine's borderValue
+__device__ __forceinline__ void canvas_px(const y3_aug_canvas& cv, int X, int Y, int (&t)[3]) {
+  for (int k = 0; k < cv.n_place; ++k) {
+    const y3_aug_place& p = cv.place[k];
+    if (X >= p.x0 && X < p.x1 && Y >= p.y0 && Y < p.y1) {
+      const uint8_t* q = static_cast<const uint8_t*>(p.src) + static_cast<size_t>(Y - p.off_y) * p.pitch + (X - p.off_x) * 3;
+      t[0] = q[0];
+      t[1] = q[1];
+      t[2] = q[2];
+      return;
+    }
+  }
+  t[0] = t[1] = t[2] = 114;
+}
+
+// cv2.warpAffine(canvas, M, INTER_LINEAR, BORDER_CONSTANT 114) at output pixel (x, y)
+__device__ __forceinline__ void warp_px(const y3_aug_canvas& cv, const ushort4* wtab, int x, int y, int (&v)[3]) {
+  const double* m = cv.inv;
+  const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[1], static_cast<double>(y)), m[2]), 1024.0)) + 16;
+  const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[4], static_cast<double>(y)), m[5]), 1024.0)) + 16;
+  const int X = (X0 + __double2int_rn(__dmul_rn(__dmul_rn(m[0], static_cast<double>(x)), 1024.0))) >> 5;
+  const int Y = (Y0 + __double2int_rn(__dmul_rn(__dmul_rn(m[3], static_cast<double>(x)), 1024.0))) >> 5;
+  const int sx = X >> 5, sy = Y >> 5;
+  const ushort4 w = wtab[(Y & 31) * 32 + (X & 31)];
+  int t00[3], t01[3], t10[3], t11[3];
+  canvas_px(cv, sx, sy, t00);
+  canvas_px(cv, sx + 1, sy, t01);
+  canvas_px(cv, sx, sy + 1, t10);
+  canvas_px(cv, sx + 1, sy + 1, t11);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) v[c] = (t00[c] * w.x + t01[c] * w.y + t10[c] * w.z + t11[c] * w.w + (1 << 14)) >> 15;
+}
+
+__device__ __forceinline__ int div_table(int num, int i) {  // rint(num / i), 0 at i == 0 (OpenCV's sdiv_table / hdiv_table)
+  return i == 0 ? 0 : __double2int_rn(__ddiv_rn(static_cast<double>(num), static_cast<double>(i)));
+}
+
+__host__ __device__ constexpr unsigned long long sector_code(int b, int g, int r) {
+  return static_cast<unsigned long long>(b | g << 2 | r << 4);
+}
+
+// cv2.COLOR_BGR2HSV (8U, hrange 180), the LUTs of augment_hsv, cv2.COLOR_HSV2BGR (8U) — in place on a BGR pixel
+__device__ __forceinline__ void hsv_px(const uint8_t (*lut)[256], const int* sdiv, const int* hdiv, int (&v)[3]) {
+  const int b = v[0], g = v[1], r = v[2];
+  const int vmax = max(max(b, g), r), diff = vmax - min(min(b, g), r);
+  const int s = (diff * sdiv[vmax] + 2048) >> 12;
+  int h = vmax == r ? g - b : (vmax == g ? b - r + 2 * diff : r - g + 4 * diff);
+  h = (h * hdiv[diff] + 2048) >> 12;
+  h += h < 0 ? 180 : 0;
+  const int H = lut[0][h], S = lut[1][s], V = lut[2][vmax];
+  const float vf = __fmul_rn(static_cast<float>(V), 1.f / 255.f);
+  float ob = vf, og = vf, orr = vf;
+  if (S != 0) {
+    const float sf = __fmul_rn(static_cast<float>(S), 1.f / 255.f);
+    const float hh = __fmul_rn(static_cast<float>(H), 6.f / 180.f);
+    const float sector = floorf(hh);
+    const float f = __fsub_rn(hh, sector);
+    const float p = __fmul_rn(vf, __fsub_rn(1.f, sf));
+    const float q = __fmul_rn(vf, __fmaf_rn(-sf, f, 1.f));
+    const float t = __fmul_rn(vf, __fmaf_rn(-sf, __fsub_rn(1.f, f), 1.f));
+    const auto tab = [&](unsigned i) { return i == 0 ? vf : (i == 1 ? p : (i == 2 ? q : t)); };  // (v, p, q, t)
+    // sector table {1,3,0},{1,0,2},{3,0,1},{0,2,1},{0,1,3},{2,1,0}: indices into tab for b, g, r
+    constexpr unsigned long long kSec = sector_code(1, 3, 0) | sector_code(1, 0, 2) << 6 | sector_code(3, 0, 1) << 12 |
+                                        sector_code(0, 2, 1) << 18 | sector_code(0, 1, 3) << 24 | sector_code(2, 1, 0) << 30;
+    const unsigned code = static_cast<unsigned>(kSec >> (6 * static_cast<int>(sector))) & 63u;
+    ob = tab(code & 3);
+    og = tab((code >> 2) & 3);
+    orr = tab((code >> 4) & 3);
+  }
+  v[0] = static_cast<int>(__fmul_rn(ob, 255.f));
+  v[1] = static_cast<int>(__fmul_rn(og, 255.f));
+  v[2] = static_cast<int>(__fmul_rn(orr, 255.f));
+}
+
+__global__ void __launch_bounds__(kAugThreads) augment_kernel(const y3_augment_desc* __restrict__ descs, int out_h, int out_w,
+                                                              uint8_t* __restrict__ out) {
+  __shared__ y3_augment_desc sd;
+  __shared__ ushort4 wtab[1024];  // unsigned: the weight of a zero fraction is 32768
+  __shared__ int sdiv[256], hdiv[256];
+  pdl_entry();
+  {
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(descs + blockIdx.z);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(&sd);
+    for (int i = threadIdx.x; i < static_cast<int>(sizeof(y3_augment_desc) / 4); i += kAugThreads) dst[i] = src[i];
+  }
+  for (int i = threadIdx.x; i < 1024; i += kAugThreads) {  // OpenCV's initInterTab2D for INTER_LINEAR, float products
+    const float fy = __fmul_rn(1.f / 32.f, static_cast<float>(i >> 5)), fx = __fmul_rn(1.f / 32.f, static_cast<float>(i & 31));
+    const float cy0 = __fsub_rn(1.f, fy), cx0 = __fsub_rn(1.f, fx);
+    wtab[i] = make_ushort4(static_cast<unsigned short>(__float2int_rn(__fmul_rn(__fmul_rn(cy0, cx0), 32768.f))),
+                           static_cast<unsigned short>(__float2int_rn(__fmul_rn(__fmul_rn(cy0, fx), 32768.f))),
+                           static_cast<unsigned short>(__float2int_rn(__fmul_rn(__fmul_rn(fy, cx0), 32768.f))),
+                           static_cast<unsigned short>(__float2int_rn(__fmul_rn(__fmul_rn(fy, fx), 32768.f))));
+  }
+  for (int i = threadIdx.x; i < 256; i += kAugThreads) {
+    sdiv[i] = div_table(255 << 12, i);
+    hdiv[i] = div_table(180 << 12, 6 * i);
+  }
+  __syncthreads();
+  const int ox = blockIdx.x * kAugThreads + threadIdx.x;
+  if (ox >= out_w) return;
+  const size_t plane = static_cast<size_t>(out_h) * out_w;
+  uint8_t* img = out + static_cast<size_t>(blockIdx.z) * 3 * plane;
+  const int x = sd.fliplr ? out_w - 1 - ox : ox;
+  for (int oy = blockIdx.y * kAugRows; oy < min(out_h, (blockIdx.y + 1) * kAugRows); ++oy) {
+    const int y = sd.flipud ? out_h - 1 - oy : oy;
+    int v[3];
+    warp_px(sd.canvas[0], wtab, x, y, v);
+    if (sd.mixup) {  // (im * r + im2 * (1 - r)).astype(np.uint8), float64
+      int v2[3];
+      warp_px(sd.canvas[1], wtab, x, y, v2);
+      const double r = sd.mix_r, r1 = __dsub_rn(1.0, r);
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        v[c] = static_cast<int>(__dadd_rn(__dmul_rn(static_cast<double>(v[c]), r), __dmul_rn(static_cast<double>(v2[c]), r1)));
+    }
+    if (sd.hsv) hsv_px(sd.lut, sdiv, hdiv, v);
+    const size_t at = static_cast<size_t>(oy) * out_w + ox;
+    img[at] = static_cast<uint8_t>(v[2]);  // RGB planes
+    img[plane + at] = static_cast<uint8_t>(v[1]);
+    img[2 * plane + at] = static_cast<uint8_t>(v[0]);
+  }
+}
+
+}  // namespace
+}  // namespace y3
+
+extern "C" int y3_resize_u8_batched(const y3_resize_item* items, int32_t n_items, int32_t max_h, int32_t max_w,
+                                    y3_stream_t stream) {
+  Y3_REQUIRE(items && n_items > 0 && n_items <= 65535 && max_h > 0 && max_h <= 65535 && max_w > 0,
+             "resize_batched: bad arguments (n_items %d, max %dx%d)", n_items, max_h, max_w);
+  Y3_CHECK_CUDA(::y3::launch_pdl(y3::resize_batched_kernel, dim3((max_w + 255) / 256, max_h, n_items), dim3(256), 0,
+                                 static_cast<cudaStream_t>(stream), items));
+  return Y3_OK;
+}
+
+extern "C" int y3_augment_u8(const y3_augment_desc* descs, int32_t n, int32_t out_h, int32_t out_w, void* out,
+                             y3_stream_t stream) {
+  Y3_REQUIRE(descs && out && n > 0 && n <= 65535 && out_h > 0 && out_w > 0, "augment: bad arguments (n %d, %dx%d)", n, out_h,
+             out_w);
+  Y3_REQUIRE((reinterpret_cast<uintptr_t>(descs) & 7) == 0, "augment: descriptors must be 8-byte aligned");
+  const int gy = (out_h + y3::kAugRows - 1) / y3::kAugRows;
+  Y3_REQUIRE(gy <= 65535, "augment: output too tall (%d rows)", out_h);
+  Y3_CHECK_CUDA(::y3::launch_pdl(y3::augment_kernel, dim3((out_w + y3::kAugThreads - 1) / y3::kAugThreads, gy, n),
+                                 dim3(y3::kAugThreads), 0, static_cast<cudaStream_t>(stream), descs, out_h, out_w,
+                                 static_cast<uint8_t*>(out)));
+  return Y3_OK;
+}

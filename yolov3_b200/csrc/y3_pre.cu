@@ -3,80 +3,30 @@
 //   im.transpose((2, 0, 1))[::-1]; ascontiguousarray  utils/dataloaders.py:308-310   (HWC -> CHW, BGR -> RGB)
 // with ONE kernel that reads the decoded uint8 HWC BGR frame and writes the letterboxed uint8 image either HWC/BGR (the
 // drop-in result of letterbox) or CHW/RGB — i.e. straight into the uint8 input buffer of the engine, whose first conv applies
-// the im/255 of detect.py:187-191.  The resize is OpenCV's 8-bit INTER_LINEAR restated bit for bit (third-party, opencv-python
-// 4.13; resize.cpp): 11-bit fixed-point coefficients from float fractions, horizontal pass to int, vertical pass
-// ((b0*(S0>>4))>>16 + (b1*(S1>>4))>>16 + 2) >> 2; an exact 2x shrink takes INTER_AREA's 2x2 average like cv::resize does.
+// the im/255 of detect.py:187-191.  The resize is OpenCV's 8-bit INTER_LINEAR restated bit for bit (y3_resize.cuh).
 // Compiled without fast-math / FMA contraction (build.py EXACT_SOURCES): every float step is the one OpenCV rounds.
 #include "y3_common.cuh"
 #include "y3_internal.h"
+#include "y3_resize.cuh"
 
 namespace y3 {
 namespace {
 
 struct LbArgs {
-  const uint8_t* src;   // [src_h, src_w, 3] bytes, row pitch src_pitch
-  int src_h, src_w, src_pitch;
-  int new_h, new_w;     // size after the resize (before the border)
+  ResizeGeom rs;        // source and resize
   int top, left;        // border offsets of the resized image inside the output
   int out_h, out_w;
-  double scale_x, scale_y;  // src / dst, as cv::resize computes them (1 / (dsize / ssize))
-  int mode;             // 0: copy (no resize), 1: bilinear, 2: 2x2 area average
   uint8_t pad[3];       // border colour in SOURCE channel order
   uint8_t* dst;
   int chw, swap_rb;     // output layout / channel order
 };
-
-__device__ __forceinline__ void coef(int d, double scale, int sn, bool clamp_frac, int& s0, int& a0, int& a1) {
-  float f = static_cast<float>((d + 0.5) * scale - 0.5);
-  int s = static_cast<int>(floorf(f));
-  f = __fsub_rn(f, static_cast<float>(s));
-  if (clamp_frac) {  // horizontal: cv::resize zeroes the fraction when it clamps the column; rows are clamped at fetch time only
-    if (s < 0) {
-      f = 0.f;
-      s = 0;
-    }
-    if (s >= sn - 1) {
-      f = 0.f;
-      s = sn - 1;
-    }
-  }
-  s0 = s;
-  a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.0f, f), 2048.0f));
-  a1 = __float2int_rn(__fmul_rn(f, 2048.0f));
-}
 
 __global__ void __launch_bounds__(256) letterbox_kernel(const LbArgs p) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= p.out_w) return;
   int v[3] = {p.pad[0], p.pad[1], p.pad[2]};
   const int dx = x - p.left, dy = y - p.top;
-  if (dx >= 0 && dx < p.new_w && dy >= 0 && dy < p.new_h) {
-    if (p.mode == 0) {
-      const uint8_t* q = p.src + static_cast<size_t>(dy) * p.src_pitch + dx * 3;
-      v[0] = q[0];
-      v[1] = q[1];
-      v[2] = q[2];
-    } else if (p.mode == 2) {
-      const uint8_t* q0 = p.src + static_cast<size_t>(2 * dy) * p.src_pitch + 2 * dx * 3;
-      const uint8_t* q1 = q0 + p.src_pitch;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) v[c] = (q0[c] + q0[3 + c] + q1[c] + q1[3 + c] + 2) >> 2;
-    } else {
-      int sx, ax0, ax1, sy, b0, b1;
-      coef(dx, p.scale_x, p.src_w, true, sx, ax0, ax1);
-      coef(dy, p.scale_y, p.src_h, false, sy, b0, b1);
-      const int sx1 = min(sx + 1, p.src_w - 1);
-      const int r0 = min(max(sy, 0), p.src_h - 1), r1 = min(max(sy + 1, 0), p.src_h - 1);
-      const uint8_t* q0 = p.src + static_cast<size_t>(r0) * p.src_pitch;
-      const uint8_t* q1 = p.src + static_cast<size_t>(r1) * p.src_pitch;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        const int s0 = q0[sx * 3 + c] * ax0 + q0[sx1 * 3 + c] * ax1;
-        const int s1 = q1[sx * 3 + c] * ax0 + q1[sx1 * 3 + c] * ax1;
-        v[c] = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
-      }
-    }
-  }
+  if (dx >= 0 && dx < p.rs.new_w && dy >= 0 && dy < p.rs.new_h) resize_pixel(p.rs, dx, dy, v);
   if (p.chw) {
     const size_t plane = static_cast<size_t>(p.out_h) * p.out_w, at = static_cast<size_t>(y) * p.out_w + x;
 #pragma unroll
@@ -96,27 +46,17 @@ extern "C" int y3_letterbox_u8(const y3_letterbox_desc* d, y3_stream_t stream) {
   Y3_REQUIRE(d->src_h > 0 && d->src_w > 0 && d->src_pitch >= 3 * d->src_w && d->new_h > 0 && d->new_w > 0, "letterbox: bad source / resize shape");
   Y3_REQUIRE(d->top >= 0 && d->left >= 0 && d->out_h >= d->top + d->new_h && d->out_w >= d->left + d->new_w, "letterbox: the resized image must fit the output");
   y3::LbArgs a;
-  a.src = static_cast<const uint8_t*>(d->src);
-  a.src_h = d->src_h;
-  a.src_w = d->src_w;
-  a.src_pitch = d->src_pitch;
-  a.new_h = d->new_h;
-  a.new_w = d->new_w;
+  a.rs.src = static_cast<const uint8_t*>(d->src);
+  a.rs.src_h = d->src_h;
+  a.rs.src_w = d->src_w;
+  a.rs.src_pitch = d->src_pitch;
+  a.rs.new_h = d->new_h;
+  a.rs.new_w = d->new_w;
+  y3::resize_setup(a.rs);
   a.top = d->top;
   a.left = d->left;
   a.out_h = d->out_h;
   a.out_w = d->out_w;
-  // cv::resize: inv_scale = dsize / ssize (double), scale = 1 / inv_scale
-  a.scale_x = 1.0 / (static_cast<double>(d->new_w) / d->src_w);
-  a.scale_y = 1.0 / (static_cast<double>(d->new_h) / d->src_h);
-  a.mode = 1;
-  if (d->new_h == d->src_h && d->new_w == d->src_w) {
-    a.mode = 0;
-  } else {
-    const long long isx = llrint(a.scale_x), isy = llrint(a.scale_y);
-    const double eps = 2.220446049250313e-16;
-    if (isx == 2 && isy == 2 && fabs(a.scale_x - isx) < eps && fabs(a.scale_y - isy) < eps) a.mode = 2;
-  }
   for (int c = 0; c < 3; ++c) a.pad[c] = d->pad[c];
   a.dst = static_cast<uint8_t*>(d->dst);
   a.chw = d->out_chw ? 1 : 0;

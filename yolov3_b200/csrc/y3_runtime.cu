@@ -141,6 +141,8 @@ extern "C" int64_t y3_abi_sizeof(int32_t which) {
     case 11: return sizeof(y3_pack_item);
     case 12: return sizeof(y3_letterbox_desc);
     case 13: return sizeof(y3_amax_desc);
+    case 14: return sizeof(y3_resize_item);
+    case 15: return sizeof(y3_augment_desc);
   }
   return -1;
 }
