@@ -403,6 +403,21 @@ typedef struct y3_augment_desc {
 } y3_augment_desc;
 int y3_augment_u8(const y3_augment_desc* descs, int32_t n, int32_t out_h, int32_t out_w, void* out, y3_stream_t stream);
 
+/* Validation loader on the device (LoadImagesAndLabels.__getitem__ with augment=False, utils/dataloaders.py:676-686,
+ * 699-756) — csrc/y3_augment.cu.  Both entry points read their item array from DEVICE memory (`items` / `descs`) and take
+ * the same array in HOST memory (`host_items` / `host_descs`), from which they validate every item and size the grid.
+ * Caller-owned buffers, no allocation, no synchronisation.
+ *
+ * y3_resize_area_u8_batched: load_image's cv2.resize(..., INTER_AREA) of every item in one launch, bit for bit: integer
+ *   factors take the block mean ((a+b+c+d+2)>>2 at 2x2), other scales the area tables of cv::resize in float.  Only
+ *   scales >= 1 in both axes (dst <= src) are built; an item that scales up is refused with Y3_ERR_BAD_ARG.
+ * y3_letterbox_u8_batched: y3_letterbox_u8 for n descriptors in one launch (letterbox's INTER_LINEAR resize + border +
+ *   layout), e.g. every image of a rect validation batch written straight into its [bs, 3, H, W] uint8 input. */
+int y3_resize_area_u8_batched(const y3_resize_item* items, const y3_resize_item* host_items, int32_t n_items,
+                              y3_stream_t stream);
+int y3_letterbox_u8_batched(const y3_letterbox_desc* descs, const y3_letterbox_desc* host_descs, int32_t n,
+                            y3_stream_t stream);
+
 /* ---------------------------------------------------------------------------------------------------------------
  * Test-time augmentation (Model._forward_augment, models/yolo.py:239-280).
  * y3_scale_img_f32: scale_img (ultralytics; yolo.py:246) — bilinear (align_corners = false) resample of fp32 [n,c,h,w] (read

@@ -230,6 +230,8 @@ def _declare(lib):
         "y3_letterbox_u8": ([C.POINTER(LetterboxDesc), vp], C.c_int),
         "y3_resize_u8_batched": ([vp, i32, i32, i32, vp], C.c_int),
         "y3_augment_u8": ([vp, i32, i32, i32, vp, vp], C.c_int),
+        "y3_resize_area_u8_batched": ([vp, vp, i32, vp], C.c_int),
+        "y3_letterbox_u8_batched": ([vp, vp, i32, vp], C.c_int),
         "y3_scale_img_f32": ([vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, C.c_float, vp, vp], C.c_int),
         "y3_tta_merge": ([vp, i32, i32, i32, i32, i32, C.c_float, i32, C.c_float, vp, i32, i32, vp], C.c_int),
         "y3_val_match": ([vp, vp, i32, i32, i32, vp, i32, vp, i32, C.c_float, vp, vp, vp], C.c_int),

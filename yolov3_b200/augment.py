@@ -10,7 +10,8 @@ to the device in one transfer and runs two launches — ``y3_resize_u8_batched``
 ``y3_augment_u8`` (everything else, written as uint8 CHW RGB into the ``[bs, 3, H, W]`` batch).
 
 Refused when the loader is built (NotImplementedError): ``perspective > 0`` (warpPerspective), segment (polygon) labels,
-an active Albumentations transform, and ``augment=False``."""
+an active Albumentations transform, and ``augment=False`` (served by ``yolov3_b200.valloader.DeviceValLoader``, which shares
+this module's batch machinery)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -124,8 +125,8 @@ class ItemPlan:
 def check_supported(dataset):
     """NotImplementedError for the options the device path does not build (DESIGN §9)."""
     if not getattr(dataset, "augment", False):
-        raise NotImplementedError("DeviceLoader runs the training augmentation (augment=True); augment=False resizes with "
-                                  "INTER_AREA, which is not built")
+        raise NotImplementedError("DeviceLoader runs the training augmentation (augment=True); a dataset with "
+                                  "augment=False is served by yolov3_b200.valloader.DeviceValLoader")
     hyp = dataset.hyp
     if hyp.get("perspective", 0.0):
         raise NotImplementedError("perspective > 0 needs cv2.warpPerspective, which is not built")
@@ -403,19 +404,21 @@ class _Slot:
         self.out = None
 
 
-class DeviceLoader:
-    """Iterates like the reference's training DataLoader (train.py:377): ``(imgs uint8 CUDA [bs, 3, H, W], targets [nt, 6]
-    (image index in the batch, cls, xywh normalised), paths, shapes)``.
+def _collate_targets(labels):
+    """collate_fn's targets (utils/dataloaders.py:824-830): the per-item labels with column 0 set to the batch index."""
+    targets = [lb.copy() for lb in labels]
+    for i, lb in enumerate(targets):
+        lb[:, 0] = i
+    return torch.from_numpy(np.concatenate(targets, 0))
 
-    dataset: the reference's ``LoadImagesAndLabels`` (what create_dataloader returns as its second value) or any object with
-    its attributes; sampler: any iterable of dataset indices (the reference's RandomSampler / SmartDistributedSampler), else
-    the indices in order.  The sources of batch k+1 are read on ``threads`` threads while batch k trains (``prefetch``); that
-    plans batch k+1 — draws its random numbers — before the consumer's step k, which equals the reference's order unless the
-    consumer itself draws from ``random`` / ``np.random`` between batches (train.py --multi-scale); prefetch=False keeps the
-    strict order.  Two batches are in flight: output images alternate between two device buffers."""
+
+class _BatchLoader:
+    """What the device loaders share: batches in sampler order, sources read on a thread pool while the previous batch is
+    consumed, two staging slots (pinned host + device work buffer + output images) and a side stream that runs one batch's
+    H2D copy and launches.  Subclasses provide ``_plan(index)`` -> (plan, labels) and ``_launch(plans, labels, images,
+    out, slot)``."""
 
     def __init__(self, dataset, batch_size, sampler=None, device=None, threads=8, prefetch=True, drop_last=False):
-        check_supported(dataset)
         self.dataset, self.batch_size = dataset, int(batch_size)
         self.sampler = sampler if sampler is not None else range(len(dataset.im_files))
         self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
@@ -441,25 +444,24 @@ class DeviceLoader:
 
     # ------------------------------------------------------------------------------------------------ host half
     def prepare(self, indices):
-        """Plan the items of one batch (in order: this is where the random numbers are drawn) and start reading their
+        """Plan the items of one batch (in order: this is where any random numbers are drawn) and start reading their
         sources on the thread pool."""
-        plans, labels = zip(*(plan_item(self.dataset, i) for i in indices))
+        plans, labels = zip(*(self._plan(i) for i in indices))
         raw = sorted({k[0] for p in plans for k in p.sources})
         reads = {i: self.pool.submit(read_source, self.dataset, i) for i in raw}
         return plans, labels, reads
 
     def launch(self, prepared, out=None, slot=None):
-        """Device half of one batch: one H2D copy (sources + descriptors), the resize launch(es) and the augment launch on
-        the loader's stream, writing into ``out`` (a uint8 CUDA [bs, 3, H, W] tensor, e.g. a TrainEngine input) or a
-        loader-owned buffer.  The current stream waits for the result; nothing synchronises the host."""
+        """Device half of one batch: one H2D copy (sources + descriptors) and the batch's launches on the loader's stream,
+        writing into ``out`` (a uint8 CUDA [bs, 3, H, W] tensor, e.g. an engine input) or a loader-owned buffer.  The
+        current stream waits for the result; nothing synchronises the host."""
         plans, labels, reads = prepared
         images = {i: np.ascontiguousarray(f.result()) for i, f in reads.items()}
         return self._launch(plans, labels, images, out, slot)
 
-    def _launch(self, plans, labels, images, out, slot):
-        bs = len(plans)
-        H, W = plans[0].out_hw
-        total = batch_bytes(plans, images)
+    def _device_batch(self, bs, H, W, total, fill, run, out, slot):
+        """Stage `total` bytes through slot `slot`: ``fill(dbase, host_u8, out)`` packs the pinned buffer as the device will see
+        it at dbase and returns a layout; the copy and ``run(layout, dbase, out, stream_handle)`` go to the side stream."""
         sl = self._slots[slot if slot is not None else 0]
         if sl.copied is not None:
             sl.copied.synchronize()  # the previous copy out of this slot's staging buffer has completed
@@ -469,7 +471,6 @@ class DeviceLoader:
             with torch.cuda.stream(self.stream):
                 sl.dev = torch.empty(sl.host.numel(), dtype=torch.uint8, device=self.device)
         dbase = sl.dev.data_ptr()
-        lay = pack_batch(plans, images, dbase, sl.host.numpy())
         if out is None:
             if sl.out is None or tuple(sl.out.shape) != (bs, 3, H, W):
                 with torch.cuda.stream(self.stream):
@@ -477,6 +478,7 @@ class DeviceLoader:
             out = sl.out
         assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (bs, 3, H, W), \
             f"out must be a contiguous uint8 CUDA [{bs}, 3, {H}, {W}] tensor"
+        lay = fill(dbase, sl.host.numpy(), out)
         main = torch.cuda.current_stream(self.device)
         s = self.stream
         s.wait_stream(main)  # `out` / the slot's previous images are no longer read by the consumer's queued work
@@ -484,18 +486,10 @@ class DeviceLoader:
             sl.dev[:total].copy_(sl.host[:total], non_blocking=True)
             sl.copied = torch.cuda.Event()
             sl.copied.record(s)
-            L, hs = _lib.lib(), s.cuda_stream
-            for off, n, mh, mw in lay["resize"]:
-                if n:
-                    _lib.check(L.y3_resize_u8_batched(dbase + off, n, mh, mw, hs), "y3_resize_u8_batched")
-            _lib.check(L.y3_augment_u8(dbase + lay["desc_off"], bs, H, W, out.data_ptr(), hs), "y3_augment_u8")
+            run(lay, dbase, out, s.cuda_stream)
         main.wait_stream(s)
         out.record_stream(main)
-        targets = [lb.copy() for lb in labels]
-        for i, lb in enumerate(targets):
-            lb[:, 0] = i  # collate_fn (utils/dataloaders.py:824-830)
-        targets = torch.from_numpy(np.concatenate(targets, 0))
-        return out, targets, tuple(p.path for p in plans), tuple(p.shapes for p in plans)
+        return out
 
     def collate(self, indices, out=None):
         """One batch of the given dataset indices, synchronously planned and read: (imgs, targets, paths, shapes)."""
@@ -522,3 +516,38 @@ class DeviceLoader:
 
     def close(self):
         self.pool.shutdown(wait=True)
+
+
+class DeviceLoader(_BatchLoader):
+    """Iterates like the reference's training DataLoader (train.py:377): ``(imgs uint8 CUDA [bs, 3, H, W], targets [nt, 6]
+    (image index in the batch, cls, xywh normalised), paths, shapes)``.
+
+    dataset: the reference's ``LoadImagesAndLabels`` (what create_dataloader returns as its second value) or any object with
+    its attributes; sampler: any iterable of dataset indices (the reference's RandomSampler / SmartDistributedSampler), else
+    the indices in order.  The sources of batch k+1 are read on ``threads`` threads while batch k trains (``prefetch``); that
+    plans batch k+1 — draws its random numbers — before the consumer's step k, which equals the reference's order unless the
+    consumer itself draws from ``random`` / ``np.random`` between batches (train.py --multi-scale); prefetch=False keeps the
+    strict order.  Two batches are in flight: output images alternate between two device buffers."""
+
+    def __init__(self, dataset, batch_size, sampler=None, device=None, threads=8, prefetch=True, drop_last=False):
+        check_supported(dataset)
+        super().__init__(dataset, batch_size, sampler, device, threads, prefetch, drop_last)
+
+    def _plan(self, index):
+        return plan_item(self.dataset, index)
+
+    def _launch(self, plans, labels, images, out, slot):
+        assert all(p.out_hw == plans[0].out_hw for p in plans), \
+            "items of one batch have different shapes (rect batches need an unshuffled sampler)"
+        H, W = plans[0].out_hw
+
+        def run(lay, dbase, out, hs):
+            L = _lib.lib()
+            for off, n, mh, mw in lay["resize"]:
+                if n:
+                    _lib.check(L.y3_resize_u8_batched(dbase + off, n, mh, mw, hs), "y3_resize_u8_batched")
+            _lib.check(L.y3_augment_u8(dbase + lay["desc_off"], len(plans), H, W, out.data_ptr(), hs), "y3_augment_u8")
+
+        out = self._device_batch(len(plans), H, W, batch_bytes(plans, images),
+                                 lambda dbase, host, _: pack_batch(plans, images, dbase, host), run, out, slot)
+        return out, _collate_targets(labels), tuple(p.path for p in plans), tuple(p.shapes for p in plans)

@@ -1,7 +1,8 @@
 // yolov3_b200 — OpenCV's 8-bit INTER_LINEAR resize (third-party, opencv-python 4.13; resize.cpp) restated bit for bit, shared
 // by the letterbox kernel (y3_pre.cu) and the batched resize of the training loader (y3_augment.cu): 11-bit fixed-point
 // coefficients from float fractions, horizontal pass to int, vertical pass ((b0*(S0>>4))>>16 + (b1*(S1>>4))>>16 + 2) >> 2; an
-// exact 2x shrink takes INTER_AREA's 2x2 average like cv::resize does, and an equal size is a plain copy.
+// exact 2x shrink takes INTER_AREA's 2x2 average like cv::resize does, and an equal size is a plain copy.  INTER_AREA for
+// scales >= 1 (the validation loader's load_image shrink, y3_augment.cu) follows at the end.
 // Include only from sources compiled without fast-math / FMA contraction (build.py EXACT_SOURCES).
 #pragma once
 
@@ -15,7 +16,8 @@ struct ResizeGeom {
   int src_h, src_w, src_pitch;
   int new_h, new_w;          // size after the resize
   double scale_x, scale_y;   // src / dst, as cv::resize computes them (1 / (dsize / ssize))
-  int mode;                  // 0: copy (no resize), 1: bilinear, 2: 2x2 area average
+  int mode;                  // 0: copy (no resize), 1: bilinear, 2: 2x2 area average, 3: kx x ky block mean, 4: area
+  int kx, ky;                // the integer factors of mode 3
 };
 
 // scale and mode of a resize from the sizes (the scalar part of cv::resize)
@@ -78,6 +80,104 @@ __device__ __forceinline__ void resize_pixel(const ResizeGeom& p, int dx, int dy
       v[c] = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
     }
   }
+}
+
+// ------------------------------------------------------------------------------------------------------------ INTER_AREA
+// cv::resize(..., INTER_AREA) for 8-bit, 3-channel images and scales >= 1 in both axes (resizeAreaFast_ / resizeArea_):
+//  * an integer factor (kx, ky) in both axes: (2, 2) is the (a+b+c+d+2)>>2 of mode 2; any other is the integer block sum
+//    times the float 1 / (kx ky), rounded half-even (mode 3);
+//  * any other scale (mode 4): per axis the spans of computeResizeAreaTab, built in double with float alphas; per source
+//    row of the y-span, buf = sum of S alpha over the x-span (float, in table order), then sum = beta buf, sum += beta buf;
+//    the output is sum rounded half-even, saturated.
+__host__ __device__ inline void area_setup(ResizeGeom& g) {
+  g.scale_x = 1.0 / (static_cast<double>(g.new_w) / g.src_w);
+  g.scale_y = 1.0 / (static_cast<double>(g.new_h) / g.src_h);
+  g.kx = g.ky = 0;
+  if (g.new_h == g.src_h && g.new_w == g.src_w) {
+    g.mode = 0;
+    return;
+  }
+  const long long isx = llrint(g.scale_x), isy = llrint(g.scale_y);
+  const double eps = 2.220446049250313e-16;
+  if (fabs(g.scale_x - isx) < eps && fabs(g.scale_y - isy) < eps) {
+    g.mode = isx == 2 && isy == 2 ? 2 : 3;
+    g.kx = static_cast<int>(isx);
+    g.ky = static_cast<int>(isy);
+  } else {
+    g.mode = 4;
+  }
+}
+
+// the entries of computeResizeAreaTab for one destination index: an optional leading partial source index (s1 - 1), the
+// full indices [s1, s2) and an optional trailing partial index s2
+struct AreaSpan {
+  int s1, s2;
+  bool lead, trail;
+  float a_lead, a_full, a_trail;
+};
+
+__device__ __forceinline__ AreaSpan area_span(int d, double scale, int ssize) {
+  AreaSpan sp;
+  const double fs1 = d * scale, fs2 = fs1 + scale;
+  const double rest = ssize - fs1;
+  const double cell = rest < scale ? rest : scale;  // std::min(scale, ssize - fsx1)
+  int s1 = static_cast<int>(ceil(fs1));
+  int s2 = static_cast<int>(floor(fs2));
+  s2 = min(s2, ssize - 1);
+  s1 = min(s1, s2);
+  sp.s1 = s1;
+  sp.s2 = s2;
+  sp.lead = s1 - fs1 > 1e-3;
+  sp.a_lead = static_cast<float>((s1 - fs1) / cell);
+  sp.a_full = static_cast<float>(1.0 / cell);
+  sp.trail = fs2 - s2 > 1e-3;
+  const double t = fs2 - s2 < 1.0 ? fs2 - s2 : 1.0;
+  sp.a_trail = static_cast<float>((cell < t ? cell : t) / cell);
+  return sp;
+}
+
+__device__ __forceinline__ void area_row(const uint8_t* row, const AreaSpan& x, float (&buf)[3]) {
+  buf[0] = buf[1] = buf[2] = 0.f;
+  const auto tap = [&](int sx, float a) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) buf[c] = __fadd_rn(buf[c], __fmul_rn(static_cast<float>(row[sx * 3 + c]), a));
+  };
+  if (x.lead) tap(x.s1 - 1, x.a_lead);
+  for (int sx = x.s1; sx < x.s2; ++sx) tap(sx, x.a_full);
+  if (x.trail) tap(x.s2, x.a_trail);
+}
+
+// pixel (dx, dy) of the INTER_AREA-resized image (area_setup), in source channel order
+__device__ __forceinline__ void area_pixel(const ResizeGeom& p, int dx, int dy, int (&v)[3]) {
+  if (p.mode == 3) {
+    const uint8_t* q = p.src + static_cast<size_t>(dy) * p.ky * p.src_pitch + static_cast<size_t>(dx) * p.kx * 3;
+    int s[3] = {0, 0, 0};
+    for (int r = 0; r < p.ky; ++r, q += p.src_pitch)
+      for (int k = 0; k < p.kx; ++k) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) s[c] += q[k * 3 + c];
+      }
+    const float inv = __fdiv_rn(1.f, static_cast<float>(p.kx * p.ky));
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = min(max(__float2int_rn(__fmul_rn(static_cast<float>(s[c]), inv)), 0), 255);
+    return;
+  }
+  if (p.mode != 4) {
+    resize_pixel(p, dx, dy, v);  // copy, 2x2
+    return;
+  }
+  const AreaSpan x = area_span(dx, p.scale_x, p.src_w), y = area_span(dy, p.scale_y, p.src_h);
+  float sum[3] = {0.f, 0.f, 0.f}, buf[3];
+  const auto row = [&](int sy, float beta) {
+    area_row(p.src + static_cast<size_t>(sy) * p.src_pitch, x, buf);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) sum[c] = __fadd_rn(sum[c], __fmul_rn(beta, buf[c]));
+  };
+  if (y.lead) row(y.s1 - 1, y.a_lead);
+  for (int sy = y.s1; sy < y.s2; ++sy) row(sy, y.a_full);
+  if (y.trail) row(y.s2, y.a_trail);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) v[c] = min(max(__float2int_rn(sum[c]), 0), 255);
 }
 
 }  // namespace y3

@@ -4,7 +4,10 @@
 returns ``bool [N, len(iouv)]`` on ``iouv.device``); ``process_batch_batched`` takes the padded NMS output of a whole batch
 (``nms_batched``: ``[bs, max_det, 6]`` + counts) and the collated labels ``[nl, 6] = (image, cls, xyxy)`` and returns
 ``[bs, max_det, niou]`` without any device->host synchronisation — the reference copies every image's IoU matrix to the host
-and runs numpy argsort/unique per threshold."""
+and runs numpy argsort/unique per threshold.
+
+``run`` is val.run (val.py:191-489) for an existing model and validation loader, the whole batch loop on the device
+(``import yolov3_b200.val as validate`` serves train.py's per-epoch call unchanged)."""
 from __future__ import annotations
 
 from typing import NamedTuple
@@ -176,3 +179,133 @@ def process_batch(detections: torch.Tensor, labels: torch.Tensor, iouv: torch.Te
     det = detections.detach().float().contiguous().view(1, n, 6)
     lab = torch.cat((torch.zeros(m, 1, device=detections.device), labels.to(detections.device).float()), 1)
     return process_batch_batched(det, None, lab, iouv)[0].to(iouv.device)
+
+
+# ------------------------------------------------------------------------------------------------------------- val.run
+class _Pending(NamedTuple):
+    """One batch whose NMS candidate overflow has not been read yet."""
+
+    z: torch.Tensor
+    det: torch.Tensor
+    counts: torch.Tensor
+    overflow: torch.Tensor     # pinned host copy of nms_batched's per-image overflow
+    ready: torch.cuda.Event    # recorded after that copy
+    targets: torch.Tensor
+    img_hw: tuple
+    shapes: tuple
+
+
+def _device_val_loader(dataloader):
+    """The DeviceValLoader serving `dataloader`; one built from a reference DataLoader is cached on it, so its thread pool
+    and staging buffers live across the epochs of a training run."""
+    from .valloader import DeviceValLoader
+
+    if isinstance(dataloader, DeviceValLoader):
+        return dataloader
+    dl = getattr(dataloader, "_y3_device_val_loader", None)
+    if dl is None:
+        dl = DeviceValLoader(dataloader)
+        try:
+            dataloader._y3_device_val_loader = dl
+        except AttributeError:
+            pass
+    return dl
+
+
+def run(data=None, weights=None, batch_size=32, imgsz=640, conf_thres=0.001, iou_thres=0.6, max_det=300, task="val",
+        device="", workers=8, single_cls=False, augment=False, verbose=False, save_txt=False, save_hybrid=False,
+        save_conf=False, save_json=False, project=None, name="exp", exist_ok=False, half=True, dnn=False, model=None,
+        dataloader=None, save_dir=None, plots=True, callbacks=None, compute_loss=None):
+    """val.run (reference val.py:191-489) for an existing model and validation loader — the per-epoch call of train.py:447-459
+    — with the whole batch loop on the device: the DeviceValLoader batch (INTER_AREA + letterbox on the GPU), the forward on
+    the uint8 batch (``/255`` fused), ``compute_loss`` (val loss), ``nms_batched`` and ``ValAccumulator``.
+
+    Returns ``((mp, mr, map50, map, *(loss / len(dataloader))), maps, t)`` with ``t`` the per-image milliseconds of
+    (pre-process, inference, NMS) measured with CUDA events and read at the end.  ``model``: a ``DetectionModel``, ``Model``
+    or ``DetectMultiBackend``; ``dataloader``: the reference's validation ``DataLoader`` or a ``DeviceValLoader``.
+    ``data`` gives ``nc`` (else the model's).  The images stay on the device, so ``callbacks`` get ``on_val_start`` and
+    ``on_val_batch_start`` but not ``on_val_image_end`` / ``on_val_batch_end``, whose arguments are per-image host
+    tensors; ``plots``, ``save_txt``, ``save_hybrid`` and ``save_json`` raise NotImplementedError (the reference's val.run
+    serves them).  Nothing is read back per batch except NMS candidate overflow: batch k's flags are read after batch
+    k+1 is queued, and a batch that overflowed runs NMS again with the exact capacity before its rows are accumulated, as
+    ``non_max_suppression`` does — the detections are always those of exact NMS."""
+    from .nms import nms_batched
+
+    if model is None or dataloader is None:
+        raise ValueError("yolov3_b200.val.run needs an existing model and dataloader (the reference's val.run builds them "
+                         "from weights and data)")
+    if plots or save_txt or save_hybrid or save_json:
+        raise NotImplementedError("plots, save_txt, save_hybrid and save_json need per-image host results; use the "
+                                  "reference's val.run for them")
+    loader = _device_val_loader(dataloader)
+    dev = torch.device(getattr(model, "device", None) or loader.device)
+    if hasattr(model, "half") and hasattr(model, "float"):
+        model.half() if half else model.float()  # val.py:284
+    if hasattr(model, "eval"):
+        model.eval()
+    if single_cls:
+        nc = 1
+    elif isinstance(data, dict) and "nc" in data:
+        nc = int(data["nc"])
+    else:
+        nc = int(getattr(model, "nc", None) or model.model.nc)
+    iouv = torch.linspace(0.5, 0.95, 10, device=dev)
+    acc = ValAccumulator(nc, iouv, single_cls=single_cls)
+    loss = torch.zeros(3, device=dev)
+    events = []
+    if callbacks is not None:
+        callbacks.run("on_val_start")
+
+    def finish(p: _Pending):
+        p.ready.synchronize()
+        det, counts, overflow = p.det, p.counts, p.overflow
+        worst = int(overflow.max())
+        while worst:  # exact retry (nms.non_max_suppression): every candidate fits
+            det, counts, ov, _ = nms_batched(p.z, conf_thres, iou_thres, multi_label=True, agnostic=single_cls,
+                                             max_det=max_det, cap=1 << (worst - 1).bit_length())
+            worst = int(ov.max())
+        acc.update(det, counts, p.targets, p.img_hw, p.shapes)
+
+    pending = None
+    seen = 0
+    with torch.no_grad():
+        it = iter(loader)
+        while True:
+            ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+            ev[0].record()
+            batch = next(it, None)
+            if batch is None:
+                break
+            if callbacks is not None:
+                callbacks.run("on_val_batch_start")
+            im, targets, paths, shapes = batch
+            targets = targets.float().pin_memory().to(dev, non_blocking=True)
+            nb, _, height, width = im.shape
+            ev[1].record()
+            preds, train_out = model(im) if compute_loss else (model(im, augment=augment), None)
+            if compute_loss:
+                loss += compute_loss(train_out, targets)[1]
+            ev[2].record()
+            z = preds[0] if isinstance(preds, (list, tuple)) else preds
+            det, counts, overflow, _ = nms_batched(z, conf_thres, iou_thres, multi_label=True, agnostic=single_cls,
+                                                   max_det=max_det)
+            ev[3].record()
+            events.append(ev)
+            ov = torch.empty(overflow.shape, dtype=overflow.dtype, pin_memory=True)
+            ov.copy_(overflow, non_blocking=True)
+            ready = torch.cuda.Event()
+            ready.record()
+            if pending is not None:
+                finish(pending)
+            pending = _Pending(z, det, counts, ov, ready, targets, (height, width), shapes)
+            seen += nb
+        if pending is not None:
+            finish(pending)
+    r = acc.results()
+    dt = np.zeros(3)
+    for ev in events:
+        dt += [ev[0].elapsed_time(ev[1]), ev[1].elapsed_time(ev[2]), ev[2].elapsed_time(ev[3])]
+    t = tuple(float(x) / max(seen, 1) for x in dt)
+    if hasattr(model, "float"):
+        model.float()  # val.py:482
+    return (r.mp, r.mr, r.map50, r.map, *(loss.cpu() / len(dataloader)).tolist()), r.maps, t
