@@ -116,3 +116,109 @@ def test_gradient_bucket_partition(name, n_buckets):
         # ... and it holds the layers whose backward finishes last (model.0 ...)
         tail = [n for n in st.order if r[-1][0] <= st.slots[n].offset < r[-1][1]]
         assert any(n.startswith("model.0.") for n in tail) and all(int(n.split(".")[1]) <= 7 for n in tail)
+
+
+# ------------------------------------------------------------------------------------------------ one copy, one version
+@pytest.mark.parametrize("name", ["yolov3", "yolov3-spp", "yolov3-tiny"])
+def test_params_is_the_store_and_packs_do_not_depend_on_where_it_lives(name):
+    from yolov3_b200.model import Model
+
+    m, st, _ = _store(name)
+    assert list(m.params) == list(st.views) and all(m.params[k] is st.views[k] for k in st.views)
+    assert m.device_params() is m.params
+    k0 = next(iter(m.params))
+    with pytest.raises(TypeError):
+        m.params[k0] = torch.zeros_like(m.params[k0])  # would detach the name from the flat buffer
+    with torch.no_grad():  # stored weights that differ from what a fresh model starts with, BN statistics included
+        for k, v in m.params.items():
+            if not k.endswith("anchors"):
+                v.mul_(1.25).add_(0.01)
+    fresh = Model(CFG / f"{name}.yaml", device="cpu")
+    fresh.load_state_dict(m.state_dict())
+    assert fresh._store is None
+    a, b = m.packed(), fresh.packed()
+    prefixes = list(a)
+    assert prefixes == list(b)
+    for prefix in prefixes:
+        assert all(torch.equal(x, y) for x, y in zip(a[prefix], b[prefix])), prefix
+        assert all(torch.equal(x, y) for x, y in zip(m.packed_e4m3(prefix), fresh.packed_e4m3(prefix))), prefix
+    for cs in m.conv_specs:
+        if cs.s == 2 and cs.k == 3:  # yolov3-tiny downsamples with max-pools: it has none
+            assert all(torch.equal(x, y) for x, y in zip(m.packed_xpair(cs.prefix), fresh.packed_xpair(cs.prefix))), cs.prefix
+
+
+def test_state_dict_round_trip_keeps_bits_and_addresses():
+    from yolov3_b200.model import Model
+
+    cfg = CFG / "yolov3-tiny.yaml"
+    m = Model(cfg, device="cpu")
+    sd = O.init_params(cfg, seed=3)
+    m.load_state_dict(sd)  # before the store exists: host tensors are replaced
+    got = m.state_dict()
+    assert list(got) == list(sd) and all(torch.equal(got[k], sd[k]) for k in sd)
+    st = m.store()
+    ptrs = {k: v.data_ptr() for k, v in st.views.items()}
+    got = m.state_dict()
+    assert list(got) == list(sd) and all(torch.equal(got[k], sd[k]) and got[k].is_contiguous() for k in sd)
+    sd2 = O.init_params(cfg, seed=4)
+    m.load_state_dict(sd2)  # after: copied in place, an optimizer built on parameters() keeps valid tensors
+    assert {k: v.data_ptr() for k, v in m.params.items()} == ptrs
+    assert all(m.params[k] is st.views[k] for k in sd2)
+    got = m.state_dict()
+    assert all(torch.equal(got[k], sd2[k]) for k in sd2)
+    assert torch.equal(m.detect.anchors, sd2[f"model.{m.detect.i}.anchors"]) and not m.detect.anchors.requires_grad
+
+
+def test_weights_version_moves_exactly_when_a_weight_may_have_changed():
+    m, _, _ = _store("yolov3-tiny")
+    m2 = type(m)(CFG / "yolov3-tiny.yaml", device="cpu")
+    v = m2.weights_version()
+    m2.packed(), m2.state_dict(), m2.eval(), m2.train(), m2.eval(), list(m2.params)
+    assert m2.weights_version() == v
+    st = m2.store()  # initialised from the same values: nothing changed
+    m2.parameters(), m2.device_params(), m2.zero_grad(), st.attach_grads(), st.zero_grad(False), m2.packed(), m2.state_dict()
+    assert m2.weights_version() == v
+    seen = {v}
+
+    def moved():
+        n = len(seen)
+        seen.add(m2.weights_version())
+        return len(seen) == n + 1
+
+    m2.load_state_dict(m.state_dict())
+    assert moved()
+    with torch.no_grad():
+        m2.params["model.0.bn.running_var"].mul_(2.0)
+    assert moved()
+    with torch.no_grad():
+        m2.params[f"model.{m2.detect.i}.m.1.weight"].add_(1.0)  # a strided nn.Parameter view
+    assert moved()
+    st.mark_written()
+    assert moved()
+    m2.state_dict(), m2.packed(), m2.eval()
+    assert not moved()
+
+
+def test_packs_calibration_and_engines_follow_the_weights_version():
+    from yolov3_b200 import _lib
+    from yolov3_b200.model import Engine
+
+    m, st, _ = _store("yolov3-tiny")
+    changes = [lambda: m.load_state_dict(O.init_params(CFG / "yolov3-tiny.yaml", seed=1)),
+               lambda: m.params["model.0.bn.running_mean"].add_(0.5),
+               st.mark_written]
+    for change in changes:
+        m.load_fp8_scales({k: 1.0 for k in m.fp8_tensor_names()})
+        W = m.packed()
+        e = Engine(m, 1, 64, 64, dry_run=True)
+        m._engines["kept"] = e
+        assert not e.stale and m.packed() is W and m.fp8_scales is not None
+        with torch.no_grad():
+            change()
+        assert e.stale
+        with pytest.raises(_lib.Y3Error, match="weights that have since changed"):
+            e._check_fresh()
+        assert m.packed() is not W and m.fp8_scales is None and not m._engines
+        with pytest.raises(_lib.Y3Error, match="no FP8 calibration"):
+            Engine(m, 1, 64, 64, dry_run=True, precision="fp8")
+        assert not Engine(m, 1, 64, 64, dry_run=True).stale

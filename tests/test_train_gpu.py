@@ -389,3 +389,97 @@ def test_train_step_vs_oracle_autograd(cfg_name):
     m.eval()
     z, _ = m(x.cuda())
     assert torch.isfinite(z).all()
+
+
+# ------------------------------------------------------------------------------------------------ weight changes reach inference
+def _tiny(seed):
+    from pathlib import Path
+
+    import yolo_oracle as O
+
+    cfg = Path(__file__).resolve().parents[1] / "yolov3_b200" / "cfg" / "yolov3-tiny.yaml"
+    return cfg, O.init_params(cfg, seed=seed)
+
+
+def _fresh_z(m, x):
+    """z of a new plain Model holding ``m``'s weights: what inference with the current weights must return."""
+    from yolov3_b200.model import Model
+
+    fresh = Model(m.yaml, device=x.device)
+    fresh.load_state_dict({k: v for k, v in m.state_dict().items() if not k.endswith("num_batches_tracked")})
+    return fresh.eval()(x)[0]
+
+
+def test_facade_eval_after_train_forward_without_optimizer_step():
+    """A train-mode forward writes the BatchNorm running statistics from a kernel; with no optimizer step after it, the
+    next eval-mode forward must still infer with them — on the eager first forward and on the graph replays alike."""
+    from yolov3_b200.module import DetectionModel
+
+    cfg, params = _tiny(0)
+    m = DetectionModel(cfg)
+    m.core.load_state_dict(params)
+    x = torch.rand(4, 3, 128, 128, generator=torch.Generator().manual_seed(5)).cuda()
+    m.eval()
+    z_prev = m(x)[0]
+    for _ in range(3):  # eager, captured + replayed, replayed
+        m.train()
+        m(x)
+        m.eval()
+        z = m(x)[0]
+        assert torch.equal(z, _fresh_z(m, x)) and not torch.equal(z, z_prev)
+        z_prev = z
+
+
+def _change_weights(m, how, x):
+    if how == "load_state_dict":
+        m.load_state_dict(_tiny(1)[1])
+    elif how == "inplace_op":
+        with torch.no_grad():
+            m.device_params()["model.2.bn.weight"].mul_(1.5)
+    else:
+        m.train()
+        m(x)
+        m.eval()
+
+
+@pytest.mark.parametrize("how", ["load_state_dict", "inplace_op", "train_forward"])
+def test_model_in_eval_mode_picks_up_weight_changes_and_kept_engines_raise(how):
+    from yolov3_b200._lib import Y3Error
+    from yolov3_b200.model import Model
+
+    cfg, params = _tiny(0)
+    m = Model(cfg)
+    m.load_state_dict(params)
+    m.eval()
+    x = torch.rand(2, 3, 128, 128, generator=torch.Generator().manual_seed(6)).cuda()
+    z0 = m(x)[0]
+    e = m.engine(2, 128, 128)
+    m.device_params()  # creating the store changes no weight: the engine stays valid
+    assert not e.stale and m.engine(2, 128, 128) is e
+    _change_weights(m, how, x)
+    assert e.stale
+    with pytest.raises(Y3Error, match="weights that have since changed"):
+        e.run(x)
+    z = m(x)[0]
+    assert torch.equal(z, _fresh_z(m, x)) and not torch.equal(z, z0)
+    assert m.engine(2, 128, 128) is not e and not m.engine(2, 128, 128).stale
+
+
+@pytest.mark.parametrize("how", ["load_state_dict", "inplace_op", "train_forward"])
+def test_fp8_calibration_goes_with_the_weights_it_was_taken_on(how):
+    from yolov3_b200._lib import Y3Error
+    from yolov3_b200.model import Engine, Model
+
+    cfg, params = _tiny(0)
+    m = Model(cfg)
+    m.load_state_dict(params)
+    x = torch.rand(2, 3, 128, 128, generator=torch.Generator().manual_seed(7)).cuda()
+    m.calibrate_fp8([x])
+    m.precision = "fp8"
+    assert torch.isfinite(m(x)[0]).all()
+    _change_weights(m, how, x)
+    with pytest.raises(Y3Error, match="no FP8 calibration"):
+        Engine(m, 2, 128, 128, precision="fp8")
+    assert m.fp8_scales is None
+    with pytest.raises(Y3Error, match="no FP8 calibration"):
+        m(x)

@@ -18,6 +18,7 @@ import ctypes as C
 import math
 from collections import OrderedDict
 from copy import deepcopy
+from types import MappingProxyType
 
 import torch
 
@@ -88,16 +89,18 @@ class Model:
         self.training = False
         self.sync_bn = False  # parallel.convert_sync_batchnorm(): train-mode BN statistics over all ranks
         self.hyp = None
+        # name -> tensor in state_dict order, the ONE copy of the weights: host tensors (assignable) until store() moves
+        # them into the flat device buffer, the store's views (read-only mapping) from then on
         self.params = self._init_params()
+        self._store = None
+        self._host_ver = 0  # load_state_dict / to(): the changes the store's own counter cannot see
         self._packed = None
         self._engines: "OrderedDict" = OrderedDict()  # LRU over input shapes, at most MAX_ENGINES alive
-        self._dev = None
-        self._store = None
         self.ddp = None  # parallel.DDP(model): overlapped gradient exchange
         self._train_engines: dict = {}
-        self._wver = 0  # bumped whenever the weights an Engine baked into its TMA descriptors may have changed
         self._precision = "bf16"
         self._fp8_scales = None  # {tensor name: scale} from calibrate_fp8 / load_fp8_scales
+        self._built = self.weights_version()  # what the packs, the FP8 calibration and the engines were made from
 
     # ------------------------------------------------------------------------------------------------ parameters
     def _init_params(self):
@@ -124,13 +127,20 @@ class Model:
 
     MAX_ENGINES = 4  # lowered inference engines kept alive (one per input shape/dtype); older ones are destroyed
 
+    def weights_version(self):
+        """Changes whenever any weight may have changed: ``load_state_dict`` / ``to()``, and once the store exists a torch
+        in-place op on any view or a kernel of ours writing the flat buffer (``ParamStore.version``)."""
+        return self._host_ver, self._store.version() if self._store is not None else (0, 0)
+
     def _invalidate(self):
         """The packed bf16 weights (whose device addresses live inside every Engine's TMA descriptors) are stale.  The FP8
-        calibration was taken with those weights: it goes too."""
-        self._wver += 1
+        calibration was taken with those weights: it goes too.  The decode descriptor and ``ComputeLoss`` read the anchors
+        on the host: that copy is re-read here."""
+        self._built = self.weights_version()
         self._packed = None
         self._fp8_scales = None
         self._engines.clear()
+        self.detect.anchors = self.params[f"model.{self.detect.i}.anchors"].detach().float().cpu()
 
     # ------------------------------------------------------------------------------------------------ FP8 inference
     PRECISIONS = ("bf16", "fp8")
@@ -211,36 +221,29 @@ class Model:
         W = self.packed()
         key = prefix + "#e4m3"
         if key not in W:
-            P = self.params
-            if prefix + ".bn.weight" in P:
-                w, b = self.fold_bn(P[prefix + ".conv.weight"], P[prefix + ".bn.weight"], P[prefix + ".bn.bias"],
-                                    P[prefix + ".bn.running_mean"], P[prefix + ".bn.running_var"])
-            else:
-                w, b = P[prefix + ".weight"], P[prefix + ".bias"]
-            W[key] = ops.pack_conv_weight_e4m3(w, b, self.device)
+            W[key] = ops.pack_conv_weight_e4m3(*self._folded(prefix), self.device)
         return W[key]
 
     def state_dict(self):
-        """Reference-named fp32 tensors (host copies).  While device masters exist (training) they are the truth."""
-        if self._dev is not None:
-            return OrderedDict((k, v.detach().float().cpu().contiguous().clone()) for k, v in self._dev.items())
-        return OrderedDict((k, v.clone()) for k, v in self.params.items())
+        """Reference-named fp32 tensors (host copies of ``params``)."""
+        return OrderedDict((k, v.detach().float().cpu().contiguous().clone()) for k, v in self.params.items())
 
     def load_state_dict(self, sd, strict=True):
         missing = [k for k in self.params if k not in sd]
         unexpected = [k for k in sd if k not in self.params and not k.endswith("num_batches_tracked")]
         if strict and (missing or unexpected):
             raise RuntimeError(f"load_state_dict: missing {missing[:4]}..., unexpected {unexpected[:4]}...")
-        for k in self.params:
+        for k, p in self.params.items():
             if k in sd:
                 v = sd[k].detach().float().cpu()
-                assert v.shape == self.params[k].shape, (k, v.shape, self.params[k].shape)
-                self.params[k] = v.clone()
-                if self._dev is not None:
+                assert v.shape == p.shape, (k, v.shape, p.shape)
+                if self._store is None:
+                    self.params[k] = v.clone()
+                else:
                     # device masters are updated IN PLACE: an optimizer / EMA built on parameters() keeps valid tensors
                     with torch.no_grad():
-                        self._dev[k].copy_(v)
-        self.detect.anchors = self.params[f"model.{self.detect.i}.anchors"]
+                        p.copy_(v)
+        self._host_ver += 1
         self._invalidate()
         return missing, unexpected
 
@@ -258,42 +261,30 @@ class Model:
         if self._store is None:
             from .params import ParamStore
 
-            self._store = ParamStore(self, ops.cout_pad)
-            self._dev = self._store.views
+            self._store = ParamStore(self, ops.cout_pad)  # initialised from the host tensors in ``params``
+            self.params = MappingProxyType(self._store.views)
         return self._store
 
     def device_params(self):
         """fp32 master copy of every parameter/buffer on the device — views of ONE flat buffer (leaf tensors, requires_grad
         for the trainable ones): what ``TrainEngine`` reads each step and what ``optimizer.step()`` writes."""
-        return self.store().views
+        self.store()
+        return self.params
 
     def zero_grad(self, set_to_none: bool = True):
         """One memset over the flat gradient buffer (instead of one fill per parameter)."""
         if self._store is not None:
             self._store.zero_grad(set_to_none)
 
-    def sync_from_device(self):
-        """Copy the trained master parameters back into ``self.params`` (invalidates packed weights and engines)."""
-        if self._dev is not None:
-            for k, v in self._dev.items():
-                self.params[k] = v.detach().float().cpu().contiguous().clone()
-            self.detect.anchors = self.params[f"model.{self.detect.i}.anchors"]
-            self._invalidate()
-
     # reference-surface no-ops / bookkeeping
     def fuse(self):
         return self  # BN is always folded when an engine is built (models/yolo.py:163-172)
 
     def eval(self):
-        if self.training and self._dev is not None:
-            self.sync_from_device()
-        self.training = False
-        return self
+        return self.train(False)
 
     def train(self, mode=True):
-        if not mode:
-            return self.eval()  # train(False) == eval(): pulls the trained masters back like eval() does
-        self.training = True
+        self.training = bool(mode)  # the weights a training phase changed reach inference through weights_version()
         return self
 
     def half(self):
@@ -305,10 +296,11 @@ class Model:
     def to(self, device):
         device = torch.device(device)
         if device != self.device:
-            if self._dev is not None:
+            if self._store is not None:
                 raise RuntimeError("Model.to(): device masters exist (an optimizer may hold them); build the model on its "
                                    "final device instead of moving it after parameters() / train()")
             self.device = device
+            self._host_ver += 1
             self._invalidate()
         return self
 
@@ -323,20 +315,31 @@ class Model:
         scale = gamma / torch.sqrt(var + eps)
         return w * scale.view(-1, 1, 1, 1), beta - mean * scale
 
+    def _folded(self, prefix):
+        """Host fp32 (weight, bias) of one conv as inference runs it: BN folded into the backbone convs, Detect heads as
+        they are.  ``params`` is read wherever it lives; the arithmetic is on the host."""
+        def host(leaf):
+            return self.params[prefix + leaf].detach().float().cpu()
+
+        if prefix + ".bn.weight" not in self.params:
+            return host(".weight"), host(".bias")
+        return self.fold_bn(host(".conv.weight"), host(".bn.weight"), host(".bn.bias"), host(".bn.running_mean"),
+                            host(".bn.running_var"))
+
     def packed(self):
+        """{conv prefix: (bf16 weight pack, fp32 bias)} of the current weights.  THE staleness check: when
+        ``weights_version()`` has moved since the packs were built, they, the FP8 calibration and the cached engines are
+        dropped (``_invalidate``) and the packs rebuilt from ``params``."""
+        if self.weights_version() != self._built:
+            self._invalidate()
         if self._packed is None:
-            P, out = self.params, {}
+            out = {}
             for idx, cs in enumerate(self.conv_specs):
-                w, b = self.fold_bn(P[cs.prefix + ".conv.weight"], P[cs.prefix + ".bn.weight"], P[cs.prefix + ".bn.bias"],
-                                    P[cs.prefix + ".bn.running_mean"], P[cs.prefix + ".bn.running_var"])
-                if idx == 0 and cs.c1 == 3:
-                    out[cs.prefix] = ops.pack_first_weight(w, b, self.device)
-                else:
-                    out[cs.prefix] = ops.pack_conv_weight(w, b, self.device)
+                pack = ops.pack_first_weight if idx == 0 and cs.c1 == 3 else ops.pack_conv_weight
+                out[cs.prefix] = pack(*self._folded(cs.prefix), self.device)
             d = self.detect
             for j in range(d.nl):
-                out[f"model.{d.i}.m.{j}"] = ops.pack_conv_weight(P[f"model.{d.i}.m.{j}.weight"], P[f"model.{d.i}.m.{j}.bias"],
-                                                                 self.device)
+                out[f"model.{d.i}.m.{j}"] = ops.pack_conv_weight(*self._folded(f"model.{d.i}.m.{j}"), self.device)
             self._packed = out
         return self._packed
 
@@ -346,15 +349,13 @@ class Model:
         W = self.packed()
         key = prefix + "#xpair"
         if key not in W:
-            P = self.params
-            w, b = self.fold_bn(P[prefix + ".conv.weight"], P[prefix + ".bn.weight"], P[prefix + ".bn.bias"],
-                                P[prefix + ".bn.running_mean"], P[prefix + ".bn.running_var"])
-            W[key] = ops.pack_conv_weight_xpair(w, b, self.device)
+            W[key] = ops.pack_conv_weight_xpair(*self._folded(prefix), self.device)
         return W[key]
 
     # ------------------------------------------------------------------------------------------------ forward
     def engine(self, n, h, w, in_dtype=torch.float32, in_div=0.0) -> "Engine":
         """The inference engine for one input shape at the model's ``precision`` (LRU-cached)."""
+        self.packed()  # weights changed since the cached engines were lowered: they are gone after this
         key = (n, h, w, in_dtype, float(in_div), self.precision)
         e = self._engines.get(key)
         if e is None:
@@ -416,9 +417,6 @@ class Engine:
         self.precision = model.precision if precision is None else precision
         if self.precision not in ("bf16", "fp8", "calib"):
             raise ValueError(f"unknown precision {self.precision!r}")
-        if self.precision == "fp8" and model._fp8_scales is None:
-            raise _lib.Y3Error("this model has no FP8 calibration (it was never calibrated, or load_state_dict / eval() "
-                               "after training / to() dropped it): run model.calibrate_fp8(batches) first")
         dev = model.device
         self.dry_run = dry_run
         if dry_run:
@@ -434,7 +432,10 @@ class Engine:
         # the TMA descriptors built below hold raw device addresses of these tensors: the engine owns a reference, and
         # remembers which weight version it was lowered from (run()/replay() refuse to use stale weights)
         self._weights = W
-        self.wver = model._wver
+        self.wver = model.weights_version()
+        if self.precision == "fp8" and model._fp8_scales is None:
+            raise _lib.Y3Error("this model has no FP8 calibration (it was never calibrated, or load_state_dict / eval() "
+                               "after training / to() dropped it): run model.calibrate_fp8(batches) first")
         det = model.detect
         self.static_in = torch.zeros(n, model.ch, h, w, dtype=in_dtype, device=dev)
 
@@ -651,13 +652,13 @@ class Engine:
         return g
 
     def _check_fresh(self):
-        if self.wver != self.model._wver:
+        if self.stale:
             raise _lib.Y3Error("this Engine was lowered from weights that have since changed (load_state_dict / training "
                                "/ to()): fetch a new one with model.engine(...)")
 
     @property
     def stale(self) -> bool:
-        return self.wver != self.model._wver
+        return self.wver != self.model.weights_version()
 
     def replay(self):
         self._check_fresh()

@@ -10,8 +10,8 @@ find what they expect behind ``Model(cfg)`` (VERDICT r1 missing #8; SURVEY §8b)
 * ``half()`` rounds the masters to fp16-representable values and makes inference return fp16 like the reference's half model
   (val.py:284,358; train.py:317 ``model.half().float()`` relies on exactly that rounding), ``float()`` returns to fp32 outputs;
 * ``forward`` runs the sm_90a engines: eval -> ``(z, [p3, p4, p5])`` (or ``(z_aug, None)`` with ``augment=True``), train -> raw maps
-  connected to autograd.  Weights changed in place by anyone (optimizer, EMA update, load_state_dict) are picked up lazily
-  through the store's version counter.
+  connected to autograd.  Weights changed in place by anyone (optimizer, EMA update, load_state_dict, a train-mode forward's
+  BatchNorm statistics) are picked up lazily through ``Model.weights_version()``.
 The modules' own ``forward`` methods are never called: all compute is in the C-ABI library."""
 from __future__ import annotations
 
@@ -125,9 +125,6 @@ class DetectionModel(nn.Module):
         for m_ in self.model:
             m_.np = sum(x.numel() for x in m_.parameters())
         self._out_dtype = torch.float32
-        self._synced = store.version()
-        core.sync_from_device()  # host copies == store (the store was initialised from them; establishes the invariant)
-        self._synced = store.version()
 
     # ------------------------------------------------------------------------------------------------ reference surface
     @property
@@ -142,20 +139,12 @@ class DetectionModel(nn.Module):
         if self.training:
             core.training = True
             return core.forward(x)
-        self._refresh()
         core.training = False
         y = core.forward(x, augment=augment, profile=profile, visualize=visualize)
         if self._out_dtype != torch.float32:
             y = tuple(t.to(self._out_dtype) if isinstance(t, torch.Tensor) else (None if t is None else [u.to(self._out_dtype) for u in t])
                       for t in y)
         return y
-
-    def _refresh(self):
-        """Inference reads packed bf16 weights folded from the host copies: refresh them when the masters changed in place."""
-        st = self.core.store()
-        if st.version() != self._synced:
-            self.core.sync_from_device()
-            self._synced = st.version()
 
     def train(self, mode: bool = True):
         super().train(mode)

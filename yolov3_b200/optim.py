@@ -94,7 +94,7 @@ class SGD:
                        "y3_grad_sumsq")
         _lib.check(L.y3_sgd_step(s.P.data_ptr(), s.G.data_ptr(), self.M.data_ptr(), ema_ptr, s.group.data_ptr(), s.n_total,
                                  self._hp.data_ptr(), self.grad_sumsq.data_ptr(), st), "y3_sgd_step")
-        s.kernel_writes += 1
+        s.mark_written()
 
     def grad_norm(self) -> torch.Tensor:
         """total gradient norm seen by the last step's clipping (before the 1/world_size average when DDP left sums)."""
@@ -139,7 +139,7 @@ class ModelEMA:
     def state_dict(self):
         s = self.store
         return {name: torch.as_strided(self.E, sl.shape, sl.stride, sl.offset).detach().float().cpu().contiguous().clone()
-                for name, sl in ((n, s.slots[n]) for n in self.model.params)}
+                for name, sl in ((n, s.slots[n]) for n in s.views)}
 
     @property
     def ema(self):

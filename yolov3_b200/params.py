@@ -111,11 +111,17 @@ class ParamStore:
             if trainable:
                 self.grads[name] = torch.as_strided(self.G, s.shape, s.stride, s.offset)
         self.grads_live = False  # True: G holds gradients of earlier backward passes that the next one must add to
-        self.kernel_writes = 0   # bumped by our own kernels that write P (torch's in-place ops bump P._version themselves)
+        self._torch_writes0 = self.P._version  # the initialising copies above are not changes
+        self._marked = 0
 
     def version(self):
-        """Changes whenever any parameter / buffer value may have changed (torch in-place op on a view, or a fused kernel)."""
-        return (self.P._version, self.kernel_writes)
+        """Changes whenever any parameter / buffer value may have changed since the store was initialised: a torch in-place
+        op on ``P`` or a view (torch counts those itself) or one of our kernels (``mark_written``)."""
+        return (self.P._version - self._torch_writes0, self._marked)
+
+    def mark_written(self):
+        """Every launch sequence of ours that writes ``P`` reports it here: torch does not see kernel writes."""
+        self._marked += 1
 
     # ------------------------------------------------------------------------------------------------ raw slot views
     def weight_rows_bf16(self, name) -> torch.Tensor:

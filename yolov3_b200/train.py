@@ -273,6 +273,7 @@ class TrainEngine:
     # ------------------------------------------------------------------------------------------------ forward
     def forward(self, x: torch.Tensor, in_div=0.0):
         self.fwd_gen += 1
+        self.store.mark_written()  # bn_finalize updates the running statistics inside P
         if not self.use_graphs:
             return self._forward_impl(x, in_div)
         st = self._graphs.setdefault("fwd", {"n": 0})
