@@ -40,7 +40,7 @@ int y3_device_check(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror definitions:
  * 0 y3_conv_desc, 1 y3_first_desc, 2 y3_pool_desc, 3 y3_detect_level, 4 y3_decode_desc, 5 y3_op, 6 y3_nms_params,
  * 7 y3_loss_desc, 8 y3_bn_act_desc, 9 y3_bn_bwd_desc, 10 y3_wgrad_desc, 11 y3_pack_item, 12 y3_letterbox_desc,
- * 13 y3_amax_desc, 14 y3_resize_item, 15 y3_augment_desc. */
+ * 13 y3_amax_desc, 14 y3_resize_item, 15 y3_augment_desc, 16 y3_jpeg_geom, 17 y3_jpeg_info, 18 y3_jpeg_desc. */
 int64_t y3_abi_sizeof(int32_t which);
 /* Programmatic dependent launch between consecutive kernels of a stream (on by default; env Y3_PDL=0 or on=0 turns it off).
  * Results are identical either way — only the launch boundaries overlap.  Returns the previous setting.  A tuning switch with
@@ -417,6 +417,58 @@ int y3_resize_area_u8_batched(const y3_resize_item* items, const y3_resize_item*
                               y3_stream_t stream);
 int y3_letterbox_u8_batched(const y3_letterbox_desc* descs, const y3_letterbox_desc* host_descs, int32_t n,
                             y3_stream_t stream);
+
+/* ---------------------------------------------------------------------------------------------------------------
+ * Baseline JPEG decode on the device, bit for bit cv2.imread / cv2.imdecode(IMREAD_COLOR) (libjpeg-turbo with its defaults:
+ * accurate integer IDCT, fancy upsampling; EXIF orientation applied) — csrc/y3_jpeg.cu, csrc/y3_jpeg.cuh.
+ *
+ * y3_jpeg_parse (HOST code, no CUDA call): reads the markers of one file.  info->eligible = 1 when the device decodes it:
+ *   SOF0 / SOF1 with 8-bit samples, Huffman coded, one interleaved scan of every component, 1 component or 3 in YCbCr, luma
+ *   sampling 1x1, 2x1, 2x2, 1x2 or 4x1 with chroma 1x1, any DRI / APPn / COM, EXIF orientation 1-8.  Anything else, and a
+ *   truncated or malformed file, gives eligible = 0 (decode it on the host).  Fills the geometry, the table blob (laid out for
+ *   the device) and up to seg_cap (start, length) pairs of the restart segments in UNSTUFFED bytes; geom.n_segs is set even
+ *   when it exceeds seg_cap (call again with room).  Returns Y3_OK, or Y3_ERR_BAD_ARG on a null argument.
+ * y3_jpeg_workspace_bytes: device scratch one image needs (unstuffed bytes, decoder state, coefficients, component planes).
+ * y3_jpeg_decode_batched: decodes n images in four launches on `stream`, each into its dst (uint8 HWC BGR [height, width, 3]
+ *   as oriented, row pitch dst_pitch).  descs in DEVICE memory, the same array in HOST memory (validation, grid size).  Each
+ *   desc's ws must lie inside [workspace, workspace + ws_bytes).  err_flags (device int32 [n]) gets 1 for an image whose
+ *   entropy-coded data is corrupt (invalid code, run past 63, data ending inside a segment, wrong block count): decode that
+ *   image on the host.  No allocation, no synchronisation, graph-capturable. */
+#define Y3_JPEG_TABLE_BYTES 6080
+typedef struct y3_jpeg_geom {
+  int32_t src_h, src_w;             /* as coded */
+  int32_t height, width;            /* as returned: swapped by EXIF orientations 5-8 */
+  int32_t orientation;              /* EXIF 1-8 */
+  int32_t ncomp;                    /* 1 or 3 */
+  int32_t hmax, vmax;               /* luma sampling factors (1, 1 for one component) */
+  int32_t mcus_x, mcus_y, blocks_per_mcu, n_blocks;
+  int32_t restart_interval;         /* MCUs per restart segment, 0: one segment */
+  int32_t n_segs;
+  int32_t data_len;                 /* entropy-coded bytes in the file, RST markers included */
+  int32_t unstuffed_len;            /* the same without byte stuffing and markers */
+  int32_t comp_dc[3], comp_ac[3];   /* Huffman table ids (0 / 1) per component */
+} y3_jpeg_geom;
+typedef struct y3_jpeg_info {
+  int32_t eligible;
+  int32_t reserved;
+  int64_t data_off;                 /* offset of the entropy-coded data in the file */
+  y3_jpeg_geom geom;
+  uint8_t tables[Y3_JPEG_TABLE_BYTES]; /* quantisation (natural order, per component) and Huffman lookup tables */
+} y3_jpeg_info;
+typedef struct y3_jpeg_desc {
+  y3_jpeg_geom geom;
+  const void* data;                 /* geom.data_len entropy-coded bytes */
+  const void* tables;               /* Y3_JPEG_TABLE_BYTES, 8-byte aligned */
+  const void* segs;                 /* int32 [n_segs][2] */
+  void* ws;                         /* y3_jpeg_workspace_bytes(&geom) bytes, 256-byte aligned */
+  void* dst;
+  int32_t dst_pitch;
+  int32_t reserved;
+} y3_jpeg_desc;
+int y3_jpeg_parse(const uint8_t* buf, int64_t len, y3_jpeg_info* info, int32_t* segs, int32_t seg_cap);
+int64_t y3_jpeg_workspace_bytes(const y3_jpeg_geom* geom);
+int y3_jpeg_decode_batched(const y3_jpeg_desc* descs, const y3_jpeg_desc* host_descs, int32_t n, void* workspace,
+                           int64_t ws_bytes, int32_t* err_flags, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Test-time augmentation (Model._forward_augment, models/yolo.py:239-280).

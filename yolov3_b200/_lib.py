@@ -202,6 +202,31 @@ class PackItem(C.Structure):
                 ("dst_co", C.c_int32), ("tile_begin", C.c_int32), ("reserved", C.c_int32)]
 
 
+JPEG_TABLE_BYTES = 6080
+
+
+class JpegGeom(C.Structure):
+    """struct y3_jpeg_geom."""
+
+    _fields_ = [(k, C.c_int32) for k in ("src_h", "src_w", "height", "width", "orientation", "ncomp", "hmax", "vmax",
+                                         "mcus_x", "mcus_y", "blocks_per_mcu", "n_blocks", "restart_interval", "n_segs",
+                                         "data_len", "unstuffed_len")] + [("comp_dc", C.c_int32 * 3), ("comp_ac", C.c_int32 * 3)]
+
+
+class JpegInfo(C.Structure):
+    """struct y3_jpeg_info."""
+
+    _fields_ = [("eligible", C.c_int32), ("reserved", C.c_int32), ("data_off", C.c_int64), ("geom", JpegGeom),
+                ("tables", C.c_uint8 * JPEG_TABLE_BYTES)]
+
+
+class JpegDesc(C.Structure):
+    """struct y3_jpeg_desc."""
+
+    _fields_ = [("geom", JpegGeom), ("data", C.c_void_p), ("tables", C.c_void_p), ("segs", C.c_void_p), ("ws", C.c_void_p),
+                ("dst", C.c_void_p), ("dst_pitch", C.c_int32), ("reserved", C.c_int32)]
+
+
 def _declare(lib):
     i32, vp, sz = C.c_int32, C.c_void_p, C.c_size_t
     sigs = {
@@ -264,6 +289,9 @@ def _declare(lib):
         "y3_nms_default_capacity": ([i32, i32, i32], i32),
         "y3_nms_workspace_bytes": ([i32, i32], C.c_int64),
         "y3_nms_batched": ([vp, C.POINTER(NmsParams), vp, C.c_int64, vp, vp, vp, vp, vp], C.c_int),
+        "y3_jpeg_parse": ([vp, C.c_int64, C.POINTER(JpegInfo), vp, i32], C.c_int),
+        "y3_jpeg_workspace_bytes": ([C.POINTER(JpegGeom)], C.c_int64),
+        "y3_jpeg_decode_batched": ([vp, vp, i32, vp, C.c_int64, vp, vp], C.c_int),
     }
     for name, (argtypes, restype) in sigs.items():
         fn = getattr(lib, name)
@@ -287,7 +315,7 @@ def lib():
         SYMBOLS.update(_declare(_lib))
         for which, st in enumerate((ConvDesc, FirstDesc, PoolDesc, DetectLevel, DecodeDesc, Op, NmsParams, LossDesc, BnActDesc,
                                     BnBwdDesc, WgradDesc, PackItem, LetterboxDesc, AmaxDesc, ResizeItem,
-                                    AugmentDesc)):
+                                    AugmentDesc, JpegGeom, JpegInfo, JpegDesc)):
             if _lib.y3_abi_sizeof(which) != C.sizeof(st):
                 raise Y3Error(f"ABI mismatch: sizeof({st.__name__}) is {C.sizeof(st)} here, "
                               f"{_lib.y3_abi_sizeof(which)} in {_LIB_PATH.name}; rebuild the library")

@@ -24,7 +24,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, jpeg
 from .preprocess import letterbox_geometry
 
 BORDER = 114
@@ -307,6 +307,14 @@ def read_source(dataset, i):
     src = getattr(dataset, "sources", None)
     if src is not None:
         return src[i]
+    js = jpeg.read(dataset.im_files[i])  # a JPEG the device decodes: its bytes, decoded into the source's slot
+    if js is not None:
+        return js
+    return host_read(dataset, i)
+
+
+def host_read(dataset, i):
+    """cv2.imread of source i: uint8 HWC BGR."""
     import cv2
 
     im = cv2.imread(dataset.im_files[i])
@@ -360,7 +368,8 @@ def pack_batch(plans, images, dbase, host):
         return dbase + raw_off[key[0]], images[key[0]].shape[1] * 3
 
     for i, im in images.items():
-        host[raw_off[i]: raw_off[i] + im.nbytes] = im.reshape(-1)
+        if not isinstance(im, jpeg.JpegSource):  # a JPEG source's slot is written by the device decode
+            host[raw_off[i]: raw_off[i] + im.nbytes] = im.reshape(-1)
     items = (_lib.ResizeItem * max(1, len(keys1) + len(keys2)))()
     for j, k in enumerate(keys1):
         im = images[k[0]]
@@ -402,6 +411,11 @@ class _Slot:
         self.copied = None  # event: the H2D copy out of `host` has completed
         self.free = None  # event: the consumer has finished with this slot's output images
         self.out = None
+        self.ws = None  # device workspace of the JPEG decode
+        self.err = None  # device int32 per-image corruption flags of the JPEG decode ...
+        self.err_host = None  # ... copied to pinned memory behind `decoded`
+        self.decoded = None
+        self.jpeg_keys = []  # dataset indices of the batch's device-decoded sources, in desc order
 
 
 def _collate_targets(labels):
@@ -427,6 +441,8 @@ class _BatchLoader:
         self.stream = torch.cuda.Stream(device=self.device)
         self._slots = [_Slot(), _Slot()]
         self._k = 0
+        self.jpeg_decoded = []  # sources of the last batch decoded on the device (dataset indices) ...
+        self.jpeg_fallbacks = []  # ... and those of them whose data the device found corrupt (read again by cv2)
 
     def __len__(self):
         n = len(self.sampler)
@@ -454,15 +470,43 @@ class _BatchLoader:
     def launch(self, prepared, out=None, slot=None):
         """Device half of one batch: one H2D copy (sources + descriptors) and the batch's launches on the loader's stream,
         writing into ``out`` (a uint8 CUDA [bs, 3, H, W] tensor, e.g. an engine input) or a loader-owned buffer.  The
-        current stream waits for the result; nothing synchronises the host."""
+        current stream waits for the result.  Without device-decoded JPEG sources nothing synchronises the host; with them,
+        the host waits for the decode's corruption flags (see ``jpeg_decoded`` / ``jpeg_fallbacks``)."""
         plans, labels, reads = prepared
-        images = {i: np.ascontiguousarray(f.result()) for i, f in reads.items()}
-        return self._launch(plans, labels, images, out, slot)
-
-    def _device_batch(self, bs, H, W, total, fill, run, out, slot):
-        """Stage `total` bytes through slot `slot`: ``fill(dbase, host_u8, out)`` packs the pinned buffer as the device will see
-        it at dbase and returns a layout; the copy and ``run(layout, dbase, out, stream_handle)`` go to the side stream."""
+        images = {}
+        for i, f in reads.items():
+            im = f.result()
+            if isinstance(im, jpeg.JpegSource) and im.shape[:2] != _hw0(self.dataset, i):
+                # the plan's shape (e.g. the reference's exif_size, which swaps only for EXIF orientations 6 and 8)
+                # differs from the decoded one: cv2.imread as before
+                im = host_read(self.dataset, i)
+            images[i] = im if isinstance(im, jpeg.JpegSource) else np.ascontiguousarray(im)
+        result = self._launch(plans, labels, images, out, slot)
         sl = self._slots[slot if slot is not None else 0]
+        self.jpeg_decoded = [i for i, im in images.items() if isinstance(im, jpeg.JpegSource)]
+        self.jpeg_fallbacks = []
+        if self.jpeg_decoded:
+            # waits for this batch's copy and decode, which the side stream runs after the previous batch's launches;
+            # those waited for the consumer's work queued before the previous launch (one batch of slack, not two)
+            sl.decoded.synchronize()
+            self.jpeg_fallbacks = [sl.jpeg_keys[k] for k in np.flatnonzero(sl.err_host.numpy()[: len(sl.jpeg_keys)])]
+            if self.jpeg_fallbacks:  # corrupt entropy-coded data: those sources are read by cv2 and the batch runs again
+                for i in self.jpeg_fallbacks:
+                    images[i] = np.ascontiguousarray(host_read(self.dataset, i))
+                result = self._launch(plans, labels, images, out, slot)
+        return result
+
+    def _device_batch(self, bs, H, W, total, fill, run, out, slot, raw_off=None, images=None):
+        """Stage `total` bytes through slot `slot`: ``fill(dbase, host_u8, out)`` packs the pinned buffer as the device will see
+        it at dbase and returns a layout; the copy and ``run(layout, dbase, out, stream_handle)`` go to the side stream.
+        JPEG sources among `images` are staged behind, and decoded into their slots at ``dbase + raw_off[i]`` on the side
+        stream ahead of ``run``; their corruption flags reach ``slot.err_host`` behind ``slot.decoded``."""
+        sl = self._slots[slot if slot is not None else 0]
+        keys = [i for i, im in (images or {}).items() if isinstance(im, jpeg.JpegSource)]
+        srcs = [images[i] for i in keys]
+        jpeg_off = _up(total)
+        if srcs:
+            total = jpeg_off + jpeg.stage_bytes(srcs)
         if sl.copied is not None:
             sl.copied.synchronize()  # the previous copy out of this slot's staging buffer has completed
         if sl.host is None or sl.host.numel() < total:
@@ -481,11 +525,33 @@ class _BatchLoader:
         lay = fill(dbase, sl.host.numpy(), out)
         main = torch.cuda.current_stream(self.device)
         s = self.stream
+        if srcs:
+            wsb = jpeg.workspace_bytes(srcs)
+            with torch.cuda.stream(s):
+                if sl.ws is None or sl.ws.numel() < wsb:
+                    sl.ws = torch.empty(int(wsb * 1.25), dtype=torch.uint8, device=self.device)
+                if sl.err is None or sl.err.numel() < len(srcs):
+                    sl.err = torch.empty(max(64, 2 * len(srcs)), dtype=torch.int32, device=self.device)
+                    sl.err_host = torch.empty(sl.err.numel(), dtype=torch.int32, pin_memory=True)
+            packed = jpeg.pack(srcs, [dbase + raw_off[i] for i in keys], dbase + jpeg_off, sl.host.numpy()[jpeg_off:],
+                               sl.ws.data_ptr())
+            sl.jpeg_keys = keys
+            # the copy and the decode touch only this slot's buffers, which the consumer never reads: they run without
+            # waiting for the consumer's queued work, so the corruption flags are known early
+            with torch.cuda.stream(s):
+                sl.dev[:total].copy_(sl.host[:total], non_blocking=True)
+                sl.copied = torch.cuda.Event()
+                sl.copied.record(s)
+                jpeg.launch(packed, dbase + jpeg_off, sl.ws.data_ptr(), sl.ws.numel(), sl.err.data_ptr(), s.cuda_stream)
+                sl.err_host[: len(srcs)].copy_(sl.err[: len(srcs)], non_blocking=True)
+                sl.decoded = torch.cuda.Event()
+                sl.decoded.record(s)
         s.wait_stream(main)  # `out` / the slot's previous images are no longer read by the consumer's queued work
         with torch.cuda.stream(s):
-            sl.dev[:total].copy_(sl.host[:total], non_blocking=True)
-            sl.copied = torch.cuda.Event()
-            sl.copied.record(s)
+            if not srcs:
+                sl.dev[:total].copy_(sl.host[:total], non_blocking=True)
+                sl.copied = torch.cuda.Event()
+                sl.copied.record(s)
             run(lay, dbase, out, s.cuda_stream)
         main.wait_stream(s)
         out.record_stream(main)
@@ -548,6 +614,7 @@ class DeviceLoader(_BatchLoader):
                     _lib.check(L.y3_resize_u8_batched(dbase + off, n, mh, mw, hs), "y3_resize_u8_batched")
             _lib.check(L.y3_augment_u8(dbase + lay["desc_off"], len(plans), H, W, out.data_ptr(), hs), "y3_augment_u8")
 
-        out = self._device_batch(len(plans), H, W, batch_bytes(plans, images),
-                                 lambda dbase, host, _: pack_batch(plans, images, dbase, host), run, out, slot)
+        lay = _layout(plans, images)
+        out = self._device_batch(len(plans), H, W, lay[-1], lambda dbase, host, _: pack_batch(plans, images, dbase, host),
+                                 run, out, slot, raw_off=lay[0], images=images)
         return out, _collate_targets(labels), tuple(p.path for p in plans), tuple(p.shapes for p in plans)

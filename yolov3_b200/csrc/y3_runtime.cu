@@ -143,6 +143,9 @@ extern "C" int64_t y3_abi_sizeof(int32_t which) {
     case 13: return sizeof(y3_amax_desc);
     case 14: return sizeof(y3_resize_item);
     case 15: return sizeof(y3_augment_desc);
+    case 16: return sizeof(y3_jpeg_geom);
+    case 17: return sizeof(y3_jpeg_info);
+    case 18: return sizeof(y3_jpeg_desc);
   }
   return -1;
 }

@@ -16,7 +16,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import _lib
+from . import _lib, jpeg
 from .augment import BORDER, _BatchLoader, _collate_targets, _load_hw, _up, xywhn2xyxy, xyxy2xywhn
 from .preprocess import letterbox_geometry
 
@@ -97,7 +97,8 @@ def pack_val_batch(plans, images, dbase, host, out_ptr):
     raw_off, res_off, resized, items_off, desc_off, total = _val_layout(plans, images)
     assert host.nbytes >= total
     for i, im in images.items():
-        host[raw_off[i]: raw_off[i] + im.nbytes] = im.reshape(-1)
+        if not isinstance(im, jpeg.JpegSource):  # a JPEG source's slot is written by the device decode
+            host[raw_off[i]: raw_off[i] + im.nbytes] = im.reshape(-1)
     load_hw = {p.index: p.load_hw for p in plans}
     # load_image (utils/dataloaders.py:751-754): INTER_AREA when it shrinks (r < 1), INTER_LINEAR when it enlarges
     area = [i for i in resized if load_hw[i][0] <= images[i].shape[0] and load_hw[i][1] <= images[i].shape[1]]
@@ -170,7 +171,8 @@ class DeviceValLoader(_BatchLoader):
             off, descs = lay["desc"]
             _lib.check(L.y3_letterbox_u8_batched(dbase + off, C.addressof(descs), len(plans), hs), "y3_letterbox_u8_batched")
 
-        out = self._device_batch(len(plans), H, W, val_batch_bytes(plans, images),
+        lay = _val_layout(plans, images)
+        out = self._device_batch(len(plans), H, W, lay[-1],
                                  lambda dbase, host, o: pack_val_batch(plans, images, dbase, host, o.data_ptr()), run, out,
-                                 slot)
+                                 slot, raw_off=lay[0], images=images)
         return out, _collate_targets(labels), tuple(p.path for p in plans), tuple(p.shapes for p in plans)
