@@ -368,8 +368,9 @@ int y3_letterbox_u8(const y3_letterbox_desc* d, y3_stream_t stream);
  * synchronisation: both entry points are graph-capturable.  The descriptor arrays live in DEVICE memory.
  *
  * y3_resize_u8_batched: load_image's cv2.resize (INTER_LINEAR; dst = ceil(w0 r) x ceil(h0 r)) of every item in one launch,
- *   the rule of y3_letterbox_u8.  src / dst are uint8 HWC BGR [h, w, 3] with row pitches in bytes; max_h / max_w bound the
- *   items' dst sizes (the grid).
+ *   the rule of y3_letterbox_u8.  src / dst are uint8 HWC BGR [h, w, 3] with row pitches in bytes.  `items` is in DEVICE
+ *   memory and `host_items` the same array in HOST memory, from which every item is validated (non-null src / dst, positive
+ *   sizes, pitches of at least 3 w bytes; Y3_ERR_BAD_ARG before any launch otherwise) and the grid is sized.
  * y3_augment_u8: one output image per descriptor into out [n, 3, out_h, out_w] (uint8 CHW RGB: a TrainEngine input).  Per
  *   output pixel: the affine warp of cv2.warpAffine (INTER_LINEAR, border 114; inv = the inverted M as
  *   cv::invertAffineTransform computes it: A11, A12, b1, A21, A22, b2) of a VIRTUAL canvas — up to 4 placements of resized
@@ -381,7 +382,8 @@ typedef struct y3_resize_item {
   const void* src; int32_t src_h, src_w, src_pitch;
   void* dst;       int32_t dst_h, dst_w, dst_pitch;
 } y3_resize_item;
-int y3_resize_u8_batched(const y3_resize_item* items, int32_t n_items, int32_t max_h, int32_t max_w, y3_stream_t stream);
+int y3_resize_u8_batched(const y3_resize_item* items, const y3_resize_item* host_items, int32_t n_items,
+                         y3_stream_t stream);
 
 #define Y3_AUG_MAX_PLACE 4
 typedef struct y3_aug_place {

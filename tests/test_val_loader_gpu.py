@@ -1,6 +1,7 @@
-"""The validation pass on the device: the INTER_AREA kernel (y3_resize_area_u8_batched) against cv2, DeviceValLoader against
-the fixtures the reference's own __getitem__ with augment=False produced (tests/golden/make_val_loader_golden.py) and
-against the numpy restatement on bs-32 640² rect batches, and yolov3_b200.val.run against the reference's own val.run."""
+"""The validation pass on the device: the INTER_AREA and INTER_LINEAR batched resizes (y3_resize_area_u8_batched,
+y3_resize_u8_batched) against cv2 and the refusals of the resize and letterbox entry points, DeviceValLoader against the
+fixtures the reference's own __getitem__ with augment=False produced (tests/golden/make_val_loader_golden.py) and against the
+numpy restatement on bs-32 640² rect batches, and yolov3_b200.val.run against the reference's own val.run."""
 import ctypes as C
 import json
 import sys
@@ -22,8 +23,8 @@ GOLDEN = np.load(G / "val_loader_cases.npz")
 CASES = sorted({k.split("/")[0] for k in GOLDEN.files})
 
 
-def _area_device(pairs):
-    """Every (image, (new_h, new_w)) of `pairs` through ONE y3_resize_area_u8_batched launch."""
+def _resize_items(pairs):
+    """Device sources and outputs of (image, (new_h, new_w)) pairs, and their y3_resize_item array (host, device copy)."""
     from yolov3_b200 import _lib
 
     srcs = [torch.from_numpy(im).cuda() for im, _ in pairs]
@@ -33,8 +34,16 @@ def _area_device(pairs):
         items[j] = _lib.ResizeItem(s.data_ptr(), s.shape[0], s.shape[1], s.shape[1] * 3, d.data_ptr(), d.shape[0],
                                    d.shape[1], d.shape[1] * 3)
     dev_items = torch.frombuffer(bytearray(bytes(items)), dtype=torch.uint8).cuda()
-    _lib.check(_lib.lib().y3_resize_area_u8_batched(dev_items.data_ptr(), C.addressof(items), len(pairs),
-                                                    torch.cuda.current_stream().cuda_stream), "y3_resize_area_u8_batched")
+    return srcs, dsts, items, dev_items
+
+
+def _resize_device(pairs, entry="y3_resize_area_u8_batched"):
+    """Every (image, (new_h, new_w)) of `pairs` through ONE launch of a batched resize entry point."""
+    from yolov3_b200 import _lib
+
+    _, dsts, items, dev_items = _resize_items(pairs)
+    _lib.check(getattr(_lib.lib(), entry)(dev_items.data_ptr(), C.addressof(items), len(pairs),
+                                          torch.cuda.current_stream().cuda_stream), entry)
     torch.cuda.synchronize()
     return [d.cpu().numpy() for d in dsts]
 
@@ -42,7 +51,7 @@ def _area_device(pairs):
 def test_area_kernel_equals_cv2():
     sweep = V.area_sweep()
     pairs = [(A.seeded_image(h * 7 + w, h, w), (nh, nw)) for (h, w), (nh, nw) in sweep]
-    got = _area_device(pairs)
+    got = _resize_device(pairs)
     bad = [sweep[k] for k, ((im, (nh, nw)), g) in enumerate(zip(pairs, got))
            if not np.array_equal(g, cv2.resize(im, (nw, nh), interpolation=cv2.INTER_AREA))]
     assert not bad, f"area kernel differs from cv2 on {bad}"
@@ -52,7 +61,77 @@ def test_area_kernel_refuses_upscaling():
     from yolov3_b200 import _lib
 
     with pytest.raises(_lib.Y3Error, match="scales up"):
-        _area_device([(A.seeded_image(1, 40, 60), (40, 61))])
+        _resize_device([(A.seeded_image(1, 40, 60), (40, 61))])
+
+
+def test_linear_batched_resize_equals_cv2():
+    """Items of different sizes in one y3_resize_u8_batched launch, whose grid comes from the items: enlargements, shrinks,
+    an exact 2x shrink, an equal size, and the largest output neither first nor last."""
+    sweep = [((300, 200), (640, 427)), ((480, 640), (360, 480)), ((1080, 1920), (540, 960)), ((17, 23), (17, 23)),
+             ((375, 500), (1000, 1333)), ((640, 427), (641, 428)), ((1280, 960), (640, 480)), ((33, 700), (20, 1401))]
+    pairs = [(A.seeded_image(h * 11 + w, h, w), (nh, nw)) for (h, w), (nh, nw) in sweep]
+    got = _resize_device(pairs, "y3_resize_u8_batched")
+    bad = [sweep[k] for k, ((im, (nh, nw)), g) in enumerate(zip(pairs, got))
+           if not np.array_equal(g, cv2.resize(im, (nw, nh), interpolation=cv2.INTER_LINEAR))]
+    assert not bad, f"batched INTER_LINEAR differs from cv2 on {bad}"
+
+
+BAD_ITEMS = {"null src": lambda it: setattr(it, "src", None), "null dst": lambda it: setattr(it, "dst", None),
+             "zero dst_h": lambda it: setattr(it, "dst_h", 0), "zero src_w": lambda it: setattr(it, "src_w", 0),
+             "short src_pitch": lambda it: setattr(it, "src_pitch", it.src_w * 3 - 1),
+             "short dst_pitch": lambda it: setattr(it, "dst_pitch", it.dst_w * 3 - 1)}
+
+
+@pytest.mark.parametrize("entry", ["y3_resize_u8_batched", "y3_resize_area_u8_batched"])
+@pytest.mark.parametrize("bad", list(BAD_ITEMS))
+def test_batched_resize_refuses_a_bad_item(entry, bad):
+    """The host copy of the second item is broken; the device copy stays valid, so nothing could fault were it launched."""
+    from yolov3_b200 import _lib
+
+    _, _, items, dev_items = _resize_items([(A.seeded_image(1, 60, 80), (30, 40)), (A.seeded_image(2, 50, 70), (25, 35))])
+    BAD_ITEMS[bad](items[1])
+    rc = getattr(_lib.lib(), entry)(dev_items.data_ptr(), C.addressof(items), 2, torch.cuda.current_stream().cuda_stream)
+    assert rc == -1 and "item 1" in _lib.last_error()  # Y3_ERR_BAD_ARG
+
+
+def _letterbox_descs(n):
+    """n valid y3_letterbox_descs (a 60x80 source letterboxed into a 64x64 CHW output each) and their buffers."""
+    from yolov3_b200 import _lib
+
+    src = torch.from_numpy(A.seeded_image(3, 60, 80)).cuda()
+    out = torch.empty(n, 3, 64, 64, dtype=torch.uint8, device="cuda")
+    descs = (_lib.LetterboxDesc * n)()
+    for b in range(n):
+        d = descs[b]
+        d.src, d.src_h, d.src_w, d.src_pitch = src.data_ptr(), 60, 80, 240
+        d.new_h, d.new_w, d.top, d.left = 48, 64, 8, 0
+        d.dst, d.out_h, d.out_w, d.out_chw, d.swap_rb = out[b].data_ptr(), 64, 64, 1, 1
+        for c in range(3):
+            d.pad[c] = 114
+    return src, out, descs
+
+
+BAD_DESCS = {"null src": lambda d: setattr(d, "src", None), "null dst": lambda d: setattr(d, "dst", None),
+             "zero new_w": lambda d: setattr(d, "new_w", 0), "zero src_h": lambda d: setattr(d, "src_h", 0),
+             "short src_pitch": lambda d: setattr(d, "src_pitch", 239)}
+
+
+@pytest.mark.parametrize("bad", list(BAD_DESCS))
+def test_letterbox_refuses_a_bad_descriptor(bad):
+    """y3_letterbox_u8 and y3_letterbox_u8_batched refuse the same descriptors (for the batched entry the device copy
+    stays valid, so nothing could fault were it launched); the valid ones run."""
+    from yolov3_b200 import _lib
+
+    L, hs = _lib.lib(), torch.cuda.current_stream().cuda_stream
+    src, out, descs = _letterbox_descs(2)
+    dev_descs = torch.frombuffer(bytearray(bytes(descs)), dtype=torch.uint8).cuda()
+    _lib.check(L.y3_letterbox_u8(C.byref(descs[0]), hs), "y3_letterbox_u8")
+    _lib.check(L.y3_letterbox_u8_batched(dev_descs.data_ptr(), C.addressof(descs), 2, hs), "y3_letterbox_u8_batched")
+    torch.cuda.synchronize()
+    BAD_DESCS[bad](descs[1])
+    assert L.y3_letterbox_u8(C.byref(descs[1]), hs) == -1  # Y3_ERR_BAD_ARG
+    assert L.y3_letterbox_u8_batched(dev_descs.data_ptr(), C.addressof(descs), 2, hs) == -1
+    assert "item 1" in _lib.last_error()
 
 
 def spec(case):

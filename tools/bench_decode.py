@@ -54,25 +54,18 @@ def kernel_time(bufs, reps):
     srcs = [jpeg.parse(b) for b in bufs]
     assert all(s is not None for s in srcs)
     outs = [torch.empty(*s.shape, dtype=torch.uint8, device="cuda") for s in srcs]
-    nb = jpeg.stage_bytes(srcs)
-    host = torch.empty(nb, dtype=torch.uint8, pin_memory=True)
-    dev = torch.empty(nb, dtype=torch.uint8, device="cuda")
-    wsb = jpeg.workspace_bytes(srcs)
-    ws = torch.empty(wsb, dtype=torch.uint8, device="cuda")
-    err = torch.empty(len(srcs), dtype=torch.int32, device="cuda")
-    packed = jpeg.pack(srcs, [o.data_ptr() for o in outs], dev.data_ptr(), host.numpy(), ws.data_ptr())
-    dev.copy_(host)
+    batch = jpeg.stage(srcs, [o.data_ptr() for o in outs], "cuda")
     s = torch.cuda.current_stream()
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(2)]
     times = []
     for k in range(reps + 3):
         ev[0].record(s)
-        jpeg.launch(packed, dev.data_ptr(), ws.data_ptr(), wsb, err.data_ptr(), s.cuda_stream)
+        batch.launch(s.cuda_stream)
         ev[1].record(s)
         ev[1].synchronize()
         if k >= 3:
             times.append(ev[0].elapsed_time(ev[1]))
-    assert not err.cpu().numpy().any(), "a clean source was flagged"
+    assert not batch.err.cpu().numpy().any(), "a clean source was flagged"
     ms = float(np.median(times))
     return {"ms_per_batch": round(ms, 3), "img_per_s": round(len(bufs) / ms * 1e3, 1)}
 

@@ -227,6 +227,21 @@ class JpegDesc(C.Structure):
                 ("dst", C.c_void_p), ("dst_pitch", C.c_int32), ("reserved", C.c_int32)]
 
 
+class Regions:
+    """Lays out a staging buffer the kernels read: each ``take(nbytes)`` returns the offset of the next region, 256-byte
+    aligned (the alignment every pointer handed to a kernel gets); ``size`` is the bytes taken so far."""
+
+    ALIGN = 256
+
+    def __init__(self):
+        self.size = 0
+
+    def take(self, nbytes):
+        off = self.size
+        self.size += (int(nbytes) + self.ALIGN - 1) // self.ALIGN * self.ALIGN
+        return off
+
+
 def _declare(lib):
     i32, vp, sz = C.c_int32, C.c_void_p, C.c_size_t
     sigs = {
@@ -253,7 +268,7 @@ def _declare(lib):
         "y3_pack_dgrad_batched": ([vp, i32, vp, i32, vp], C.c_int),
         "y3_head_grad_pack": ([vp, i32, i32, i32, i32, i32, vp, i32, i32, vp, vp], C.c_int),
         "y3_letterbox_u8": ([C.POINTER(LetterboxDesc), vp], C.c_int),
-        "y3_resize_u8_batched": ([vp, i32, i32, i32, vp], C.c_int),
+        "y3_resize_u8_batched": ([vp, vp, i32, vp], C.c_int),
         "y3_augment_u8": ([vp, i32, i32, i32, vp, vp], C.c_int),
         "y3_resize_area_u8_batched": ([vp, vp, i32, vp], C.c_int),
         "y3_letterbox_u8_batched": ([vp, vp, i32, vp], C.c_int),

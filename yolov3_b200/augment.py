@@ -5,30 +5,30 @@ bit-exact with OpenCV's 8-bit arithmetic (csrc/y3_augment.cu).
 ``plan_item(dataset, index)`` restates ``__getitem__``'s control flow on the host: it consumes Python's ``random`` and
 ``np.random`` exactly as the reference does and computes the final labels with the reference's numpy operations, but
 instead of images it returns a plan: which resized sources sit where on the (virtual) mosaic / letterbox canvas, the affine
-M, the MixUp ratio, the HSV LUTs and the flips.  ``DeviceLoader`` reads the sources of a batch on a thread pool, copies them
-to the device in one transfer and runs two launches — ``y3_resize_u8_batched`` (load_image's cv2.resize of every source) and
-``y3_augment_u8`` (everything else, written as uint8 CHW RGB into the ``[bs, 3, H, W]`` batch).
+M, the MixUp ratio, the HSV LUTs and the flips.  ``letterbox_item`` and ``labels_out`` state the letterboxed item and the
+labels' tail of ``__getitem__`` once for both planners (``yolov3_b200.valloader.plan_val_item`` is the other).
+``DeviceLoader`` (on ``yolov3_b200.loader.BatchLoader``: reads, staging, JPEG decode) packs a batch's y3_resize_item and
+y3_augment_desc arrays and runs two launches — ``y3_resize_u8_batched`` (load_image's cv2.resize of every source, then
+letterbox's second resize) and ``y3_augment_u8`` (everything else, written as uint8 CHW RGB into the ``[bs, 3, H, W]``
+batch).
 
 Refused when the loader is built (NotImplementedError): ``perspective > 0`` (warpPerspective), segment (polygon) labels,
-an active Albumentations transform, and ``augment=False`` (served by ``yolov3_b200.valloader.DeviceValLoader``, which shares
-this module's batch machinery)."""
+an active Albumentations transform, and ``augment=False`` (served by ``yolov3_b200.valloader.DeviceValLoader``)."""
 from __future__ import annotations
 
 import ctypes as C
 import math
 import random
-from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass, field
-from pathlib import Path
 
 import numpy as np
-import torch
 
-from . import _lib, jpeg
+from . import _lib
+from .loader import BatchLoader, load_hw
+from .loader import host_read, read_source  # noqa: F401  load_image's read, still part of this module's interface
 from .preprocess import letterbox_geometry
 
 BORDER = 114
-_ALIGN = 256
 
 
 # ------------------------------------------------------------------------------------------ label arithmetic (restated)
@@ -139,31 +139,6 @@ def check_supported(dataset):
         raise NotImplementedError("an active Albumentations transform is not built")
 
 
-def _hw0(dataset, i):
-    """Shape of source i as load_image reads it, without reading it: the RAM cache's, an .npy header's, else the (w, h)
-    the dataset recorded when it verified the image."""
-    ims = getattr(dataset, "ims", None)
-    if ims is not None and ims[i] is not None:
-        return tuple(dataset.im_hw0[i])
-    npy = getattr(dataset, "npy_files", None)
-    if npy is not None and Path(npy[i]).exists():
-        return tuple(np.load(npy[i], mmap_mode="r").shape[:2])
-    w, h = dataset.shapes[i]
-    return int(h), int(w)
-
-
-def _load_hw(dataset, i):
-    """((h0, w0), (h, w)) of load_image(i) (utils/dataloaders.py:737-756)."""
-    ims = getattr(dataset, "ims", None)
-    if ims is not None and ims[i] is not None:
-        return tuple(dataset.im_hw0[i]), tuple(dataset.im_hw[i])
-    h0, w0 = _hw0(dataset, i)
-    r = dataset.img_size / max(h0, w0)
-    if r != 1:
-        return (h0, w0), (math.ceil(h0 * r), math.ceil(w0 * r))
-    return (h0, w0), (h0, w0)
-
-
 def _random_perspective(height0, width0, targets, degrees, translate, scale, shear, perspective, border=(0, 0)):
     """random_perspective (utils/augmentations.py:137-216) for an im of height0 x width0 and box targets: (M, targets)."""
     height = height0 + border[0] * 2
@@ -225,7 +200,7 @@ def _plan_mosaic(dataset, index):
     indices = [index, *random.choices(dataset.indices, k=3)]
     random.shuffle(indices)
     for i, mosaic_index in enumerate(indices):
-        _, (h, w) = _load_hw(dataset, mosaic_index)
+        _, (h, w) = load_hw(dataset, mosaic_index)
         x1a, y1a, x2a, y2a, x1b, y1b = _mosaic_rects(i, xc, yc, w, h, s)
         padw, padh = x1a - x1b, y1a - y1b
         if x2a > x1a and y2a > y1a:
@@ -240,6 +215,37 @@ def _plan_mosaic(dataset, index):
     M, labels4 = _random_perspective(2 * s, 2 * s, labels4, hyp["degrees"], hyp["translate"], hyp["scale"], hyp["shear"],
                                      hyp["perspective"], border=dataset.mosaic_border)
     return Canvas(places, M), labels4
+
+
+def letterbox_item(dataset, index, scaleup):
+    """The item of __getitem__ without mosaic (utils/dataloaders.py:676-686) before any random draw: load_image's size
+    (h, w), letterbox into the (rect) batch shape — (new_unpad (w, h), top, left, out_hw) — the ``shapes`` entry and the
+    labels in output pixels (xyxy)."""
+    (h0, w0), (h, w) = load_hw(dataset, index)
+    shape = dataset.batch_shapes[dataset.batch[index]] if dataset.rect else dataset.img_size
+    new_unpad, ratio, pad, top, bottom, left, right = letterbox_geometry((h, w), shape, auto=False, scaleup=scaleup)
+    out_hw = (new_unpad[1] + top + bottom, new_unpad[0] + left + right)
+    shapes = (h0, w0), ((h / h0, w / w0), pad)
+    labels = dataset.labels[index].copy()
+    if labels.size:
+        labels[:, 1:] = xywhn2xyxy(labels[:, 1:], ratio[0] * w, ratio[1] * h, padw=pad[0], padh=pad[1])
+    return (h, w), new_unpad, top, left, out_hw, shapes, labels
+
+
+def labels_out(labels, out_hw, flipud=False, fliplr=False):
+    """The tail of __getitem__ (utils/dataloaders.py:703-735) for pixel xyxy `labels` of an out_hw image: normalised xywh
+    clipped to the image, the flips, and labels_out float32 [nl, 6] with column 0 zero."""
+    nl = len(labels)
+    if nl:
+        labels[:, 1:5] = xyxy2xywhn(labels[:, 1:5], w=out_hw[1], h=out_hw[0], clip=True, eps=1e-3)
+        if flipud:
+            labels[:, 2] = 1 - labels[:, 2]
+        if fliplr:
+            labels[:, 1] = 1 - labels[:, 1]
+    out = np.zeros((nl, 6), dtype=np.float32)
+    if nl:
+        out[:, 1:] = labels
+    return out
 
 
 def plan_item(dataset, index):
@@ -259,332 +265,26 @@ def plan_item(dataset, index):
             canvases.append(canvas2)
         out_hw = (2 * s + 2 * dataset.mosaic_border[0], 2 * s + 2 * dataset.mosaic_border[1])
     else:
-        (h0, w0), (h, w) = _load_hw(dataset, index)
-        shape = dataset.batch_shapes[dataset.batch[index]] if dataset.rect else dataset.img_size
-        new_unpad, ratio, pad, top, bottom, left, right = letterbox_geometry((h, w), shape, auto=False, scaleup=dataset.augment)
+        (h, w), new_unpad, top, left, out_hw, shapes, labels = letterbox_item(dataset, index, scaleup=dataset.augment)
         key = (index, h, w) if (w, h) == tuple(new_unpad) else (index, h, w, new_unpad[1], new_unpad[0])
-        hh, ww = new_unpad[1] + top + bottom, new_unpad[0] + left + right
-        shapes = (h0, w0), ((h / h0, w / w0), pad)
-        labels = dataset.labels[index].copy()
-        if labels.size:
-            labels[:, 1:] = xywhn2xyxy(labels[:, 1:], ratio[0] * w, ratio[1] * h, padw=pad[0], padh=pad[1])
-        M, labels = _random_perspective(hh, ww, labels, hyp["degrees"], hyp["translate"], hyp["scale"], hyp["shear"],
+        M, labels = _random_perspective(*out_hw, labels, hyp["degrees"], hyp["translate"], hyp["scale"], hyp["shear"],
                                         hyp["perspective"])
         canvases = [Canvas([(key, left, top, left + new_unpad[0], top + new_unpad[1], left, top)], M)]
-        mix_r, out_hw = 0.0, (hh, ww)
-    nl = len(labels)
-    if nl:
-        labels[:, 1:5] = xyxy2xywhn(labels[:, 1:5], w=out_hw[1], h=out_hw[0], clip=True, eps=1e-3)
+        mix_r = 0.0
     luts = None
     hgain, sgain, vgain = hyp["hsv_h"], hyp["hsv_s"], hyp["hsv_v"]
     if hgain or sgain or vgain:
         luts = hsv_luts(np.random.uniform(-1, 1, 3) * [hgain, sgain, vgain] + 1)
     flipud = random.random() < hyp["flipud"]
-    if flipud and nl:
-        labels[:, 2] = 1 - labels[:, 2]
     fliplr = random.random() < hyp["fliplr"]
-    if fliplr and nl:
-        labels[:, 1] = 1 - labels[:, 1]
-    labels_out = np.zeros((nl, 6), dtype=np.float32)
-    if nl:
-        labels_out[:, 1:] = labels
     sources = {p[0] for c in canvases for p in c.places}
     plan = ItemPlan(index, tuple(int(v) for v in out_hw), canvases, mix_r, luts, flipud, fliplr, dataset.im_files[index],
                     shapes, sources)
-    return plan, labels_out
+    return plan, labels_out(labels, out_hw, flipud, fliplr)
 
 
 # ------------------------------------------------------------------------------------------------------------ loader
-def read_source(dataset, i):
-    """load_image's read without the resize (utils/dataloaders.py:739-750): the RAM cache (already resized), an .npy file,
-    an in-memory ``sources`` list, else cv2.imread.  uint8 HWC BGR."""
-    ims = getattr(dataset, "ims", None)
-    if ims is not None and ims[i] is not None:
-        return ims[i]
-    npy = getattr(dataset, "npy_files", None)
-    if npy is not None and Path(npy[i]).exists():
-        return np.load(npy[i])
-    src = getattr(dataset, "sources", None)
-    if src is not None:
-        return src[i]
-    js = jpeg.read(dataset.im_files[i])  # a JPEG the device decodes: its bytes, decoded into the source's slot
-    if js is not None:
-        return js
-    return host_read(dataset, i)
-
-
-def host_read(dataset, i):
-    """cv2.imread of source i: uint8 HWC BGR."""
-    import cv2
-
-    im = cv2.imread(dataset.im_files[i])
-    assert im is not None, f"Image Not Found {dataset.im_files[i]}"
-    return im
-
-
-def _up(n, a=_ALIGN):
-    return (n + a - 1) // a * a
-
-
-def _layout(plans, images):
-    """Byte offsets of one batch in the device work buffer: raw sources, resized sources, descriptors, resize items."""
-    off, raw_off, res_off = 0, {}, {}
-    for i, im in images.items():
-        raw_off[i] = off
-        off += _up(im.nbytes)
-    keys1 = [k for k in sorted({k[:3] for p in plans for k in p.sources}) if (k[1], k[2]) != images[k[0]].shape[:2]]
-    keys2 = sorted({k for p in plans for k in p.sources if len(k) == 5})
-    for k in keys1:
-        res_off[k] = off
-        off += _up(k[1] * k[2] * 3)
-    for k in keys2:
-        res_off[k] = off
-        off += _up(k[3] * k[4] * 3)
-    desc_off = off
-    items_off = desc_off + _up(len(plans) * C.sizeof(_lib.AugmentDesc))
-    total = items_off + _up(max(1, len(keys1) + len(keys2)) * C.sizeof(_lib.ResizeItem))
-    return raw_off, res_off, keys1, keys2, desc_off, items_off, total
-
-
-def batch_bytes(plans, images):
-    """Size of the device work buffer pack_batch fills."""
-    return _layout(plans, images)[-1]
-
-
-def pack_batch(plans, images, dbase, host):
-    """Fill `host` (uint8, >= batch_bytes) with one batch as the device will see it at address `dbase`: the raw sources,
-    room for the resized ones, the y3_augment_desc array and the y3_resize_item arrays of the two resize passes (load_image's
-    resize, then letterbox's second resize).  Returns the offsets and the passes' (items offset, count, max h, max w)."""
-    for i, im in images.items():
-        assert im.dtype == np.uint8 and im.ndim == 3 and im.shape[2] == 3, f"source {i}: uint8 HWC BGR expected"
-    assert all(p.out_hw == plans[0].out_hw for p in plans), \
-        "items of one batch have different shapes (rect batches need an unshuffled sampler)"
-    raw_off, res_off, keys1, keys2, desc_off, items_off, total = _layout(plans, images)
-    assert host.nbytes >= total
-
-    def src(key):  # (device address, row pitch) of a source key
-        if key in res_off:
-            return dbase + res_off[key], key[-1] * 3
-        return dbase + raw_off[key[0]], images[key[0]].shape[1] * 3
-
-    for i, im in images.items():
-        if not isinstance(im, jpeg.JpegSource):  # a JPEG source's slot is written by the device decode
-            host[raw_off[i]: raw_off[i] + im.nbytes] = im.reshape(-1)
-    items = (_lib.ResizeItem * max(1, len(keys1) + len(keys2)))()
-    for j, k in enumerate(keys1):
-        im = images[k[0]]
-        items[j] = _lib.ResizeItem(dbase + raw_off[k[0]], im.shape[0], im.shape[1], im.shape[1] * 3, dbase + res_off[k], k[1],
-                                   k[2], k[2] * 3)
-    for j, k in enumerate(keys2, len(keys1)):
-        sp, pitch = src(k[:3])
-        items[j] = _lib.ResizeItem(sp, k[1], k[2], pitch, dbase + res_off[k], k[3], k[4], k[4] * 3)
-    C.memmove(host[items_off:].ctypes.data, C.addressof(items), C.sizeof(items))
-    descs = (_lib.AugmentDesc * len(plans))()
-    for b, p in enumerate(plans):
-        d = descs[b]
-        for ci, cv in enumerate(p.canvases):
-            dc = d.canvas[ci]
-            dc.n_place = len(cv.places)
-            for pi, (key, x0, y0, x1, y1, ox, oy) in enumerate(cv.places):
-                ptr, pitch = src(key)
-                dc.place[pi] = _lib.AugPlace(ptr, pitch, x0, y0, x1, y1, ox, oy)
-            for q, v in enumerate(invert_affine(cv.M)):
-                dc.inv[q] = v
-        d.mixup = int(len(p.canvases) > 1)
-        d.mix_r = p.mix_r
-        d.hsv = int(p.luts is not None)
-        if p.luts is not None:
-            C.memmove(C.addressof(d.lut), np.ascontiguousarray(p.luts).ctypes.data, 768)
-        d.flipud, d.fliplr = int(p.flipud), int(p.fliplr)
-    C.memmove(host[desc_off:].ctypes.data, C.addressof(descs), C.sizeof(descs))
-    sz = C.sizeof(_lib.ResizeItem)
-    passes = [(items_off, len(keys1), max([k[1] for k in keys1], default=0), max([k[2] for k in keys1], default=0)),
-              (items_off + len(keys1) * sz, len(keys2), max([k[3] for k in keys2], default=0),
-               max([k[4] for k in keys2], default=0))]
-    return {"raw": raw_off, "resized": res_off, "desc_off": desc_off, "resize": passes, "total": total}
-
-
-class _Slot:
-    def __init__(self):
-        self.host = None
-        self.dev = None
-        self.copied = None  # event: the H2D copy out of `host` has completed
-        self.free = None  # event: the consumer has finished with this slot's output images
-        self.out = None
-        self.ws = None  # device workspace of the JPEG decode
-        self.err = None  # device int32 per-image corruption flags of the JPEG decode ...
-        self.err_host = None  # ... copied to pinned memory behind `decoded`
-        self.decoded = None
-        self.jpeg_keys = []  # dataset indices of the batch's device-decoded sources, in desc order
-
-
-def _collate_targets(labels):
-    """collate_fn's targets (utils/dataloaders.py:824-830): the per-item labels with column 0 set to the batch index."""
-    targets = [lb.copy() for lb in labels]
-    for i, lb in enumerate(targets):
-        lb[:, 0] = i
-    return torch.from_numpy(np.concatenate(targets, 0))
-
-
-class _BatchLoader:
-    """What the device loaders share: batches in sampler order, sources read on a thread pool while the previous batch is
-    consumed, two staging slots (pinned host + device work buffer + output images) and a side stream that runs one batch's
-    H2D copy and launches.  Subclasses provide ``_plan(index)`` -> (plan, labels) and ``_launch(plans, labels, images,
-    out, slot)``."""
-
-    def __init__(self, dataset, batch_size, sampler=None, device=None, threads=8, prefetch=True, drop_last=False):
-        self.dataset, self.batch_size = dataset, int(batch_size)
-        self.sampler = sampler if sampler is not None else range(len(dataset.im_files))
-        self.device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-        self.pool = ThreadPoolExecutor(max(1, int(threads)))
-        self.prefetch, self.drop_last = prefetch, drop_last
-        self.stream = torch.cuda.Stream(device=self.device)
-        self._slots = [_Slot(), _Slot()]
-        self._k = 0
-        self.jpeg_decoded = []  # sources of the last batch decoded on the device (dataset indices) ...
-        self.jpeg_fallbacks = []  # ... and those of them whose data the device found corrupt (read again by cv2)
-
-    def __len__(self):
-        n = len(self.sampler)
-        return n // self.batch_size if self.drop_last else (n + self.batch_size - 1) // self.batch_size
-
-    def _batches(self):
-        b = []
-        for i in self.sampler:
-            b.append(int(i))
-            if len(b) == self.batch_size:
-                yield b
-                b = []
-        if b and not self.drop_last:
-            yield b
-
-    # ------------------------------------------------------------------------------------------------ host half
-    def prepare(self, indices):
-        """Plan the items of one batch (in order: this is where any random numbers are drawn) and start reading their
-        sources on the thread pool."""
-        plans, labels = zip(*(self._plan(i) for i in indices))
-        raw = sorted({k[0] for p in plans for k in p.sources})
-        reads = {i: self.pool.submit(read_source, self.dataset, i) for i in raw}
-        return plans, labels, reads
-
-    def launch(self, prepared, out=None, slot=None):
-        """Device half of one batch: one H2D copy (sources + descriptors) and the batch's launches on the loader's stream,
-        writing into ``out`` (a uint8 CUDA [bs, 3, H, W] tensor, e.g. an engine input) or a loader-owned buffer.  The
-        current stream waits for the result.  Without device-decoded JPEG sources nothing synchronises the host; with them,
-        the host waits for the decode's corruption flags (see ``jpeg_decoded`` / ``jpeg_fallbacks``)."""
-        plans, labels, reads = prepared
-        images = {}
-        for i, f in reads.items():
-            im = f.result()
-            if isinstance(im, jpeg.JpegSource) and im.shape[:2] != _hw0(self.dataset, i):
-                # the plan's shape (e.g. the reference's exif_size, which swaps only for EXIF orientations 6 and 8)
-                # differs from the decoded one: cv2.imread as before
-                im = host_read(self.dataset, i)
-            images[i] = im if isinstance(im, jpeg.JpegSource) else np.ascontiguousarray(im)
-        result = self._launch(plans, labels, images, out, slot)
-        sl = self._slots[slot if slot is not None else 0]
-        self.jpeg_decoded = [i for i, im in images.items() if isinstance(im, jpeg.JpegSource)]
-        self.jpeg_fallbacks = []
-        if self.jpeg_decoded:
-            # waits for this batch's copy and decode, which the side stream runs after the previous batch's launches;
-            # those waited for the consumer's work queued before the previous launch (one batch of slack, not two)
-            sl.decoded.synchronize()
-            self.jpeg_fallbacks = [sl.jpeg_keys[k] for k in np.flatnonzero(sl.err_host.numpy()[: len(sl.jpeg_keys)])]
-            if self.jpeg_fallbacks:  # corrupt entropy-coded data: those sources are read by cv2 and the batch runs again
-                for i in self.jpeg_fallbacks:
-                    images[i] = np.ascontiguousarray(host_read(self.dataset, i))
-                result = self._launch(plans, labels, images, out, slot)
-        return result
-
-    def _device_batch(self, bs, H, W, total, fill, run, out, slot, raw_off=None, images=None):
-        """Stage `total` bytes through slot `slot`: ``fill(dbase, host_u8, out)`` packs the pinned buffer as the device will see
-        it at dbase and returns a layout; the copy and ``run(layout, dbase, out, stream_handle)`` go to the side stream.
-        JPEG sources among `images` are staged behind, and decoded into their slots at ``dbase + raw_off[i]`` on the side
-        stream ahead of ``run``; their corruption flags reach ``slot.err_host`` behind ``slot.decoded``."""
-        sl = self._slots[slot if slot is not None else 0]
-        keys = [i for i, im in (images or {}).items() if isinstance(im, jpeg.JpegSource)]
-        srcs = [images[i] for i in keys]
-        jpeg_off = _up(total)
-        if srcs:
-            total = jpeg_off + jpeg.stage_bytes(srcs)
-        if sl.copied is not None:
-            sl.copied.synchronize()  # the previous copy out of this slot's staging buffer has completed
-        if sl.host is None or sl.host.numel() < total:
-            sl.host = torch.empty(int(total * 1.25), dtype=torch.uint8, pin_memory=True)
-        if sl.dev is None or sl.dev.numel() < total:
-            with torch.cuda.stream(self.stream):
-                sl.dev = torch.empty(sl.host.numel(), dtype=torch.uint8, device=self.device)
-        dbase = sl.dev.data_ptr()
-        if out is None:
-            if sl.out is None or tuple(sl.out.shape) != (bs, 3, H, W):
-                with torch.cuda.stream(self.stream):
-                    sl.out = torch.empty(bs, 3, H, W, dtype=torch.uint8, device=self.device)
-            out = sl.out
-        assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (bs, 3, H, W), \
-            f"out must be a contiguous uint8 CUDA [{bs}, 3, {H}, {W}] tensor"
-        lay = fill(dbase, sl.host.numpy(), out)
-        main = torch.cuda.current_stream(self.device)
-        s = self.stream
-        if srcs:
-            wsb = jpeg.workspace_bytes(srcs)
-            with torch.cuda.stream(s):
-                if sl.ws is None or sl.ws.numel() < wsb:
-                    sl.ws = torch.empty(int(wsb * 1.25), dtype=torch.uint8, device=self.device)
-                if sl.err is None or sl.err.numel() < len(srcs):
-                    sl.err = torch.empty(max(64, 2 * len(srcs)), dtype=torch.int32, device=self.device)
-                    sl.err_host = torch.empty(sl.err.numel(), dtype=torch.int32, pin_memory=True)
-            packed = jpeg.pack(srcs, [dbase + raw_off[i] for i in keys], dbase + jpeg_off, sl.host.numpy()[jpeg_off:],
-                               sl.ws.data_ptr())
-            sl.jpeg_keys = keys
-            # the copy and the decode touch only this slot's buffers, which the consumer never reads: they run without
-            # waiting for the consumer's queued work, so the corruption flags are known early
-            with torch.cuda.stream(s):
-                sl.dev[:total].copy_(sl.host[:total], non_blocking=True)
-                sl.copied = torch.cuda.Event()
-                sl.copied.record(s)
-                jpeg.launch(packed, dbase + jpeg_off, sl.ws.data_ptr(), sl.ws.numel(), sl.err.data_ptr(), s.cuda_stream)
-                sl.err_host[: len(srcs)].copy_(sl.err[: len(srcs)], non_blocking=True)
-                sl.decoded = torch.cuda.Event()
-                sl.decoded.record(s)
-        s.wait_stream(main)  # `out` / the slot's previous images are no longer read by the consumer's queued work
-        with torch.cuda.stream(s):
-            if not srcs:
-                sl.dev[:total].copy_(sl.host[:total], non_blocking=True)
-                sl.copied = torch.cuda.Event()
-                sl.copied.record(s)
-            run(lay, dbase, out, s.cuda_stream)
-        main.wait_stream(s)
-        out.record_stream(main)
-        return out
-
-    def collate(self, indices, out=None):
-        """One batch of the given dataset indices, synchronously planned and read: (imgs, targets, paths, shapes)."""
-        return self.launch(self.prepare(indices), out=out, slot=self._next_slot())
-
-    def _next_slot(self):
-        self._k ^= 1
-        return self._k
-
-    def __iter__(self):
-        batches = self._batches()
-        first = next(batches, None)
-        if first is None:
-            return
-        pending = self.prepare(first)
-        while pending is not None:
-            slot = self._next_slot()
-            result = self.launch(pending, slot=slot)
-            nxt = next(batches, None)
-            pending = self.prepare(nxt) if (nxt is not None and self.prefetch) else nxt
-            yield result
-            if pending is not None and not self.prefetch:
-                pending = self.prepare(pending)
-
-    def close(self):
-        self.pool.shutdown(wait=True)
-
-
-class DeviceLoader(_BatchLoader):
+class DeviceLoader(BatchLoader):
     """Iterates like the reference's training DataLoader (train.py:377): ``(imgs uint8 CUDA [bs, 3, H, W], targets [nt, 6]
     (image index in the batch, cls, xywh normalised), paths, shapes)``.
 
@@ -602,19 +302,60 @@ class DeviceLoader(_BatchLoader):
     def _plan(self, index):
         return plan_item(self.dataset, index)
 
-    def _launch(self, plans, labels, images, out, slot):
-        assert all(p.out_hw == plans[0].out_hw for p in plans), \
-            "items of one batch have different shapes (rect batches need an unshuffled sampler)"
+    def _stage(self, plans, images, raw, lay):
+        """The resized sources (load_image's resize, then letterbox's second resize), the y3_resize_item arrays of those
+        two passes and the y3_augment_desc array."""
+        keys1 = [k for k in sorted({k[:3] for p in plans for k in p.sources}) if (k[1], k[2]) != images[k[0]].shape[:2]]
+        keys2 = sorted({k for p in plans for k in p.sources if len(k) == 5})
+        res = {k: lay.take(k[1] * k[2] * 3) for k in keys1}
+        res.update({k: lay.take(k[3] * k[4] * 3) for k in keys2})
+        desc_off = lay.take(len(plans) * C.sizeof(_lib.AugmentDesc))
+        items_off = lay.take(max(1, len(keys1) + len(keys2)) * C.sizeof(_lib.ResizeItem))
         H, W = plans[0].out_hw
 
-        def run(lay, dbase, out, hs):
-            L = _lib.lib()
-            for off, n, mh, mw in lay["resize"]:
-                if n:
-                    _lib.check(L.y3_resize_u8_batched(dbase + off, n, mh, mw, hs), "y3_resize_u8_batched")
-            _lib.check(L.y3_augment_u8(dbase + lay["desc_off"], len(plans), H, W, out.data_ptr(), hs), "y3_augment_u8")
+        def fill(host, dbase, out):
+            def src(key):  # (device address, row pitch) of a source key
+                if key in res:
+                    return dbase + res[key], key[-1] * 3
+                return dbase + raw[key[0]], images[key[0]].shape[1] * 3
 
-        lay = _layout(plans, images)
-        out = self._device_batch(len(plans), H, W, lay[-1], lambda dbase, host, _: pack_batch(plans, images, dbase, host),
-                                 run, out, slot, raw_off=lay[0], images=images)
-        return out, _collate_targets(labels), tuple(p.path for p in plans), tuple(p.shapes for p in plans)
+            items = (_lib.ResizeItem * max(1, len(keys1) + len(keys2)))()
+            for j, k in enumerate(keys1):
+                im = images[k[0]]
+                items[j] = _lib.ResizeItem(dbase + raw[k[0]], im.shape[0], im.shape[1], im.shape[1] * 3, dbase + res[k],
+                                           k[1], k[2], k[2] * 3)
+            for j, k in enumerate(keys2, len(keys1)):
+                sp, pitch = src(k[:3])
+                items[j] = _lib.ResizeItem(sp, k[1], k[2], pitch, dbase + res[k], k[3], k[4], k[4] * 3)
+            C.memmove(host[items_off:].ctypes.data, C.addressof(items), C.sizeof(items))
+            descs = (_lib.AugmentDesc * len(plans))()
+            for b, p in enumerate(plans):
+                d = descs[b]
+                for ci, cv in enumerate(p.canvases):
+                    dc = d.canvas[ci]
+                    dc.n_place = len(cv.places)
+                    for pi, (key, x0, y0, x1, y1, ox, oy) in enumerate(cv.places):
+                        ptr, pitch = src(key)
+                        dc.place[pi] = _lib.AugPlace(ptr, pitch, x0, y0, x1, y1, ox, oy)
+                    for q, v in enumerate(invert_affine(cv.M)):
+                        dc.inv[q] = v
+                d.mixup = int(len(p.canvases) > 1)
+                d.mix_r = p.mix_r
+                d.hsv = int(p.luts is not None)
+                if p.luts is not None:
+                    C.memmove(C.addressof(d.lut), np.ascontiguousarray(p.luts).ctypes.data, 768)
+                d.flipud, d.fliplr = int(p.flipud), int(p.fliplr)
+            C.memmove(host[desc_off:].ctypes.data, C.addressof(descs), C.sizeof(descs))
+            sz = C.sizeof(_lib.ResizeItem)
+
+            def run(hs):
+                L = _lib.lib()
+                for first, n in ((0, len(keys1)), (len(keys1), len(keys2))):  # a pass reads what the one before wrote
+                    if n:
+                        _lib.check(L.y3_resize_u8_batched(dbase + items_off + first * sz, C.addressof(items) + first * sz,
+                                                          n, hs), "y3_resize_u8_batched")
+                _lib.check(L.y3_augment_u8(dbase + desc_off, len(plans), H, W, out.data_ptr(), hs), "y3_augment_u8")
+
+            return run
+
+        return fill

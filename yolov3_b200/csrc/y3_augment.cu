@@ -8,7 +8,8 @@
 // The mosaic canvas is virtual: every warp tap looks its pixel up in the item's placement table (114 where no source is placed),
 // so the 2s x 2s img4 is never written.  The random draws, the geometry and the labels stay on the host (yolov3_b200/augment.py).
 // The validation loader (augment=False) uses y3_resize_area_u8_batched (load_image's INTER_AREA shrink) and
-// y3_letterbox_u8_batched (letterbox without a warp, straight into the CHW RGB batch).
+// y3_letterbox_u8_batched (letterbox without a warp, straight into the CHW RGB batch).  y3_letterbox_u8 is the same letterbox
+// for one image (preprocess.py: detect.py's letterbox(im0) and transpose((2, 0, 1))[::-1], HWC BGR or CHW RGB out).
 //
 // OpenCV's 8-bit rules restated bit for bit (opencv-python 4.13; pinned against cv2 by tests/test_augment_cpu.py):
 //  * warpAffine INTER_LINEAR: coordinates (A11 x) 1024 per column and (A12 y + b1) 1024 per row, each rounded half-even in
@@ -33,13 +34,7 @@ __global__ void __launch_bounds__(256) resize_batched_kernel(const y3_resize_ite
   const y3_resize_item it = items[blockIdx.z];
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= it.dst_w || y >= it.dst_h) return;
-  ResizeGeom g;
-  g.src = static_cast<const uint8_t*>(it.src);
-  g.src_h = it.src_h;
-  g.src_w = it.src_w;
-  g.src_pitch = it.src_pitch;
-  g.new_h = it.dst_h;
-  g.new_w = it.dst_w;
+  ResizeGeom g = resize_geom(it.src, it.src_h, it.src_w, it.src_pitch, it.dst_h, it.dst_w);
   resize_setup(g);
   int v[3];
   resize_pixel(g, x, y, v);
@@ -56,13 +51,7 @@ __global__ void __launch_bounds__(256) resize_area_batched_kernel(const y3_resiz
   const y3_resize_item it = items[blockIdx.z];
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
   if (x >= it.dst_w || y >= it.dst_h) return;
-  ResizeGeom g;
-  g.src = static_cast<const uint8_t*>(it.src);
-  g.src_h = it.src_h;
-  g.src_w = it.src_w;
-  g.src_pitch = it.src_pitch;
-  g.new_h = it.dst_h;
-  g.new_w = it.dst_w;
+  ResizeGeom g = resize_geom(it.src, it.src_h, it.src_w, it.src_pitch, it.dst_h, it.dst_w);
   area_setup(g);
   int v[3];
   area_pixel(g, x, y, v);
@@ -72,36 +61,18 @@ __global__ void __launch_bounds__(256) resize_area_batched_kernel(const y3_resiz
   o[2] = static_cast<uint8_t>(v[2]);
 }
 
-// letterbox without a warp, for a whole batch (the validation loader): letterbox's INTER_LINEAR resize of each source, the
-// 114 border and the HWC BGR -> CHW RGB store of the reference's __getitem__ with augment=False
+// letterbox without a warp: letterbox's INTER_LINEAR resize, the border and the store, for one image (y3_letterbox_u8) ...
+__global__ void __launch_bounds__(256) letterbox_kernel(const y3_letterbox_desc d) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x;
+  if (x < d.out_w) letterbox_pixel(d, x, blockIdx.y);
+}
+
+// ... and for a whole batch (the validation loader: the 114 border and the CHW RGB store of __getitem__ with augment=False)
 __global__ void __launch_bounds__(256) letterbox_batched_kernel(const y3_letterbox_desc* __restrict__ descs) {
   pdl_entry();
   const y3_letterbox_desc d = descs[blockIdx.z];
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
-  if (x >= d.out_w || y >= d.out_h) return;
-  int v[3] = {d.pad[0], d.pad[1], d.pad[2]};
-  const int dx = x - d.left, dy = y - d.top;
-  if (dx >= 0 && dx < d.new_w && dy >= 0 && dy < d.new_h) {
-    ResizeGeom g;
-    g.src = static_cast<const uint8_t*>(d.src);
-    g.src_h = d.src_h;
-    g.src_w = d.src_w;
-    g.src_pitch = d.src_pitch;
-    g.new_h = d.new_h;
-    g.new_w = d.new_w;
-    resize_setup(g);
-    resize_pixel(g, dx, dy, v);
-  }
-  uint8_t* dst = static_cast<uint8_t*>(d.dst);
-  const size_t at = static_cast<size_t>(y) * d.out_w + x;
-  if (d.out_chw) {
-    const size_t plane = static_cast<size_t>(d.out_h) * d.out_w;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) dst[(d.swap_rb ? 2 - c : c) * plane + at] = static_cast<uint8_t>(v[c]);
-  } else {
-#pragma unroll
-    for (int c = 0; c < 3; ++c) dst[at * 3 + (d.swap_rb ? 2 - c : c)] = static_cast<uint8_t>(v[c]);
-  }
+  if (x < d.out_w && y < d.out_h) letterbox_pixel(d, x, y);
 }
 
 // one canvas pixel: a placed source pixel, else the 114 of img4 / the letterbox border / warpAffine's borderValue
@@ -230,33 +201,65 @@ __global__ void __launch_bounds__(kAugThreads) augment_kernel(const y3_augment_d
 }  // namespace
 }  // namespace y3
 
-extern "C" int y3_resize_u8_batched(const y3_resize_item* items, int32_t n_items, int32_t max_h, int32_t max_w,
-                                    y3_stream_t stream) {
-  Y3_REQUIRE(items && n_items > 0 && n_items <= 65535 && max_h > 0 && max_h <= 65535 && max_w > 0,
-             "resize_batched: bad arguments (n_items %d, max %dx%d)", n_items, max_h, max_w);
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::resize_batched_kernel, dim3((max_w + 255) / 256, max_h, n_items), dim3(256), 0,
-                                 static_cast<cudaStream_t>(stream), items));
+namespace y3 {
+namespace {
+
+// what every resize entry point requires of an item
+int check_resize_item(const y3_resize_item& it, const char* who, int i) {
+  Y3_REQUIRE(it.src && it.dst && it.src_h > 0 && it.src_w > 0 && it.dst_h > 0 && it.dst_w > 0 &&
+                 it.src_pitch >= 3 * it.src_w && it.dst_pitch >= 3 * it.dst_w,
+             "%s: item %d: bad shape or pointer", who, i);
   return Y3_OK;
 }
 
-extern "C" int y3_resize_area_u8_batched(const y3_resize_item* items, const y3_resize_item* host_items, int32_t n_items,
-                                         y3_stream_t stream) {
-  Y3_REQUIRE(items && host_items && n_items > 0 && n_items <= 65535, "resize_area: bad arguments (n_items %d)", n_items);
+// what every letterbox entry point requires of a descriptor
+int check_letterbox_desc(const y3_letterbox_desc& d, const char* who, int i) {
+  Y3_REQUIRE(d.src && d.dst && d.src_h > 0 && d.src_w > 0 && d.src_pitch >= 3 * d.src_w && d.new_h > 0 && d.new_w > 0,
+             "%s: item %d: bad source / resize shape or null pointer", who, i);
+  Y3_REQUIRE(d.top >= 0 && d.left >= 0 && d.out_h >= d.top + d.new_h && d.out_w >= d.left + d.new_w,
+             "%s: item %d: the resized image must fit the output", who, i);
+  return Y3_OK;
+}
+
+// one launch of a batched resize kernel over `items` (device), validated and sized from `host_items`; `shrink_only` refuses
+// an item that scales up (INTER_AREA is built for scales >= 1 only)
+int launch_resize(void (*kern)(const y3_resize_item*), const char* who, bool shrink_only, const y3_resize_item* items,
+                  const y3_resize_item* host_items, int32_t n_items, y3_stream_t stream) {
+  Y3_REQUIRE(items && host_items && n_items > 0 && n_items <= 65535, "%s: bad arguments (n_items %d)", who, n_items);
   int max_h = 0, max_w = 0;
   for (int i = 0; i < n_items; ++i) {
     const y3_resize_item& it = host_items[i];
-    Y3_REQUIRE(it.src && it.dst && it.src_h > 0 && it.src_w > 0 && it.dst_h > 0 && it.dst_w > 0 &&
-                   it.src_pitch >= 3 * it.src_w && it.dst_pitch >= 3 * it.dst_w,
-               "resize_area: item %d: bad shape or pointer", i);
-    Y3_REQUIRE(it.dst_h <= it.src_h && it.dst_w <= it.src_w,
-               "resize_area: item %d: %dx%d -> %dx%d scales up; INTER_AREA is built for scales >= 1 only", i, it.src_h,
+    if (const int rc = check_resize_item(it, who, i)) return rc;
+    Y3_REQUIRE(!shrink_only || (it.dst_h <= it.src_h && it.dst_w <= it.src_w),
+               "%s: item %d: %dx%d -> %dx%d scales up; INTER_AREA is built for scales >= 1 only", who, i, it.src_h,
                it.src_w, it.dst_h, it.dst_w);
     max_h = max(max_h, it.dst_h);
     max_w = max(max_w, it.dst_w);
   }
-  Y3_REQUIRE(max_h <= 65535, "resize_area: output too tall (%d rows)", max_h);
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::resize_area_batched_kernel, dim3((max_w + 255) / 256, max_h, n_items), dim3(256), 0,
-                                 static_cast<cudaStream_t>(stream), items));
+  Y3_REQUIRE(max_h <= 65535, "%s: output too tall (%d rows)", who, max_h);
+  Y3_CHECK_CUDA(launch_pdl(kern, dim3((max_w + 255) / 256, max_h, n_items), dim3(256), 0, static_cast<cudaStream_t>(stream),
+                           items));
+  return Y3_OK;
+}
+
+}  // namespace
+}  // namespace y3
+
+extern "C" int y3_resize_u8_batched(const y3_resize_item* items, const y3_resize_item* host_items, int32_t n_items,
+                                    y3_stream_t stream) {
+  return y3::launch_resize(y3::resize_batched_kernel, "resize", false, items, host_items, n_items, stream);
+}
+
+extern "C" int y3_resize_area_u8_batched(const y3_resize_item* items, const y3_resize_item* host_items, int32_t n_items,
+                                         y3_stream_t stream) {
+  return y3::launch_resize(y3::resize_area_batched_kernel, "resize_area", true, items, host_items, n_items, stream);
+}
+
+extern "C" int y3_letterbox_u8(const y3_letterbox_desc* d, y3_stream_t stream) {
+  Y3_REQUIRE(d, "letterbox: null descriptor");
+  if (const int rc = y3::check_letterbox_desc(*d, "letterbox", 0)) return rc;
+  y3::letterbox_kernel<<<dim3((d->out_w + 255) / 256, d->out_h), 256, 0, static_cast<cudaStream_t>(stream)>>>(*d);
+  Y3_CHECK_CUDA(cudaGetLastError());
   return Y3_OK;
 }
 
@@ -265,13 +268,9 @@ extern "C" int y3_letterbox_u8_batched(const y3_letterbox_desc* descs, const y3_
   Y3_REQUIRE(descs && host_descs && n > 0 && n <= 65535, "letterbox_batched: bad arguments (n %d)", n);
   int max_h = 0, max_w = 0;
   for (int i = 0; i < n; ++i) {
-    const y3_letterbox_desc& d = host_descs[i];
-    Y3_REQUIRE(d.src && d.dst && d.src_h > 0 && d.src_w > 0 && d.src_pitch >= 3 * d.src_w && d.new_h > 0 && d.new_w > 0,
-               "letterbox_batched: item %d: bad source / resize shape", i);
-    Y3_REQUIRE(d.top >= 0 && d.left >= 0 && d.out_h >= d.top + d.new_h && d.out_w >= d.left + d.new_w,
-               "letterbox_batched: item %d: the resized image must fit the output", i);
-    max_h = max(max_h, d.out_h);
-    max_w = max(max_w, d.out_w);
+    if (const int rc = y3::check_letterbox_desc(host_descs[i], "letterbox_batched", i)) return rc;
+    max_h = max(max_h, host_descs[i].out_h);
+    max_w = max(max_w, host_descs[i].out_w);
   }
   Y3_REQUIRE(max_h <= 65535, "letterbox_batched: output too tall (%d rows)", max_h);
   Y3_CHECK_CUDA(::y3::launch_pdl(y3::letterbox_batched_kernel, dim3((max_w + 255) / 256, max_h, n), dim3(256), 0,

@@ -1,13 +1,15 @@
 // yolov3_b200 — OpenCV's 8-bit INTER_LINEAR resize (third-party, opencv-python 4.13; resize.cpp) restated bit for bit, shared
-// by the letterbox kernel (y3_pre.cu) and the batched resize of the training loader (y3_augment.cu): 11-bit fixed-point
-// coefficients from float fractions, horizontal pass to int, vertical pass ((b0*(S0>>4))>>16 + (b1*(S1>>4))>>16 + 2) >> 2; an
-// exact 2x shrink takes INTER_AREA's 2x2 average like cv::resize does, and an equal size is a plain copy.  INTER_AREA for
-// scales >= 1 (the validation loader's load_image shrink, y3_augment.cu) follows at the end.
+// by the letterbox kernels and the batched resize of the loaders (y3_augment.cu): 11-bit fixed-point coefficients from float
+// fractions, horizontal pass to int, vertical pass ((b0*(S0>>4))>>16 + (b1*(S1>>4))>>16 + 2) >> 2; an exact 2x shrink takes
+// INTER_AREA's 2x2 average like cv::resize does, and an equal size is a plain copy.  The letterbox pixel (border, resize,
+// HWC / CHW store) and INTER_AREA for scales >= 1 (the validation loader's load_image shrink) follow.
 // Include only from sources compiled without fast-math / FMA contraction (build.py EXACT_SOURCES).
 #pragma once
 
 #include <math.h>
 #include <stdint.h>
+
+#include "../../include/yolov3_b200.h"
 
 namespace y3 {
 
@@ -19,6 +21,18 @@ struct ResizeGeom {
   int mode;                  // 0: copy (no resize), 1: bilinear, 2: 2x2 area average, 3: kx x ky block mean, 4: area
   int kx, ky;                // the integer factors of mode 3
 };
+
+// the source and the output size of a resize; resize_setup / area_setup derive the rest
+__device__ __forceinline__ ResizeGeom resize_geom(const void* src, int src_h, int src_w, int src_pitch, int new_h, int new_w) {
+  ResizeGeom g;
+  g.src = static_cast<const uint8_t*>(src);
+  g.src_h = src_h;
+  g.src_w = src_w;
+  g.src_pitch = src_pitch;
+  g.new_h = new_h;
+  g.new_w = new_w;
+  return g;
+}
 
 // scale and mode of a resize from the sizes (the scalar part of cv::resize)
 __host__ __device__ inline void resize_setup(ResizeGeom& g) {
@@ -79,6 +93,28 @@ __device__ __forceinline__ void resize_pixel(const ResizeGeom& p, int dx, int dy
       const int s1 = q1[sx * 3 + c] * ax0 + q1[sx1 * 3 + c] * ax1;
       v[c] = (((b0 * (s0 >> 4)) >> 16) + ((b1 * (s1 >> 4)) >> 16) + 2) >> 2;
     }
+  }
+}
+
+// output pixel (x, y) of the letterbox d: pad[] outside the resized image, its INTER_LINEAR pixel inside; stored HWC or CHW,
+// the channels reversed when swap_rb
+__device__ __forceinline__ void letterbox_pixel(const y3_letterbox_desc& d, int x, int y) {
+  int v[3] = {d.pad[0], d.pad[1], d.pad[2]};
+  const int dx = x - d.left, dy = y - d.top;
+  if (dx >= 0 && dx < d.new_w && dy >= 0 && dy < d.new_h) {
+    ResizeGeom g = resize_geom(d.src, d.src_h, d.src_w, d.src_pitch, d.new_h, d.new_w);
+    resize_setup(g);
+    resize_pixel(g, dx, dy, v);
+  }
+  uint8_t* dst = static_cast<uint8_t*>(d.dst);
+  const size_t at = static_cast<size_t>(y) * d.out_w + x;
+  if (d.out_chw) {
+    const size_t plane = static_cast<size_t>(d.out_h) * d.out_w;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) dst[(d.swap_rb ? 2 - c : c) * plane + at] = static_cast<uint8_t>(v[c]);
+  } else {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) dst[at * 3 + (d.swap_rb ? 2 - c : c)] = static_cast<uint8_t>(v[c]);
   }
 }
 

@@ -6,9 +6,9 @@ or extended-sequential 8-bit Huffman, one interleaved scan, grayscale or YCbCr, 
 4:1:1).  Every other file — progressive, arithmetic, lossless, 12-bit, CMYK, PNG, ... — and every file whose entropy-coded
 data turns out corrupt on the device is decoded by cv2, so the result is always cv2's.
 
-``imdecode_batch(bufs)`` decodes a list of encoded buffers into uint8 CUDA ``[h, w, 3]`` BGR tensors.  The training and
-validation loaders (``yolov3_b200.augment``, ``yolov3_b200.valloader``) use ``read`` / ``stage_bytes`` / ``pack`` /
-``launch`` to decode their JPEG sources straight into the slots their resize kernels read."""
+``imdecode_batch(bufs)`` decodes a list of encoded buffers into uint8 CUDA ``[h, w, 3]`` BGR tensors.  ``Batch`` stages the
+sources of one decode launch: ``stage`` gives it buffers of its own, and the device loaders (``yolov3_b200.loader``) lay it
+out in their staging buffer, decoding their JPEG sources straight into the slots their resize kernels read."""
 from __future__ import annotations
 
 import ctypes as C
@@ -17,12 +17,6 @@ import numpy as np
 import torch
 
 from . import _lib
-
-_ALIGN = 256
-
-
-def _up(n, a=_ALIGN):
-    return (n + a - 1) // a * a
 
 
 class JpegSource:
@@ -73,58 +67,58 @@ def read(path):
         return parse(np.frombuffer(head + f.read(), dtype=np.uint8))
 
 
-def _stage_layout(srcs):
-    off, offs = 0, []
-    for s in srcs:
-        g = s.info.geom
-        t = off
-        d = t + _up(_lib.JPEG_TABLE_BYTES)
-        sg = d + _up(g.data_len)
-        off = sg + _up(8 * g.n_segs)
-        offs.append((t, d, sg))
-    desc_off = off
-    return offs, desc_off, desc_off + _up(len(srcs) * C.sizeof(_lib.JpegDesc))
+class Batch:
+    """JpegSources staged for one y3_jpeg_decode_batched launch.  The constructor lays out, in the caller's
+    ``_lib.Regions``, each file's tables, entropy-coded bytes and restart segments, then the y3_jpeg_desc array, and sizes
+    the device workspace (``ws_bytes``); ``pack`` fills the staging buffer and ``launch`` runs the decode."""
+
+    def __init__(self, srcs, lay):
+        L = _lib.lib()
+        self.srcs = srcs
+        self.offs = [(lay.take(_lib.JPEG_TABLE_BYTES), lay.take(s.info.geom.data_len), lay.take(8 * s.info.geom.n_segs))
+                     for s in srcs]
+        self.desc_off = lay.take(len(srcs) * C.sizeof(_lib.JpegDesc))
+        ws = _lib.Regions()
+        self.ws_offs = [ws.take(L.y3_jpeg_workspace_bytes(C.byref(s.info.geom))) for s in srcs]
+        self.ws_bytes = ws.size
+
+    def pack(self, host, dbase, dsts, ws_ptr, err_ptr):
+        """Fill `host` (uint8, the staging buffer as the device sees it at `dbase`) to decode source k into ``dsts[k]``
+        (device address, HWC BGR, dense rows), its workspace carved from ``ws_ptr`` (>= ws_bytes) and its corruption flag
+        written to ``err_ptr[k]`` (device int32)."""
+        descs = (_lib.JpegDesc * len(self.srcs))()
+        for k, (s, (t, d, sg), w) in enumerate(zip(self.srcs, self.offs, self.ws_offs)):
+            g = s.info.geom
+            host[t: t + _lib.JPEG_TABLE_BYTES] = np.frombuffer(s.info.tables, dtype=np.uint8)
+            a = s.info.data_off
+            host[d: d + g.data_len] = s.buf[a: a + g.data_len]
+            host[sg: sg + 8 * g.n_segs] = s.segs.reshape(-1).view(np.uint8)
+            dd = descs[k]
+            dd.geom = g
+            dd.data, dd.tables, dd.segs = dbase + d, dbase + t, dbase + sg
+            dd.ws, dd.dst, dd.dst_pitch = ws_ptr + w, dsts[k], g.width * 3
+        C.memmove(host[self.desc_off:].ctypes.data, C.addressof(descs), C.sizeof(descs))
+        self._descs, self._ptrs = descs, (dbase + self.desc_off, ws_ptr, err_ptr)
+
+    def launch(self, stream_handle):
+        """The decode of the packed batch on a stream, once its staging buffer has reached the device."""
+        desc_ptr, ws_ptr, err_ptr = self._ptrs
+        _lib.check(_lib.lib().y3_jpeg_decode_batched(desc_ptr, C.addressof(self._descs), len(self._descs), ws_ptr,
+                                                     self.ws_bytes, err_ptr, stream_handle), "y3_jpeg_decode_batched")
 
 
-def stage_bytes(srcs):
-    """Bytes of the host-to-device staging region pack() fills for these sources."""
-    return _stage_layout(srcs)[-1]
-
-
-def workspace_bytes(srcs):
-    L = _lib.lib()
-    return sum(_up(L.y3_jpeg_workspace_bytes(C.byref(s.info.geom))) for s in srcs)
-
-
-def pack(srcs, dsts, dbase, host, ws_ptr):
-    """Stage `srcs` into `host` (uint8, >= stage_bytes) as the device sees it at `dbase`: each file's tables, entropy-coded
-    bytes and segments, then the y3_jpeg_desc array decoding source k into ``dsts[k]`` (device address, HWC BGR, dense
-    rows), with its workspace carved from ``ws_ptr``.  Returns (desc offset, host descs)."""
-    L = _lib.lib()
-    offs, desc_off, total = _stage_layout(srcs)
-    assert host.nbytes >= total
-    descs = (_lib.JpegDesc * len(srcs))()
-    ws = ws_ptr
-    for k, (s, (t, d, sg)) in enumerate(zip(srcs, offs)):
-        g = s.info.geom
-        host[t: t + _lib.JPEG_TABLE_BYTES] = np.frombuffer(s.info.tables, dtype=np.uint8)
-        a = s.info.data_off
-        host[d: d + g.data_len] = s.buf[a: a + g.data_len]
-        host[sg: sg + 8 * g.n_segs] = s.segs.reshape(-1).view(np.uint8)
-        dd = descs[k]
-        dd.geom = g
-        dd.data, dd.tables, dd.segs = dbase + d, dbase + t, dbase + sg
-        dd.ws, dd.dst, dd.dst_pitch = ws, dsts[k], g.width * 3
-        ws += _up(L.y3_jpeg_workspace_bytes(C.byref(g)))
-    C.memmove(host[desc_off:].ctypes.data, C.addressof(descs), C.sizeof(descs))
-    return desc_off, descs
-
-
-def launch(packed, dbase, ws_ptr, ws_bytes, err_ptr, stream_handle):
-    """y3_jpeg_decode_batched of a pack() result on a stream; err_ptr: device int32 [n] of per-image corruption flags."""
-    desc_off, descs = packed
-    _lib.check(_lib.lib().y3_jpeg_decode_batched(dbase + desc_off, C.addressof(descs), len(descs), ws_ptr, ws_bytes, err_ptr,
-                                                 stream_handle), "y3_jpeg_decode_batched")
+def stage(srcs, dsts, device):
+    """A Batch decoding `srcs` into `dsts` (device addresses) with buffers of its own: staged, workspace and flags (``err``,
+    int32 CUDA [n]) allocated on `device`, and the staging buffer copied on the current stream."""
+    lay = _lib.Regions()
+    b = Batch(srcs, lay)
+    host = torch.empty(lay.size, dtype=torch.uint8, pin_memory=True)
+    b.dev = torch.empty(lay.size, dtype=torch.uint8, device=device)
+    b.ws = torch.empty(b.ws_bytes, dtype=torch.uint8, device=device)
+    b.err = torch.empty(len(srcs), dtype=torch.int32, device=device)
+    b.pack(host.numpy(), b.dev.data_ptr(), dsts, b.ws.data_ptr(), b.err.data_ptr())
+    b.dev.copy_(host, non_blocking=True)
+    return b
 
 
 def _host_decode(buf, device):
@@ -140,16 +134,9 @@ def decode_batch(srcs, device=None):
     device = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
     with torch.cuda.device(device):
         outs = [torch.empty(*s.shape, dtype=torch.uint8, device=device) for s in srcs]
-        nb = stage_bytes(srcs)
-        host = torch.empty(nb, dtype=torch.uint8, pin_memory=True)
-        dev = torch.empty(nb, dtype=torch.uint8, device=device)
-        wsb = workspace_bytes(srcs)
-        ws = torch.empty(wsb, dtype=torch.uint8, device=device)
-        err = torch.empty(len(srcs), dtype=torch.int32, device=device)
-        packed = pack(srcs, [o.data_ptr() for o in outs], dev.data_ptr(), host.numpy(), ws.data_ptr())
-        dev.copy_(host, non_blocking=True)
-        launch(packed, dev.data_ptr(), ws.data_ptr(), wsb, err.data_ptr(), torch.cuda.current_stream(device).cuda_stream)
-        return outs, err.cpu().numpy()
+        b = stage(srcs, [o.data_ptr() for o in outs], device)
+        b.launch(torch.cuda.current_stream(device).cuda_stream)
+        return outs, b.err.cpu().numpy()
 
 
 def imdecode_batch(bufs, device=None):

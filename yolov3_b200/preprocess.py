@@ -4,7 +4,8 @@
 image (returns ``(im, ratio, (dw, dh))`` exactly like the reference, the image staying on the device), and ``preprocess`` — what
 ``LoadImages.__next__`` hands to the model (utils/dataloaders.py:305-310: letterbox, HWC->CHW, BGR->RGB, contiguous) written
 straight into a CHW uint8 tensor such as an engine's input buffer; ``im.float() / 255`` (detect.py:187-191) is applied by the
-first conv kernel.  One launch; the resize is OpenCV's 8-bit INTER_LINEAR bit for bit (csrc/y3_pre.cu)."""
+first conv kernel.  One launch of ``y3_letterbox_u8``, whose per-pixel routine the validation loader's batched letterbox
+shares; the resize is OpenCV's 8-bit INTER_LINEAR bit for bit (csrc/y3_resize.cuh, csrc/y3_augment.cu)."""
 from __future__ import annotations
 
 import ctypes as C
