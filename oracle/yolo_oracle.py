@@ -694,8 +694,10 @@ def build_targets(shapes, targets, anchors, anchor_t=4.0):
         gxy, gwh, a = t[:, 2:4], t[:, 4:6], t[:, 6].long()
         gij = (gxy - offsets).long()
         gi, gj = gij[:, 0].clamp(0, nx - 1), gij[:, 1].clamp(0, ny - 1)
-        # NB reference clamps gj/gi in place AFTER gij is used for tbox (loss.py:239-240): tbox uses unclamped gij
-        out.append(dict(b=b, a=a, gj=gj, gi=gi, tbox=torch.cat((gxy - gij, gwh), 1), anch=anchors[i][a], tcls=c))
+        # the reference's gi, gj are views of gij clamped in place (loss.py:239) BEFORE tbox is formed (loss.py:240):
+        # tbox uses the clamped cell, so a target at x or y == 1.0 gets a box offset of 1.0
+        tbox = torch.cat((gxy - torch.stack((gi, gj), 1), gwh), 1)
+        out.append(dict(b=b, a=a, gj=gj, gi=gi, tbox=tbox, anch=anchors[i][a], tcls=c))
     return out
 
 

@@ -194,8 +194,8 @@ def gen_scale_boxes():
 
 def loss_inputs(case):
     g = torch.Generator().manual_seed(200 + case)
-    bs = [2, 3, 1, 2][case]
-    hw = [(8, 8), (8, 12), (4, 4), (8, 8)][case]
+    bs = [2, 3, 1, 2, 3][case]
+    hw = [(8, 8), (8, 12), (4, 4), (8, 8), (6, 10)][case]
     p = [torch.randn(bs, 3, hw[0] * s, hw[1] * s, 85, generator=g) for s in (4, 2, 1)]
     if case == 0:
         t = O.synth_targets(bs, seed=2)
@@ -205,8 +205,18 @@ def loss_inputs(case):
         t[1, 2:4] = torch.tensor([0.001, 0.999])  # near the image edge -> index clamp
     elif case == 2:
         t = torch.zeros(0, 6)  # no targets
-    else:
+    elif case == 3:
         t = O.synth_targets(bs, seed=9)[:1]  # single target
+    else:
+        # centres exactly on the far edge (the dataset's <= 1 label check accepts them): the cell index is clamped to
+        # the last column / row, and the box offset is taken from the clamped cell (tx or ty = 1.0)
+        edge = torch.tensor([[0, 3, 1.0, 0.40, 0.20, 0.30],
+                             [1, 17, 0.30, 1.0, 0.10, 0.05],
+                             [2, 42, 1.0, 1.0, 0.30, 0.25],
+                             [1, 0, 1.0, 0.75, 0.05, 0.08],
+                             [2, 79, 0.60, 1.0, 0.40, 0.50],
+                             [0, 5, 1.0, 1.0, 0.02, 0.03]])
+        t = torch.cat((O.synth_targets(bs, seed=13), edge))
     return p, t
 
 
@@ -220,7 +230,7 @@ def gen_loss():
     cl = ComputeLoss(m)
     anchors = m.model[-1].anchors
     store = {"hyp": np.array(repr(m.hyp))}
-    for case in range(4):
+    for case in range(5):
         p, t = loss_inputs(case)
         pr = [x.clone().requires_grad_(True) for x in p]
         loss, items = cl(pr, t.clone())

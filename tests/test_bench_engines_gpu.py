@@ -520,35 +520,12 @@ def _nhwc(t):
     return t.permute(0, 2, 3, 1)
 
 
-def test_train_step_640_bs8_every_block():
-    """One eager step, then a CUDA-graph replayed step (gradients zeroed in between) of the benchmark's training engine:
-    split-K wgrad (deterministic = False) and graphs, as tools/bench_workloads.train_step_workload runs it."""
-    from yolov3_b200 import synth
-    from yolov3_b200.loss import ComputeLoss
-    from yolov3_b200.model import Model
-    from yolov3_b200.train import TrainEngine, TrainFn
-
-    torch.manual_seed(0)
-    m = Model("yolov3.yaml", device="cuda")
-    m.hyp = synth.scaled_hyp()
-    m.train()
-    n, hw = 8, 640
-    te = TrainEngine(m, n, hw, hw, keep_all=True)
-    te.deterministic, te.use_graphs = False, True
-    m._train_engines[(n, hw, hw)] = te
-    x = torch.randint(0, 256, (n, 3, hw, hw), dtype=torch.uint8, generator=torch.Generator().manual_seed(11)).cuda()
-    targets = synth.synth_targets(n, seed=2).cuda()
-    P = m.device_params()
-    loss_fn = ComputeLoss(m)
-    for _ in range(2):
-        m.store().G.zero_()
-        raw = list(TrainFn.apply(te, x, 255.0, *[P[k] for k in te.param_names]))
-        loss, _ = loss_fn(raw, targets)
-        loss.backward()
-        torch.cuda.synchronize()
-        te.check_errors()
-    assert "graph" in te._graphs["fwd"] and all("graph" in st for key, st in te._graphs.items() if key[0] == "bwd")
-
+def check_train_blocks(te, P, worst, bad, tag="train"):
+    """Every Conv block of a TrainEngine on the tensors its last step left behind (references in float32 on the device):
+    y, a, dy, dgamma, dbeta, dW, and dx where the block is the only contribution to its input.  Failures are appended to
+    ``bad``, measured values to ``worst``; returns ({damaged reference: [rejected, ...]}, number of blocks whose dx was
+    compared).  Damaged references are tried where the blocks they need exist (block 1, model.16, model.2.cv1, the first
+    dx with a shortcut gradient)."""
     n_contrib, shortcut_of = {}, {}
     for b in te.blocks:
         if not b.first:
@@ -559,7 +536,7 @@ def test_train_step_640_bs8_every_block():
     head_inputs = {(hd["x"].buf.data_ptr(), hd["x"].coff, hd["x"].c) for hd in te.heads}
     pooled = {b.a.buf.data_ptr() for b in te.blocks if b.post_fwd}
 
-    worst, bad, damaged = Worst(), [], {}
+    damaged = {}
     n_dx = 0
     for bi, b in enumerate(te.blocks):
         pre = b.prefix
@@ -699,7 +676,41 @@ def test_train_step_640_bs8_every_block():
                 damaged["dx"] = [not bf16_ok(check_bf16(dx_got, dr, l1, EPS_DX), MIN_EXACT_DX) for dr in (
                     tile_from_next_image(dx_ref), channel_shifted(dx_ref), residual_missing(dx_ref, g_sc))]
             del dx_ref, l1
-        print(f"train {pre} {b.c1}->{b.c2} {b.k}x{b.k}/{b.s} @{b.x.h}x{b.x.w}: worst err/bound " + ", ".join(line))
+        print(f"{tag} {pre} {b.c1}->{b.c2} {b.k}x{b.k}/{b.s} @{b.x.h}x{b.x.w}: worst err/bound " + ", ".join(line))
+    return damaged, n_dx
+
+
+def test_train_step_640_bs8_every_block():
+    """One eager step, then a CUDA-graph replayed step (gradients zeroed in between) of the benchmark's training engine:
+    split-K wgrad (deterministic = False) and graphs, as tools/bench_workloads.train_step_workload runs it."""
+    from yolov3_b200 import synth
+    from yolov3_b200.loss import ComputeLoss
+    from yolov3_b200.model import Model
+    from yolov3_b200.train import TrainEngine, TrainFn
+
+    torch.manual_seed(0)
+    m = Model("yolov3.yaml", device="cuda")
+    m.hyp = synth.scaled_hyp()
+    m.train()
+    n, hw = 8, 640
+    te = TrainEngine(m, n, hw, hw, keep_all=True)
+    te.deterministic, te.use_graphs = False, True
+    m._train_engines[(n, hw, hw)] = te
+    x = torch.randint(0, 256, (n, 3, hw, hw), dtype=torch.uint8, generator=torch.Generator().manual_seed(11)).cuda()
+    targets = synth.synth_targets(n, seed=2).cuda()
+    P = m.device_params()
+    loss_fn = ComputeLoss(m)
+    for _ in range(2):
+        m.store().G.zero_()
+        raw = list(TrainFn.apply(te, x, 255.0, *[P[k] for k in te.param_names]))
+        loss, _ = loss_fn(raw, targets)
+        loss.backward()
+        torch.cuda.synchronize()
+        te.check_errors()
+    assert "graph" in te._graphs["fwd"] and all("graph" in st for key, st in te._graphs.items() if key[0] == "bwd")
+
+    worst, bad = Worst(), []
+    damaged, n_dx = check_train_blocks(te, P, worst, bad)
     worst.report("train")
     print(f"train: dx compared on {n_dx} blocks; damaged references rejected: {damaged}")
     assert not bad, "\n".join(bad[:20])

@@ -31,7 +31,7 @@ def _model(anchors, hyp):
     return m
 
 
-@pytest.mark.parametrize("case", range(4))
+@pytest.mark.parametrize("case", range(5))
 def test_loss_golden(case):
     from make_golden import loss_inputs
 

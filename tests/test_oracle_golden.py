@@ -55,7 +55,7 @@ def test_nms_bit_exact(case):
         assert np.array_equal(s, g[f"{case}/src{xi}"])
 
 
-@pytest.mark.parametrize("case", range(4))
+@pytest.mark.parametrize("case", range(5))
 def test_loss_matches_reference(case):
     import sys
     sys.path.insert(0, str(G))

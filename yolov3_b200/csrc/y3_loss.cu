@@ -73,8 +73,10 @@ __global__ void __launch_bounds__(256) loss_match_kernel(const LossArgs p) {
   mt.a = a;
   mt.gi = min(max(gi0, 0), d.nx[l] - 1);
   mt.gj = min(max(gj0, 0), d.ny[l] - 1);
-  mt.tx = gx - static_cast<float>(gi0);
-  mt.ty = gy - static_cast<float>(gj0);
+  // loss.py:239 clamps gi / gj in place (they are views of gij) before line 240 forms gxy - gij: a target on the far
+  // edge (x or y == 1.0) gets its box offset from the clamped cell, tx = 1.0
+  mt.tx = gx - static_cast<float>(mt.gi);
+  mt.ty = gy - static_cast<float>(mt.gj);
   mt.tw = gw;
   mt.th = gh;
   mt.aw = aw;

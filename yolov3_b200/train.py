@@ -71,6 +71,7 @@ class TrainEngine:
         self.blocks: list[_Block] = []
         self.keep = []
         self.grad_bufs: dict[int, PaddedNHWC] = {}
+        self.pools: list[dict] = []  # one record per max-pool: its wiring, for the tests (the launches are closures)
         self.scratch: dict[tuple, PaddedNHWC] = {}
         self.keep_all = keep_all
         self.zero_bias = torch.zeros(4096, dtype=torch.float32, device=dev)  # identity-epilogue convs (forward and dgrad)
@@ -150,6 +151,7 @@ class TrainEngine:
                     idx = torch.zeros(n * ly.h * ly.w * c_, dtype=torch.uint8, device=dev)
                     self.keep.append(idx)
                     src, dst = cat.slice(0, c_), cat.slice((q + 1) * c_, c_)
+                    self.pools.append(dict(src=src, dst=dst, k=k, stride=1, off=-(k // 2), oob_zero=False))
                     b1.post_fwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_train_fwd(src, dst, k, idx))
                     b1.pre_bwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_bwd(self.grad_of(dst), self.grad_of(src),
                                                                                         k, idx, accumulate=True))
@@ -164,6 +166,7 @@ class TrainEngine:
                 y = out_of(ly)
                 idx = torch.zeros(n * y.h * y.w * x.c, dtype=torch.uint8, device=dev)
                 self.keep.append(idx)
+                self.pools.append(dict(src=x, dst=y, k=p.k, stride=p.s, off=-p.pad, oob_zero=p.oob_zero))
                 host = self.blocks[-1]  # the pool runs after the latest block's forward and before that block's backward
                 host.post_fwd.append(lambda x=x, y=y, p=p, idx=idx:
                                      T.maxpool_train_fwd(x, y, p.k, idx, stride=p.s, off=-p.pad, oob_zero=p.oob_zero))
