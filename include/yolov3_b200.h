@@ -40,7 +40,8 @@ int y3_device_check(void);
 /* sizeof() of the ABI structs, for bindings to verify their mirror definitions:
  * 0 y3_conv_desc, 1 y3_first_desc, 2 y3_pool_desc, 3 y3_detect_level, 4 y3_decode_desc, 5 y3_op, 6 y3_nms_params,
  * 7 y3_loss_desc, 8 y3_bn_act_desc, 9 y3_bn_bwd_desc, 10 y3_wgrad_desc, 11 y3_pack_item, 12 y3_letterbox_desc,
- * 13 y3_amax_desc, 14 y3_resize_item, 15 y3_augment_desc, 16 y3_jpeg_geom, 17 y3_jpeg_info, 18 y3_jpeg_desc. */
+ * 13 y3_amax_desc, 14 y3_resize_item, 15 y3_augment_desc, 16 y3_jpeg_geom, 17 y3_jpeg_info, 18 y3_jpeg_desc,
+ * 19 y3_halo_item. */
 int64_t y3_abi_sizeof(int32_t which);
 /* Programmatic dependent launch between consecutive kernels of a stream (on by default; env Y3_PDL=0 or on=0 turns it off).
  * Results are identical either way — only the launch boundaries overlap.  Returns the previous setting.  A tuning switch with
@@ -344,6 +345,23 @@ int y3_add_nhwc(const void* src, int32_t src_ld, int32_t src_coff, void* dst, in
  * NHWC buffer, column (c*3+kh)*3+kw; lets training run layer 0 as a 1x1 conv with the generic kernels */
 int y3_im2col_first(const void* in, int32_t in_dtype, float in_div, int32_t n, int32_t h, int32_t w, void* out,
                     int32_t out_ld, int32_t out_coff, y3_stream_t stream);
+/* y3_im2col_first of the [n,3,src_h,src_w] image rescaled to h x w: the multi-scale step of the reference's training loop,
+ * imgs.float() / 255 then F.interpolate(imgs, (h, w), mode="bilinear", align_corners=False), fused into layer 0's im2col.
+ * The arithmetic restates torch's CUDA upsample_bilinear2d with no scale factors given: scale = float(src) / dst, source
+ * index max(scale * (d + 0.5) - 0.5, 0), the +1 neighbour only inside the image.  Y3_IN_U8 with in_div > 0 multiplies
+ * each source byte by the fp32 reciprocal of in_div first, as torch's division by a CPU scalar does. */
+int y3_im2col_first_resize(const void* in, int32_t in_dtype, float in_div, int32_t n, int32_t src_h, int32_t src_w,
+                           int32_t h, int32_t w, void* out, int32_t out_ld, int32_t out_coff, y3_stream_t stream);
+/* Zeroes, for every item of a device-resident table, the one-pixel halo of a bf16 padded NHWC buffer [n, h+2, w+2, ld] and
+ * channels [c_lo, ld) of its interior (c_lo = ld: none).  Training engines of different batch shapes share one activation
+ * arena; an engine that takes the arena over from another restores with this one launch the zeros its kernels read. */
+typedef struct y3_halo_item {
+  void* p;
+  int32_t n, h, w, ld;
+  int32_t c_lo;
+  int32_t reserved;
+} y3_halo_item;
+int y3_zero_halo_batched(const y3_halo_item* items_dev, int32_t n_items, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Image pre-processing on the device (SURVEY §8(f) row f1): letterbox (utils/augmentations.py:104-134: cv2.resize

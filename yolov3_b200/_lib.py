@@ -202,6 +202,13 @@ class PackItem(C.Structure):
                 ("dst_co", C.c_int32), ("tile_begin", C.c_int32), ("reserved", C.c_int32)]
 
 
+class HaloItem(C.Structure):
+    """struct y3_halo_item."""
+
+    _fields_ = [("p", C.c_void_p), ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("ld", C.c_int32), ("c_lo", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
 JPEG_TABLE_BYTES = 6080
 
 
@@ -289,6 +296,8 @@ def _declare(lib):
         "y3_conv_wgrad": ([C.POINTER(WgradDesc), vp], C.c_int),
         "y3_add_nhwc": ([vp, i32, i32, vp, i32, i32, i32, i32, i32, i32, i32, vp], C.c_int),
         "y3_im2col_first": ([vp, i32, C.c_float, i32, i32, i32, vp, i32, i32, vp], C.c_int),
+        "y3_im2col_first_resize": ([vp, i32, C.c_float, i32, i32, i32, i32, i32, vp, i32, i32, vp], C.c_int),
+        "y3_zero_halo_batched": ([vp, i32, vp], C.c_int),
         "y3_box_iou": ([vp, i32, vp, i32, C.c_float, vp, vp], C.c_int),
         "y3_loss_workspace_bytes": ([C.POINTER(LossDesc)], C.c_int64),
         "y3_loss_fwd_bwd": ([C.POINTER(LossDesc), vp, C.c_int64, vp, vp], C.c_int),
@@ -330,7 +339,7 @@ def lib():
         SYMBOLS.update(_declare(_lib))
         for which, st in enumerate((ConvDesc, FirstDesc, PoolDesc, DetectLevel, DecodeDesc, Op, NmsParams, LossDesc, BnActDesc,
                                     BnBwdDesc, WgradDesc, PackItem, LetterboxDesc, AmaxDesc, ResizeItem,
-                                    AugmentDesc, JpegGeom, JpegInfo, JpegDesc)):
+                                    AugmentDesc, JpegGeom, JpegInfo, JpegDesc, HaloItem)):
             if _lib.y3_abi_sizeof(which) != C.sizeof(st):
                 raise Y3Error(f"ABI mismatch: sizeof({st.__name__}) is {C.sizeof(st)} here, "
                               f"{_lib.y3_abi_sizeof(which)} in {_LIB_PATH.name}; rebuild the library")

@@ -16,6 +16,8 @@ NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-
 # kernels whose arithmetic must match the reference bit for bit are compiled without fast-math / FMA contraction
 EXACT_SOURCES = {"y3_nms.cu", "y3_detect.cu", "y3_loss.cu", "y3_iou.cu", "y3_val.cu", "y3_tta.cu",
                  "y3_metrics.cu", "y3_augment.cu", "y3_jpeg.cu"}
+# kernels that restate one of torch's own CUDA kernels: compiled as torch compiles them, no fast math, FMA contraction on
+TORCH_SOURCES = {"y3_im2col_resize.cu"}
 
 
 def nvcc_path() -> str:
@@ -50,6 +52,8 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         flags = [f for f in NVCC_FLAGS if f != "-shared"]
         if src.name in EXACT_SOURCES:
             flags = [f for f in flags if f != "--use_fast_math"] + ["-fmad=false"]
+        elif src.name in TORCH_SOURCES:
+            flags = [f for f in flags if f != "--use_fast_math"]
         cmd = [nvcc, *flags, "-c", str(src), "-o", str(obj)]
         if verbose:
             print(" ".join(cmd))

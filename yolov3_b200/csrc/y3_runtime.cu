@@ -146,6 +146,7 @@ extern "C" int64_t y3_abi_sizeof(int32_t which) {
     case 16: return sizeof(y3_jpeg_geom);
     case 17: return sizeof(y3_jpeg_info);
     case 18: return sizeof(y3_jpeg_desc);
+    case 19: return sizeof(y3_halo_item);
   }
   return -1;
 }

@@ -568,6 +568,49 @@ __global__ void __launch_bounds__(256) im2col_first_kernel(const TIN* __restrict
   }
 }
 
+// ---------------------------------------------------------------------------------------------- arena halos
+// Item blockIdx.y: the 16-byte words of its one-pixel halo ring (all ld channels), then those of channels [c_lo, ld) of its
+// interior, grid-strided over blockIdx.x.
+__global__ void __launch_bounds__(256) zero_halo_batched_kernel(const y3_halo_item* __restrict__ items) {
+  pdl_entry();
+  const y3_halo_item it = items[blockIdx.y];
+  const int ld8 = it.ld / 8, up8 = (it.ld - it.c_lo) / 8, hp = it.h + 2, wp = it.w + 2;
+  const long long ring = 2ll * wp + 2ll * it.h;  // halo pixels of one image: top row, bottom row, two side columns
+  const long long halo = it.n * ring * ld8;
+  const long long total = halo + static_cast<long long>(it.n) * it.h * it.w * up8;
+  uint4* p = static_cast<uint4*>(it.p);
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    long long pix;
+    int cg;
+    if (i < halo) {
+      cg = static_cast<int>(i % ld8);
+      const long long t = i / ld8;
+      int r = static_cast<int>(t % ring), y, x;
+      const int b = static_cast<int>(t / ring);
+      if (r < wp) {
+        y = 0, x = r;
+      } else if (r < 2 * wp) {
+        y = hp - 1, x = r - wp;
+      } else {
+        r -= 2 * wp;
+        y = 1 + (r >> 1), x = (r & 1) ? wp - 1 : 0;
+      }
+      pix = (static_cast<long long>(b) * hp + y) * wp + x;
+    } else {
+      const long long j = i - halo;
+      cg = ld8 - up8 + static_cast<int>(j % up8);
+      long long t = j / up8;
+      const int x = static_cast<int>(t % it.w);
+      t /= it.w;
+      const int y = static_cast<int>(t % it.h);
+      const int b = static_cast<int>(t / it.h);
+      pix = (static_cast<long long>(b) * hp + y + 1) * wp + x + 1;
+    }
+    p[pix * ld8 + cg] = make_uint4(0u, 0u, 0u, 0u);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------- batched weight packs
 // The fp32 master weights live in ONE flat buffer, every conv weight stored [co][kh][kw][ci] (PyTorch channels_last
 // strides of the [co,ci,k,k] parameter) — which IS the forward pack's order.  Per optimizer step the whole buffer is
@@ -872,6 +915,13 @@ extern "C" int y3_im2col_first(const void* in, int32_t in_dtype, float in_div, i
     Y3_CHECK_CUDA(::y3::launch_pdl(y3::im2col_first_kernel<uint8_t>, dim3(y3::grid_for(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), static_cast<const uint8_t*>(in), in_div, n, h, w, o));
   else
     Y3_CHECK_CUDA(::y3::launch_pdl(y3::im2col_first_kernel<float>, dim3(y3::grid_for(total)), dim3(256), 0, static_cast<cudaStream_t>(stream), static_cast<const float*>(in), in_div, n, h, w, o));
+  Y3_CHECK_CUDA(cudaGetLastError());
+  return Y3_OK;
+}
+
+extern "C" int y3_zero_halo_batched(const y3_halo_item* items_dev, int32_t n_items, y3_stream_t stream) {
+  Y3_REQUIRE(items_dev && n_items > 0 && n_items <= 65535, "zero_halo_batched: bad arguments");
+  Y3_CHECK_CUDA(::y3::launch_pdl(y3::zero_halo_batched_kernel, dim3(32, n_items), dim3(256), 0, static_cast<cudaStream_t>(stream), items_dev));
   Y3_CHECK_CUDA(cudaGetLastError());
   return Y3_OK;
 }

@@ -15,6 +15,7 @@ FP8 inference is opt-in: ``calibrate_fp8(batches)`` records one activation scale
 from __future__ import annotations
 
 import ctypes as C
+import gc
 import math
 from collections import OrderedDict
 from copy import deepcopy
@@ -97,7 +98,9 @@ class Model:
         self._packed = None
         self._engines: "OrderedDict" = OrderedDict()  # LRU over input shapes, at most MAX_ENGINES alive
         self.ddp = None  # parallel.DDP(model): overlapped gradient exchange
-        self._train_engines: dict = {}
+        self._train_engines: dict = {}  # (n, h, w) -> TrainEngine, every one on ``_arena``
+        self._arena = None   # train.Arena: the activation memory the training engines of every batch shape share
+        self._train_packs = None  # the training engines' shape-independent dgrad packs (train._shared_packs)
         self._precision = "bf16"
         self._fp8_scales = None  # {tensor name: scale} from calibrate_fp8 / load_fp8_scales
         self._built = self.weights_version()  # what the packs, the FP8 calibration and the engines were made from
@@ -366,8 +369,39 @@ class Model:
             self._engines.move_to_end(key)
         return e
 
-    def forward(self, x, augment=False, profile=False, visualize=False):
-        """Eval-mode Model.forward (models/yolo.py:233-237): returns (z[bs, rows, no], [p_i[bs,na,ny,nx,no]])."""
+    def train_engine(self, n, h, w) -> "TrainEngine":
+        """The training engine of one batch shape.  Engines are kept per shape and share one activation arena, which grows to
+        the largest shape requested; growing drops the cached engines (their graphs hold the old addresses)."""
+        from .train import Arena, TrainEngine
+
+        te = self._train_engines.get((n, h, w))
+        if te is None:
+            if self._arena is None:
+                self._arena = Arena(self.device, on_grow=self._drop_train_engines)
+            te = self._train_engines[(n, h, w)] = TrainEngine(self, n, h, w, arena=self._arena)
+        return te
+
+    def _drop_train_engines(self):
+        self._train_engines.clear()
+        gc.collect()  # an engine's launch closures refer back to it: only the collector frees its views of the arena
+
+    def _train_size(self, size, h, w):
+        """(h, w) of ``forward(x, size=...)``: an int or an (h, w) pair, each a multiple of the largest stride."""
+        if size is None:
+            return h, w
+        hs, ws = (size, size) if isinstance(size, int) else (int(size[0]), int(size[1]))
+        gs = int(self.stride.max())
+        if hs <= 0 or ws <= 0 or hs % gs or ws % gs:
+            raise ValueError(f"size={size!r}: the rescaled batch must be a positive multiple of the largest stride ({gs})")
+        return hs, ws
+
+    def forward(self, x, augment=False, profile=False, visualize=False, size=None):
+        """Eval-mode Model.forward (models/yolo.py:233-237): returns (z[bs, rows, no], [p_i[bs,na,ny,nx,no]]).
+        Train mode returns the raw maps; ``size=(h, w)`` (or an int) rescales the batch bilinearly to that size on the way
+        into layer 0, fusing train.py's ``--multi-scale`` ``F.interpolate(imgs, size=ns, mode="bilinear",
+        align_corners=False)``: pass the loader's uint8 batch, the ``/ 255`` is applied as the reference does."""
+        if size is not None and not self.training:
+            raise ValueError("size= rescales a training batch (train.py --multi-scale); eval-mode forward takes no size")
         if profile or visualize:
             raise NotImplementedError("profile/visualize are outside the accelerated path (SURVEY §8a)")
         if not x.is_cuda:
@@ -385,12 +419,9 @@ class Model:
         assert c == self.ch, f"expected {self.ch} input channels"
         if self.training:
             # train mode (models/yolo.py:110 returns the raw maps): BatchNorm batch statistics, autograd-connected
-            from .train import TrainEngine, TrainFn
+            from .train import TrainFn
 
-            te = self._train_engines.get((n, h, w))
-            if te is None:
-                self._train_engines.clear()
-                te = self._train_engines[(n, h, w)] = TrainEngine(self, n, h, w)
+            te = self.train_engine(n, *self._train_size(size, h, w))
             P = self.device_params()
             return list(TrainFn.apply(te, x, 255.0 if x.dtype == torch.uint8 else 0.0, *[P[k] for k in te.param_names]))
         e = self.engine(n, h, w, x.dtype, 255.0 if x.dtype == torch.uint8 else 0.0)  # uint8 images: im/255

@@ -131,14 +131,17 @@ class DetectionModel(nn.Module):
     def device(self):
         return self.core.device
 
-    def forward(self, x, augment=False, profile=False, visualize=False):
+    def forward(self, x, augment=False, profile=False, visualize=False, size=None):
+        """``size``: train mode only, see ``Model.forward`` (the fused ``--multi-scale`` rescale)."""
         core = self.core
         core.hyp, core.names = self.hyp, self.names
         if x.dtype == torch.float16:
             x = x.float()
         if self.training:
             core.training = True
-            return core.forward(x)
+            return core.forward(x, size=size)
+        if size is not None:
+            raise ValueError("size= rescales a training batch (train.py --multi-scale); eval-mode forward takes no size")
         core.training = False
         y = core.forward(x, augment=augment, profile=profile, visualize=visualize)
         if self._out_dtype != torch.float32:

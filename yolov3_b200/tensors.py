@@ -29,7 +29,7 @@ class PaddedNHWC:
     __slots__ = ("buf", "coff", "c", "scale")
 
     def __init__(self, buf: torch.Tensor, coff: int = 0, c: int | None = None, scale: float = 1.0):
-        assert buf.dtype in DTYPES and buf.dim() == 4 and buf.is_contiguous() and (buf.is_cuda or DRY_RUN)
+        assert buf.dtype in DTYPES and buf.dim() == 4 and buf.is_contiguous() and (buf.is_cuda or buf.is_meta or DRY_RUN)
         self.buf, self.coff = buf, coff
         self.c = buf.shape[3] - coff if c is None else c
         self.scale = float(scale)

@@ -27,6 +27,8 @@ graphs and write every tensor to the same place.
 from __future__ import annotations
 
 import ctypes as C
+import weakref
+from collections import OrderedDict
 
 import torch
 import torch.distributed as dist
@@ -45,44 +47,168 @@ class _Block:
     """One Conv+BN+SiLU block (models/common.py:57-81) with everything its forward and backward need."""
 
     __slots__ = ("prefix", "c1", "c2", "k", "s", "x", "y", "a", "res", "upsample", "wf", "wd", "st", "dw", "first", "dy",
-                 "post_fwd", "pre_bwd", "gamma", "beta", "rmean", "rvar", "dgamma", "dbeta", "nblk")
+                 "post_fwd", "pre_bwd", "gamma", "beta", "rmean", "rvar", "dgamma", "dbeta", "nblk", "count")
+
+
+def gather_shapes(n: int, h: int, w: int) -> list[tuple[int, int, int]]:
+    """(n, h, w) of every rank's batch, in rank order: one all-gather.  Under ``--multi-scale`` each rank draws its own size
+    (the reference seeds every rank differently, train.py's ``init_seeds(opt.seed + 1 + RANK)``)."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend() == "nccl" else torch.device("cpu")
+    mine = torch.tensor([n, h, w], dtype=torch.int64, device=dev)
+    out = [torch.empty_like(mine) for _ in range(dist.get_world_size())]
+    dist.all_gather(out, mine)
+    return [tuple(int(v) for v in t.tolist()) for t in out]
+
+
+def bn_counts(shapes, h: int, w: int, grids) -> list[float]:
+    """Pixels each BatchNorm normalises over all ranks, as nn.SyncBatchNorm's all-gathered counts give them: a layer whose
+    output grid is (gh, gw) at this rank's input (h, w) covers n_r * (gh * h_r / h) * (gw * w_r / w) pixels of rank r
+    (every size is a multiple of the model's strides, so the divisions are exact)."""
+    return [float(sum(nr * (gh * hr // h) * (gw * wr // w) for nr, hr, wr in shapes)) for gh, gw in grids]
+
+
+def _shared_packs(model, te) -> dict:
+    """The dgrad pack of every conv (``wd``: its transposed, tap-flipped bf16 weight), the table that re-packs them all in
+    one launch (y3_pack_dgrad_batched) and the zero bias of the identity-epilogue convs.  None of them depends on the batch
+    shape: the model holds one copy for its engines of every shape, made from the first engine's lowering."""
+    sh = model._train_packs
+    if sh is not None:
+        return sh
+    dev, store = model.device, model.store()
+    head_ld = ops.cout_pad(model.detect.na * model.detect.no)
+    wd, items, tile = {}, [], 0
+    for hd in te.heads:
+        s = store.slots[hd["wname"]]
+        wd[hd["wname"]] = torch.zeros(ops.cout_pad(hd["c1"]), head_ld, dtype=torch.bfloat16, device=dev)
+        items.append((s.offset, wd[hd["wname"]], s.rows, s.ci, 1, head_ld))
+    for b in te.blocks:
+        if not b.first:
+            s = store.slots[b.prefix + ".conv.weight"]
+            wd[b.prefix] = torch.zeros(ops.cout_pad(b.c1), b.k * b.k * b.c2, dtype=torch.bfloat16, device=dev)
+            items.append((s.offset, wd[b.prefix], s.rows, s.ci, b.k, b.c2))
+    arr = (_lib.PackItem * len(items))()
+    for i, (off, dst, rows, ci, k, dst_co) in enumerate(items):
+        it = arr[i]
+        rows = min(rows, dst_co)
+        it.src_off, it.dst, it.co_rows, it.ci, it.k, it.dst_co, it.tile_begin = off, dst.data_ptr(), rows, ci, k, dst_co, tile
+        tile += k * k * ((rows + 31) // 32) * ((ci + 31) // 32)
+    model._train_packs = dict(wd=wd, items=torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev),
+                              n_items=len(items), tiles=tile, zero_bias=torch.zeros(4096, dtype=torch.float32, device=dev))
+    return model._train_packs
+
+
+class Arena:
+    """One device allocation that the training engines of every batch shape of a model take their shape-dependent buffers
+    from (activations, Concat buffers, dy scratch, activation gradients, pool argmax, head out / raw / dy, partial sums), in
+    a fixed order through a 256-byte aligned bump allocator.  Engines of different shapes alias the same bytes, so a
+    multi-scale run holds the largest shape's activations, not the sum over its shapes.
+
+    ``grow`` reallocates: ``on_grow`` first drops every engine built on the old bytes (they hold their pointers in CUDA
+    graphs and TMA descriptors), so the old bytes are free before the new ones are taken.  ``owner`` is the engine whose
+    buffers the bytes hold (None: fresh zeros); ``fwd_gen`` counts the forwards of all its engines, so a backward must belong
+    to the arena's last forward.  ``slots`` holds the forward graphs' input buffers, one per input shape and dtype, shared
+    by every engine; a slot lives as long as a captured graph reads it."""
+
+    ALIGN = 256
+
+    def __init__(self, device, on_grow=None):
+        self.device = torch.device(device)
+        self.buf = torch.zeros(0, dtype=torch.uint8, device=self.device)
+        self.on_grow = on_grow
+        self.owner = None
+        self.fwd_gen = 0
+        self.slots = weakref.WeakValueDictionary()
+
+    @property
+    def nbytes(self) -> int:
+        return self.buf.numel()
+
+    def grow(self, nbytes: int):
+        if self.on_grow is not None:
+            self.on_grow()
+        self.buf = torch.zeros(0, dtype=torch.uint8, device=self.device)
+        if self.device.type == "cuda":
+            torch.cuda.empty_cache()  # hand the old arena's block back: the larger one may need its bytes
+        self.buf = torch.zeros(nbytes, dtype=torch.uint8, device=self.device)
+        self.owner = None
+
+    def slot(self, x: torch.Tensor) -> torch.Tensor:
+        key = (tuple(x.shape), x.dtype)
+        t = self.slots.get(key)
+        if t is None:
+            t = self.slots[key] = torch.empty_like(x)
+        return t
 
 
 class TrainEngine:
     use_graphs = True        # replay forward / backward segments as CUDA graphs after one eager warm-up step
     deterministic = False    # True: wgrad without split-K (bit-reproducible steps; slower on the early layers)
     n_buckets = 4            # gradient ranges all-reduced separately, each as soon as its layers are done
+    MAX_FWD_GRAPHS = 4       # forward graphs kept per engine, one per input shape fed to it (rect batches rescaled to it)
 
-    def __init__(self, model, n, h, w, keep_all=False):
+    def __init__(self, model, n, h, w, keep_all=False, arena=None):
         """keep_all=True gives every block its own dy buffer (per-layer gradient checks in the tests); the default shares
-        one scratch buffer per shape."""
-        dev = model.device
+        one scratch buffer per shape.  ``arena``: where the shape-dependent buffers live (``Model`` passes the one its
+        engines of every shape share); None gives the engine an arena of its own."""
         self.model, self.n, self.h, self.w = model, n, h, w
-        det = model.detect
-        plan = graph.lower(model.nodes, model.ch, h, w)
-        self.fwd_gen = 0  # activations live in this engine's buffers: a backward must belong to the LAST forward
-        store = model.store()
-        self.store = store
+        self.keep_all = keep_all
+        self.arena = Arena(model.device) if arena is None else arena
+        self.store = model.store()
         self.P = model.device_params()
         self.world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
         self.sync_bn = bool(getattr(model, "sync_bn", False)) and self.world > 1
         if self.sync_bn:
             self.use_graphs = False  # the per-layer collectives stay eager launches
+        self._measure = True  # the first pass only measures: it holds no byte of an arena that is about to grow
+        self._lower()
+        if self._top > self.arena.nbytes:
+            self.arena.grow(self._top)
+        self._measure = False
+        self._lower()
+        self.comm = None          # side stream of the gradient exchange (parallel.DDP)
+        self._graphs: dict = {}   # "fwd": the forward graph of the last input, ("bwd", i): backward segments, "bwd_in"
+        self._fwd_graphs: OrderedDict = OrderedDict()  # input signature -> forward graph state, least recently used first
+
+    def _take(self, shape, dtype) -> torch.Tensor:
+        """The next buffer of the arena (a meta tensor in the measuring pass)."""
+        off = self._top
+        nbytes = torch.Size(shape).numel() * dtype.itemsize
+        self._top += (nbytes + Arena.ALIGN - 1) // Arena.ALIGN * Arena.ALIGN
+        if self._measure:
+            return torch.empty(shape, dtype=dtype, device="meta")
+        assert self._top <= self.arena.nbytes
+        return self.arena.buf[off:off + nbytes].view(dtype).view(shape)
+
+    def _lower(self):
+        model, n, h, w = self.model, self.n, self.h, self.w
+        dev = model.device
+        det = model.detect
+        store = self.store
+        plan = graph.lower(model.nodes, model.ch, h, w)
+        self._top = 0
         self.blocks: list[_Block] = []
         self.keep = []
-        self.grad_bufs: dict[int, PaddedNHWC] = {}
         self.pools: list[dict] = []  # one record per max-pool: its wiring, for the tests (the launches are closures)
         self.scratch: dict[tuple, PaddedNHWC] = {}
-        self.keep_all = keep_all
-        self.zero_bias = torch.zeros(4096, dtype=torch.float32, device=dev)  # identity-epilogue convs (forward and dgrad)
+        padded = []  # (buffer, channels in use): the table of y3_zero_halo_batched
+        with_grad = {}  # id(buffer) -> buffer, for every activation buffer a backward writes the gradient of
         max_partial = 0
+
+        def pad(c, hh, ww, ld):
+            b = PaddedNHWC(self._take((n, hh + 2, ww + 2, ld), torch.bfloat16), 0, c)
+            padded.append((b.buf, c if c < ld else ld))
+            return b
 
         def buf(c, hh, ww, ld=None):
             # the conv kernel produces multiples of 32 output channels: a 16-channel tensor (yolov3-tiny layers 0-2) lives in a
             # 32-channel buffer whose upper half stays zero (zero weight rows / zero dgrad rows), everything else sees c = 16
-            b = PaddedNHWC.zeros(n, hh, ww, c, device=dev, ld=max(ld or c, 32))
+            b = pad(c, hh, ww, max(ld or c, 32))
             self.keep.append(b)
             return b
+
+        def grad(*ts):
+            for t in ts:
+                with_grad[id(t.buf)] = t.buf
 
         def f32(c):
             t = torch.zeros(c, dtype=torch.float32, device=dev)
@@ -95,10 +221,11 @@ class TrainEngine:
             c1, k, s = (32, 1, 1) if first else (cb.c1, cb.k, cb.s)  # layer 0 = 1x1 conv over the im2col
             b = _Block()
             b.prefix, b.c1, b.c2, b.k, b.s, b.x, b.a, b.res, b.upsample, b.first = prefix, c1, c2, k, s, x, a, res, upsample, first
+            grad(a) if first else grad(a, x)
             ho, wo = x.h // s, x.w // s
             b.y = buf(c2, ho, wo)
             b.wf = store.weight_rows_bf16(prefix + ".conv.weight")
-            b.wd = None if first else torch.zeros(ops.cout_pad(c1), k * k * c2, dtype=torch.bfloat16, device=dev)
+            b.wd = None
             b.dw = store.grad_rows(prefix + ".conv.weight")
             b.gamma, b.beta = store.flat(prefix + ".bn.weight"), store.flat(prefix + ".bn.bias")
             b.dgamma, b.dbeta = store.flat(prefix + ".bn.weight", grad=True), store.flat(prefix + ".bn.bias", grad=True)
@@ -106,8 +233,9 @@ class TrainEngine:
             b.st = {name: f32(c2) for name in ("scale", "shift", "mean", "rstd")}
             b.st.update(sums=f32(2 * c2), gsums=f32(2 * c2))  # [sum | sumsq] forward, [sum dz | sum dz*xhat] backward
             b.nblk = T.partial_blocks(n, ho, wo, c2)
+            b.count = float(n * ho * wo)
             max_partial = max(max_partial, b.nblk * 2 * c2)
-            b.dy = buf(c2, ho, wo) if keep_all else self._scratch(c2, ho, wo, dev)
+            b.dy = buf(c2, ho, wo) if self.keep_all else self._scratch(c2, ho, wo, pad)
             b.post_fwd, b.pre_bwd = [], []  # extra launches after this block's forward / before its backward (SPP pools)
             self.blocks.append(b)
             return b
@@ -148,9 +276,10 @@ class TrainEngine:
                 cat = buf(cv2.c1, ly.h, ly.w)
                 b1 = new_block(cv1, x, cat.slice(0, c_))
                 for q, k in enumerate(cv1.ks):
-                    idx = torch.zeros(n * ly.h * ly.w * c_, dtype=torch.uint8, device=dev)
+                    idx = self._take((n * ly.h * ly.w * c_,), torch.uint8)
                     self.keep.append(idx)
                     src, dst = cat.slice(0, c_), cat.slice((q + 1) * c_, c_)
+                    grad(src, dst)
                     self.pools.append(dict(src=src, dst=dst, k=k, stride=1, off=-(k // 2), oob_zero=False))
                     b1.post_fwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_train_fwd(src, dst, k, idx))
                     b1.pre_bwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_bwd(self.grad_of(dst), self.grad_of(src),
@@ -164,8 +293,9 @@ class TrainEngine:
                 p = ly.pool
                 x = tens[p.src]
                 y = out_of(ly)
-                idx = torch.zeros(n * y.h * y.w * x.c, dtype=torch.uint8, device=dev)
+                idx = self._take((n * y.h * y.w * x.c,), torch.uint8)
                 self.keep.append(idx)
+                grad(x, y)
                 self.pools.append(dict(src=x, dst=y, k=p.k, stride=p.s, off=-p.pad, oob_zero=p.oob_zero))
                 host = self.blocks[-1]  # the pool runs after the latest block's forward and before that block's backward
                 host.post_fwd.append(lambda x=x, y=y, p=p, idx=idx:
@@ -179,12 +309,13 @@ class TrainEngine:
         dec = _lib.DecodeDesc()
         for j, ph in enumerate(plan.heads):
             x = tens[ph.src]
+            grad(x)
             wname, bname = f"model.{det.i}.m.{j}.weight", f"model.{det.i}.m.{j}.bias"
             hd = dict(x=x, c1=x.c, j=j, wname=wname, bname=bname)
-            hd["out"] = torch.zeros(n * x.h * x.w, head_ld, dtype=torch.float32, device=dev)
-            hd["raw"] = torch.zeros(n, det.na, x.h, x.w, det.no, dtype=torch.float32, device=dev)
+            hd["out"] = self._take((n * x.h * x.w, head_ld), torch.float32)
+            hd["raw"] = self._take((n, det.na, x.h, x.w, det.no), torch.float32)
+            hd["graw"] = self._take((n, det.na, x.h, x.w, det.no), torch.float32)  # dL/draw input of the backward graph
             hd["wf"] = store.weight_rows_bf16(wname)                   # [head_ld, c1]: rows >= na*no are the slot's zero pad rows
-            hd["wd"] = torch.zeros(ops.cout_pad(x.c), head_ld, dtype=torch.bfloat16, device=dev)
             hd["bias"] = store.flat(bname, padded=True)[:head_ld]      # fp32 master bias read in place (pad entry = 0)
             hd["dy"] = buf(head_ld, x.h, x.w)
             hd["dw"] = store.grad_rows(wname)                          # [head_ld, 1, c1]
@@ -200,25 +331,32 @@ class TrainEngine:
         dec.nl, dec.bs, dec.na, dec.no, dec.z = det.nl, n, det.na, det.no, None
         self.dec = dec
         self.err = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.partial = torch.zeros(max_partial, dtype=torch.float32, device=dev)  # first-stage rows of every reduction
+        self.partial = self._take((max_partial,), torch.float32)  # first-stage rows of every reduction
 
-        # ---- one table for the batched dgrad re-pack (y3_pack_dgrad_batched)
-        items, tile = [], 0
-        for hd in self.heads:
-            s = store.slots[hd["wname"]]
-            items.append((s.offset, hd["wd"], s.rows, s.ci, 1, head_ld))
+        # ---- one gradient buffer per activation buffer that receives a gradient (same geometry, same channel use)
+        self.grad_bufs: dict[int, PaddedNHWC] = {}
+        for t in with_grad.values():
+            g = pad(t.shape[3], t.shape[1] - 2, t.shape[2] - 2, t.shape[3])
+            self.grad_bufs[t.data_ptr()] = g
+            padded[-1] = (g.buf, next(c for b, c in padded if b is t))
+
+        # ---- dgrad packs, the batched re-pack table and the zero bias: shape-independent, held once per model
+        shared = _shared_packs(model, self)
+        self.pack_items, self.n_pack_items, self.pack_tiles = shared["items"], shared["n_items"], shared["tiles"]
+        self.zero_bias = shared["zero_bias"]  # identity-epilogue convs (forward and dgrad)
         for b in self.blocks:
-            if b.wd is not None:
-                s = store.slots[b.prefix + ".conv.weight"]
-                items.append((s.offset, b.wd, s.rows, s.ci, b.k, b.c2))
-        arr = (_lib.PackItem * len(items))()
-        for i, (off, dst, rows, ci, k, dst_co) in enumerate(items):
+            b.wd = shared["wd"].get(b.prefix)
+        for hd in self.heads:
+            hd["wd"] = shared["wd"][hd["wname"]]
+
+        # ---- the zeros every kernel reads: halos of every padded buffer, upper halves of 16-in-32 buffers
+        arr = (_lib.HaloItem * len(padded))()
+        for i, (t, c_lo) in enumerate(padded):
+            assert c_lo % 8 == 0 and t.shape[3] % 8 == 0
             it = arr[i]
-            rows = min(rows, dst_co)
-            it.src_off, it.dst, it.co_rows, it.ci, it.k, it.dst_co, it.tile_begin = off, dst.data_ptr(), rows, ci, k, dst_co, tile
-            tile += k * k * ((rows + 31) // 32) * ((ci + 31) // 32)
-        self.pack_items = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
-        self.n_pack_items, self.pack_tiles = len(items), tile
+            it.p, it.n, it.h, it.w, it.ld, it.c_lo = t.data_ptr(), t.shape[0], t.shape[1] - 2, t.shape[2] - 2, t.shape[3], c_lo
+        self.halo_items = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(dev)
+        self.n_halo = len(padded)
 
         self.param_names = []
         for b in self.blocks:
@@ -236,23 +374,17 @@ class TrainEngine:
             while off >= ends[si]:
                 si += 1
             self.segments[si].append(b)
-        self.comm = None          # side stream of the gradient exchange (parallel.DDP)
-        self._graphs: dict = {}
 
     # ------------------------------------------------------------------------------------------------ helpers
-    def _scratch(self, c, hh, ww, dev):
+    def _scratch(self, c, hh, ww, pad):
         key = (c, hh, ww)
         if key not in self.scratch:
-            self.scratch[key] = PaddedNHWC.zeros(self.n, hh, ww, c, device=dev)
+            self.scratch[key] = pad(c, hh, ww, c)
         return self.scratch[key]
 
     def grad_of(self, t: PaddedNHWC) -> PaddedNHWC:
         """Gradient buffer mirroring an activation buffer (same geometry, same channel slice)."""
-        key = t.buf.data_ptr()
-        g = self.grad_bufs.get(key)
-        if g is None:
-            g = self.grad_bufs[key] = PaddedNHWC(torch.zeros_like(t.buf), 0, t.buf.shape[3])
-        return g.slice(t.coff, t.c)
+        return self.grad_bufs[t.buf.data_ptr()].slice(t.coff, t.c)
 
     def _run(self, key, fn):
         """Run ``fn`` eagerly the first time (function attributes, lazy allocations), capture AND replay it the second time,
@@ -274,23 +406,41 @@ class TrainEngine:
         return st["out"]
 
     # ------------------------------------------------------------------------------------------------ forward
+    @property
+    def fwd_gen(self):
+        """Forwards run on this engine's arena so far: a backward must belong to the arena's LAST forward."""
+        return self.arena.fwd_gen
+
     def forward(self, x: torch.Tensor, in_div=0.0):
-        self.fwd_gen += 1
+        """x: the batch at (h, w), or at any other size to be rescaled to (h, w) on the way into layer 0."""
+        ar = self.arena
+        ar.fwd_gen += 1
+        if ar.owner is not self:
+            if ar.owner is not None:  # another shape's engine ran last: its interiors overlap this engine's zero regions
+                T.zero_halo_batched(self.halo_items, self.n_halo)
+            ar.owner = self
         self.store.mark_written()  # bn_finalize updates the running statistics inside P
         if not self.use_graphs:
             return self._forward_impl(x, in_div)
-        st = self._graphs.setdefault("fwd", {"n": 0})
+        sig = (tuple(x.shape), x.dtype, float(in_div))
+        st = self._fwd_graphs.get(sig)
+        if st is None:
+            st = self._fwd_graphs[sig] = {"n": 0}
+            while len(self._fwd_graphs) > self.MAX_FWD_GRAPHS:
+                self._fwd_graphs.popitem(last=False)
+        else:
+            self._fwd_graphs.move_to_end(sig)
+        self._graphs["fwd"] = st
         if st["n"] == 0:
             st["n"] = 1
             return self._forward_impl(x, in_div)
         if "graph" not in st:
-            st["x"], st["div"] = x.clone(), in_div
+            st["x"] = ar.slot(x)  # shared by the engines of every size that read the same input shape
             torch.cuda.synchronize()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 st["out"] = self._forward_impl(st["x"], in_div)
             st["graph"] = g
-        assert in_div == st["div"] and x.shape == st["x"].shape and x.dtype == st["x"].dtype
         st["x"].copy_(x)
         st["graph"].replay()
         return st["out"]
@@ -304,20 +454,26 @@ class TrainEngine:
     def _forward_impl(self, x: torch.Tensor, in_div=0.0):
         det = self.model.detect
         self.refresh_packs()
-        T.im2col_first(x, self.im2col, in_div)
+        if tuple(x.shape[2:]) == (self.h, self.w):
+            T.im2col_first(x, self.im2col, in_div)
+        else:
+            T.im2col_first_resize(x, self.im2col, in_div)
         zb = self.zero_bias
+        if self.sync_bn:  # ranks may run different shapes (--multi-scale draws per rank): count every rank's pixels
+            grids = [(b.y.h, b.y.w) for b in self.blocks]
+            for b, c in zip(self.blocks, bn_counts(gather_shapes(self.n, self.h, self.w), self.h, self.w, grids)):
+                b.count = c
         for b in self.blocks:
             ops.conv_bn_act(b.x, b.wf, zb, max(b.c2, 32), b.k, b.s, ops.ACT_NONE, out=_wide(b.y), err=self.err)
             st = b.st
             T.bn_stats(b.y, self.partial)
-            count = self.n * b.y.h * b.y.w
             if self.sync_bn:  # nn.SyncBatchNorm (train.py:270-272): batch statistics over every rank's pixels
                 T.colreduce(self.partial, b.nblk, 2 * b.c2, st["sums"])
                 dist.all_reduce(st["sums"])  # [sum | sumsq] share one buffer: one collective per layer
-                T.bn_finalize(st["sums"], 1, b.gamma, b.beta, count * self.world, st["scale"], st["shift"], st["mean"],
-                              st["rstd"], b.rmean, b.rvar)
+                T.bn_finalize(st["sums"], 1, b.gamma, b.beta, b.count, st["scale"], st["shift"], st["mean"], st["rstd"],
+                              b.rmean, b.rvar)
             else:
-                T.bn_finalize(self.partial, b.nblk, b.gamma, b.beta, count, st["scale"], st["shift"], st["mean"], st["rstd"],
+                T.bn_finalize(self.partial, b.nblk, b.gamma, b.beta, b.count, st["scale"], st["shift"], st["mean"], st["rstd"],
                               b.rmean, b.rvar)
             T.bn_act_fwd(b.y, st["scale"], st["shift"], b.a, b.res, b.upsample)
             for fn in b.post_fwd:
@@ -344,9 +500,7 @@ class TrainEngine:
             self.comm = torch.cuda.Stream(device=self.model.device, priority=-1)
         main = torch.cuda.current_stream()
         if self.use_graphs:
-            st = self._graphs.setdefault("bwd_in", {})
-            if "g" not in st:
-                st["g"] = [g.detach().float().contiguous().clone() for g in graws]
+            st = self._graphs.setdefault("bwd_in", {"g": [hd["graw"] for hd in self.heads]})
             for dst, src in zip(st["g"], graws):
                 dst.copy_(src)
             graws = st["g"]
@@ -425,8 +579,7 @@ class TrainEngine:
                 T.bn_act_bwd(b.y, da, b.dy, st, st["sums"], self.partial, b.dbeta, b.dgamma, b.upsample, phase=1)
                 st["gsums"].copy_(st["sums"])
                 dist.all_reduce(st["gsums"])
-                T.bn_act_bwd(b.y, da, b.dy, st, st["gsums"], None, None, None, b.upsample, phase=2,
-                             count=self.n * b.y.h * b.y.w * self.world)
+                T.bn_act_bwd(b.y, da, b.dy, st, st["gsums"], None, None, None, b.upsample, phase=2, count=b.count)
             else:
                 T.bn_act_bwd(b.y, da, b.dy, st, st["sums"], self.partial, b.dbeta, b.dgamma, b.upsample)
             T.conv_wgrad(b.dy, b.x, b.dw, b.k, accumulate=True, deterministic=det_flag, stride=b.s)
@@ -473,7 +626,8 @@ class TrainFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, *graws):
         if ctx.gen != ctx.engine.fwd_gen:
-            raise RuntimeError("backward() of a train-mode forward whose activations were overwritten by a later forward of the "
-                               "same shape: call loss.backward() before the next model(imgs) (one forward in flight per shape)")
+            raise RuntimeError("backward() of a train-mode forward whose activations were overwritten by a later forward (the "
+                               "engines of every batch shape share one activation arena): call loss.backward() before the "
+                               "next model(imgs) (one forward in flight per model)")
         ctx.engine.backward(graws)
         return (None, None, None) + (None,) * ctx.n_params

@@ -136,6 +136,22 @@ def im2col_first(x: torch.Tensor, out: PaddedNHWC, in_div=0.0):
     return out
 
 
+def im2col_first_resize(x: torch.Tensor, out: PaddedNHWC, in_div=0.0):
+    """``im2col_first`` of ``x`` bilinearly rescaled to ``out``'s (h, w): equals
+    ``im2col_first(F.interpolate(x.float() / in_div, (h, w), mode="bilinear", align_corners=False))`` within one bf16 step."""
+    assert x.is_cuda and x.is_contiguous() and x.shape[1] == 3 and x.dtype in (torch.float32, torch.uint8) and out.c == 32
+    n, _, sh, sw = x.shape
+    _lib.check(_lib.lib().y3_im2col_first_resize(x.data_ptr(), _lib.IN_U8 if x.dtype == torch.uint8 else _lib.IN_F32,
+                                                 float(in_div), n, sh, sw, out.h, out.w, out.ptr, out.ld, out.coff, _stream()),
+               "y3_im2col_first_resize")
+    return out
+
+
+def zero_halo_batched(items_dev: torch.Tensor, n_items: int):
+    """One launch: for each ``y3_halo_item`` of the device table, zero a padded NHWC buffer's halo and upper channels."""
+    _lib.check(_lib.lib().y3_zero_halo_batched(items_dev.data_ptr(), int(n_items), _stream()), "y3_zero_halo_batched")
+
+
 def maxpool_train_fwd(x: PaddedNHWC, out: PaddedNHWC, k: int, idx: torch.Tensor, stride: int = 1, off: int | None = None,
                       oob_zero: bool = False):
     """Max-pool that also records the argmax idx[n,ho,wo,c] uint8 for the backward.  Default: the stride-1 'same' pools of SPP;
