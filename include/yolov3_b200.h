@@ -556,14 +556,16 @@ int y3_ap_per_class(const float* conf, const float* cls, const uint8_t* tp, cons
  * Optimizer step over ONE flat fp32 parameter buffer (train.py:411-421: clip_grad_norm_(10.0), SGD-nesterov with the three
  * parameter groups of smart_optimizer utils/torch_utils.py:207-237, ModelEMA.update) — csrc/y3_optim.cu.
  * Layout contract: every parameter occupies a slot whose length is a multiple of 256 elements; group[i] is the group of
- * elements [256 i, 256 i + 256): 0 = weights with decay, 1 = BatchNorm weights, 2 = biases, >= 3 = not trained (buffers).
+ * elements [256 i, 256 i + 256): 0 = weights with decay, 1 = BatchNorm weights, 2 = biases, >= 3 = not trained (buffers,
+ * and frozen parameters: requires_grad False).
  * hp_dev: DEVICE float[11] = lr[3], weight_decay[3], momentum, nesterov, max_norm (0: no clipping), ema decay of this
  * update, gradient pre-scale (1/world_size after a SUM all-reduce) — read at run time, so the launches can sit in a CUDA
  * graph while the scheduler changes them.
  */
 int32_t y3_sumsq_blocks(void);  /* floats of workspace y3_grad_sumsq needs */
-/* out[0] = sum g[i]^2 (two-stage, fixed order: bit-reproducible); n % 4 == 0 */
-int y3_grad_sumsq(const float* g, int64_t n, float* partial, float* out, y3_stream_t stream);
+/* out[0] = sum g[i]^2 (two-stage, fixed order: bit-reproducible); n % 4 == 0.  group (optional, then n % 256 == 0): only the
+ * elements whose group is < 3 count */
+int y3_grad_sumsq(const float* g, const uint8_t* group, int64_t n, float* partial, float* out, y3_stream_t stream);
 /* p, m (momentum buffer, zero-initialised), ema (optional) updated in place from g; gsumsq (from y3_grad_sumsq) is read
  * only when hp_dev[8] > 0.  n = elements of p (and of ema); g and m are only touched where group < 3. */
 int y3_sgd_step(float* p, const float* g, float* m, float* ema, const uint8_t* group, int64_t n, const float* hp_dev,

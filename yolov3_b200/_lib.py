@@ -288,7 +288,7 @@ def _declare(lib):
         "y3_ap_per_class": ([vp, vp, vp, vp, i32, i32, i32, vp, i32, i32, vp, vp, vp, C.c_int64, vp, vp, vp, vp, vp, vp, vp],
                             C.c_int),
         "y3_sumsq_blocks": ([], i32),
-        "y3_grad_sumsq": ([vp, C.c_int64, vp, vp, vp], C.c_int),
+        "y3_grad_sumsq": ([vp, vp, C.c_int64, vp, vp, vp], C.c_int),
         "y3_sgd_step": ([vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp], C.c_int),
         "y3_bn_act_fwd": ([C.POINTER(BnActDesc), vp], C.c_int),
         "y3_bn_act_bwd": ([C.POINTER(BnBwdDesc), vp], C.c_int),

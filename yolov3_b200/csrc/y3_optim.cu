@@ -15,12 +15,16 @@ namespace {
 
 constexpr int kChunk = 256;  // elements per group-map entry; every parameter's slot in the flat buffer is a multiple of it
 
-// first stage: partial[b] = sum of g^2 over block b's grid-stride range (fixed association order per block)
-__global__ void __launch_bounds__(256) sumsq_partial_kernel(const float* __restrict__ g, long long n4, float* __restrict__ partial) {
+// first stage: partial[b] = sum of g^2 over block b's grid-stride range (fixed association order per block).  group
+// (optional): the chunks it does not tag trainable (< 3) are left out — frozen parameters, whose slot of g may hold anything,
+// count in the clip norm no more than they do in clip_grad_norm_, which skips a parameter whose .grad is None
+__global__ void __launch_bounds__(256) sumsq_partial_kernel(const float* __restrict__ g, const uint8_t* __restrict__ group,
+                                                            long long n4, float* __restrict__ partial) {
   pdl_entry();
   float acc = 0.f;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n4;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    if (group && group[(i * 4) / kChunk] >= 3) continue;
     const float4 v = __ldg(reinterpret_cast<const float4*>(g) + i);
     acc = fmaf(v.x, v.x, acc);
     acc = fmaf(v.y, v.y, acc);
@@ -71,7 +75,7 @@ __global__ void __launch_bounds__(256) sgd_step_kernel(float* __restrict__ p, co
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int grp = group[(i * 4) / kChunk];
     float4 pv = reinterpret_cast<float4*>(p)[i];
-    if (grp < 3) {  // trainable
+    if (grp < 3) {  // trainable; a frozen parameter (G_FROZEN in the map) keeps p and its momentum, and still takes the EMA
       const float lr = hp[grp], wd = hp[3 + grp];
       const float4 gv = __ldg(reinterpret_cast<const float4*>(g) + i);
       float4 mv = reinterpret_cast<float4*>(m)[i];
@@ -110,12 +114,13 @@ int blocks_for(long long n4) {
 
 extern "C" int32_t y3_sumsq_blocks(void) { return 1024; }
 
-extern "C" int y3_grad_sumsq(const float* g, int64_t n, float* partial, float* out, y3_stream_t stream_) {
+extern "C" int y3_grad_sumsq(const float* g, const uint8_t* group, int64_t n, float* partial, float* out, y3_stream_t stream_) {
   Y3_REQUIRE(g && partial && out && n > 0 && n % 4 == 0 && (reinterpret_cast<uintptr_t>(g) & 15) == 0,
              "grad_sumsq: n must be a multiple of 4, g 16-byte aligned");
+  Y3_REQUIRE(!group || n % y3::kChunk == 0, "grad_sumsq: with a group map n must be a multiple of 256");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const int nblk = y3_sumsq_blocks();  // fixed: the partial sums — and so the result — do not depend on the device
-  Y3_CHECK_CUDA(::y3::launch_pdl(y3::sumsq_partial_kernel, dim3(nblk), dim3(256), 0, stream, g, n / 4, partial));
+  Y3_CHECK_CUDA(::y3::launch_pdl(y3::sumsq_partial_kernel, dim3(nblk), dim3(256), 0, stream, g, group, n / 4, partial));
   Y3_CHECK_CUDA(::y3::launch_pdl(y3::sumsq_final_kernel, dim3(1), dim3(256), 0, stream, partial, nblk, out));
   Y3_CHECK_CUDA(cudaGetLastError());
   return Y3_OK;

@@ -98,7 +98,7 @@ class Model:
         self._packed = None
         self._engines: "OrderedDict" = OrderedDict()  # LRU over input shapes, at most MAX_ENGINES alive
         self.ddp = None  # parallel.DDP(model): overlapped gradient exchange
-        self._train_engines: dict = {}  # (n, h, w) -> TrainEngine, every one on ``_arena``
+        self._train_engines: dict = {}  # (n, h, w) [+ frozen set, when not empty] -> TrainEngine, every one on ``_arena``
         self._arena = None   # train.Arena: the activation memory the training engines of every batch shape share
         self._train_packs = None  # the training engines' shape-independent dgrad packs (train._shared_packs)
         self._precision = "bf16"
@@ -251,13 +251,14 @@ class Model:
         return missing, unexpected
 
     def parameters(self):
-        """Trainable parameters: ALWAYS the device-resident fp32 master tensors (created on first use), so an optimizer
+        """Parameters (not buffers): ALWAYS the device-resident fp32 master tensors (created on first use), so an optimizer
         built before the first forward — the reference order, train.py:252-262 before :403 — updates what the training
-        engine reads.  Their addresses never change for the life of the model (load_state_dict copies in place)."""
-        return iter([v for v in self.device_params().values() if v.requires_grad])
+        engine reads.  Their addresses never change for the life of the model (load_state_dict copies in place).  Like
+        nn.Module's, frozen parameters (``requires_grad`` False: train.py ``--freeze``) are included."""
+        return iter([v for v in self.device_params().values() if isinstance(v, torch.nn.Parameter)])
 
     def named_parameters(self):
-        return iter([(k, v) for k, v in self.device_params().items() if v.requires_grad])
+        return iter([(k, v) for k, v in self.device_params().items() if isinstance(v, torch.nn.Parameter)])
 
     def store(self):
         """The flat device store of every parameter / buffer (``params.ParamStore``), created on first use."""
@@ -369,16 +370,19 @@ class Model:
             self._engines.move_to_end(key)
         return e
 
-    def train_engine(self, n, h, w) -> "TrainEngine":
-        """The training engine of one batch shape.  Engines are kept per shape and share one activation arena, which grows to
-        the largest shape requested; growing drops the cached engines (their graphs hold the old addresses)."""
+    def train_engine(self, n, h, w, frozen=frozenset()) -> "TrainEngine":
+        """The training engine of one batch shape and frozen set (names of the parameters with ``requires_grad`` False).
+        Engines are kept per shape and frozen set and share one activation arena, which grows to the largest shape
+        requested; growing drops the cached engines (their graphs hold the old addresses)."""
         from .train import Arena, TrainEngine
 
-        te = self._train_engines.get((n, h, w))
+        frozen = frozenset(frozen)
+        key = (n, h, w, frozen) if frozen else (n, h, w)
+        te = self._train_engines.get(key)
         if te is None:
             if self._arena is None:
                 self._arena = Arena(self.device, on_grow=self._drop_train_engines)
-            te = self._train_engines[(n, h, w)] = TrainEngine(self, n, h, w, arena=self._arena)
+            te = self._train_engines[key] = TrainEngine(self, n, h, w, arena=self._arena, frozen=frozen)
         return te
 
     def _drop_train_engines(self):
@@ -421,7 +425,7 @@ class Model:
             # train mode (models/yolo.py:110 returns the raw maps): BatchNorm batch statistics, autograd-connected
             from .train import TrainFn
 
-            te = self.train_engine(n, *self._train_size(size, h, w))
+            te = self.train_engine(n, *self._train_size(size, h, w), frozen=self.store().frozen_now())
             P = self.device_params()
             return list(TrainFn.apply(te, x, 255.0 if x.dtype == torch.uint8 else 0.0, *[P[k] for k in te.param_names]))
         e = self.engine(n, h, w, x.dtype, 255.0 if x.dtype == torch.uint8 else 0.0)  # uint8 images: im/255

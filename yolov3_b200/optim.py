@@ -4,7 +4,9 @@
     (train.py:411-421, with smart_optimizer's three parameter groups, utils/torch_utils.py:207-237, and ModelEMA)
 
 as three launches over one buffer (csrc/y3_optim.cu): a two-stage gradient-norm reduction, then ONE pass that applies the clip
-coefficient, weight decay, SGD momentum (nesterov), the parameter update and the EMA update.  Hyper-parameters live in a small
+coefficient, weight decay, SGD momentum (nesterov), the parameter update and the EMA update.  Frozen parameters
+(``requires_grad`` False, train.py ``--freeze``) are marked in the store's group map: they keep their values and momentum,
+do not count in the norm, and their EMA still moves, as the reference's torch optimizer and ModelEMA treat them.  Hyper-parameters live in a small
 device array that is refreshed from the host before each step, so a scheduler can change them every iteration (warm-up,
 train.py:364-375) without rebuilding anything.  ``param_groups`` mirrors torch.optim's list of dicts (lr, momentum,
 weight_decay, nesterov, initial_lr) so that ``torch.optim.lr_scheduler.LambdaLR`` and the reference's warm-up loop, which write
@@ -90,8 +92,10 @@ class SGD:
             self._hp_used[slot] = True
         st = _stream()
         if self.max_norm > 0:
-            _lib.check(L.y3_grad_sumsq(s.G.data_ptr(), s.n_train, self._partial.data_ptr(), self.grad_sumsq.data_ptr(), st),
-                       "y3_grad_sumsq")
+            # frozen parameters (G_FROZEN in the group map) are left out of the norm, as clip_grad_norm_ skips grad None
+            group = s.group.data_ptr() if s.frozen else None
+            _lib.check(L.y3_grad_sumsq(s.G.data_ptr(), group, s.n_train, self._partial.data_ptr(), self.grad_sumsq.data_ptr(),
+                                       st), "y3_grad_sumsq")
         _lib.check(L.y3_sgd_step(s.P.data_ptr(), s.G.data_ptr(), self.M.data_ptr(), ema_ptr, s.group.data_ptr(), s.n_total,
                                  self._hp.data_ptr(), self.grad_sumsq.data_ptr(), st), "y3_sgd_step")
         s.mark_written()

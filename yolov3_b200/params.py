@@ -10,8 +10,9 @@ buffer), laid out for the training hot path:
   forward packs are views of one elementwise bf16 copy of this buffer and the wgrad kernel accumulates straight into the
   parameter's ``.grad`` view (no permute, no per-layer copies);
 * every slot is padded to a multiple of 256 elements and tagged with its optimizer group (smart_optimizer,
-  utils/torch_utils.py:207-237: 0 = weights with decay, 1 = BatchNorm weights, 2 = biases; 255 = buffers), which is all the
-  fused SGD / clip / EMA kernels (csrc/y3_optim.cu) need to treat the buffer as one array.
+  utils/torch_utils.py:207-237: 0 = weights with decay, 1 = BatchNorm weights, 2 = biases; 255 = buffers and frozen
+  parameters, ``requires_grad`` False: train.py ``--freeze``), which is all the fused SGD / clip / EMA kernels
+  (csrc/y3_optim.cu) need to treat the buffer as one array.
 
 ``views[name]`` are ordinary (strided) torch tensors aliasing the flat storage: optimizers, ``state_dict()``, checkpointing
 and the reference's parameter-name contract keep working on them.
@@ -96,7 +97,10 @@ class ParamStore:
         gm = torch.full((self.n_total // CHUNK,), G_FROZEN, dtype=torch.uint8)
         for s in slots:
             gm[s.offset // CHUNK:(s.offset + s.numel) // CHUNK] = s.group
+        self._group_host = gm.clone()  # the groups with nothing frozen (gm.to() aliases gm on the host)
         self.group = gm.to(dev)
+        self.frozen: frozenset = frozenset()  # trainable slots the group map marks G_FROZEN (set_frozen)
+        self._attached_frozen: frozenset = frozenset()  # the frozen set of the last attach_grads
         self.views: "OrderedDict[str, torch.Tensor]" = OrderedDict()
         self.grads: dict[str, torch.Tensor] = {}
         for name in model.params:  # state_dict order
@@ -140,12 +144,43 @@ class ParamStore:
         n = s.numel if padded else s.shape[0]
         return (self.G if grad else self.P)[s.offset:s.offset + n]
 
-    def attach_grads(self):
-        """Make every trainable parameter's ``.grad`` the view of the flat gradient buffer."""
+    def frozen_now(self) -> frozenset:
+        """Names of the parameters whose ``requires_grad`` is False now (train.py ``--freeze``, train.py:217-223)."""
+        return frozenset(name for name in self.grads if not self.views[name].requires_grad)
+
+    def set_frozen(self, frozen: frozenset):
+        """Mark ``frozen`` G_FROZEN in the group map the fused kernels read: the SGD step keeps their values and momentum
+        (their EMA still moves, as ModelEMA averages every entry) and the clip norm leaves them out."""
+        if frozen == self.frozen:
+            return
+        gm = self._group_host.clone()
+        for name in frozen:
+            s = self.slots[name]
+            gm[s.offset // CHUNK:(s.offset + s.numel) // CHUNK] = G_FROZEN
+        self.group.copy_(gm)
+        self.frozen = frozenset(frozen)
+
+    def begin_backward(self, frozen: frozenset):
+        """Before a backward with the frozen set ``frozen``: zero G unless earlier gradients are live; if they are, zero
+        the slots of parameters frozen at the last backward and trainable now (autograd gives them a fresh ``.grad``)."""
+        self.set_frozen(frozen)
+        if not self.grads_are_live():
+            self.G.zero_()
+            return
+        for name in self._attached_frozen - frozen:
+            s = self.slots[name]
+            self.G[s.offset:s.offset + s.numel].zero_()
+
+    def attach_grads(self, frozen: frozenset = frozenset()):
+        """Make every trainable parameter's ``.grad`` the view of the flat gradient buffer; a frozen parameter's stays None."""
         for name, g in self.grads.items():
             p = self.views[name]
-            if p.grad is not g:
+            if name in frozen:
+                if p.grad is g:
+                    p.grad = None
+            elif p.grad is not g:
                 p.grad = g
+        self._attached_frozen = frozenset(frozen)
         self.grads_live = True
 
     def zero_grad(self, set_to_none: bool = True):
@@ -161,21 +196,25 @@ class ParamStore:
     def grads_are_live(self) -> bool:
         if not self.grads_live:
             return False
-        first = self.views[self.order[0]]
-        return first.grad is not None  # an optimizer's zero_grad(set_to_none=True) detached them: start from zero
+        first = next((self.views[n] for n in self.order if n in self.grads and n not in self._attached_frozen), None)
+        return first is not None and first.grad is not None  # an optimizer's zero_grad(set_to_none=True) detached them
 
-    def bucket_ranges(self, n_buckets=4, tail_fraction=0.012):
+    def bucket_ranges(self, n_buckets=4, tail_fraction=0.012, frozen: frozenset = frozenset()):
         """Contiguous element ranges of G (slot-aligned) in backward-completion order.  The LAST bucket — the only one whose
         all-reduce cannot hide behind remaining backward work — is kept small (``tail_fraction`` of the gradient bytes: in
         YOLOv3 the layers back-propagated last, 0..5, hold ~1 % of the parameters (2.8 MB), so their exchange after the
         backward is short; a larger tail — layers 0..7, 18 MB — left a visible share of the exchange exposed); the rest is
-        split evenly."""
-        names = [n for n in self.order if self.slots[n].group != G_FROZEN]
-        total = self.n_train
-        cuts = [total * (1 - tail_fraction) * (i + 1) / (n_buckets - 1) for i in range(n_buckets - 1)] if n_buckets > 1 else []
-        ranges, start, ci = [], 0, 0
-        for nm in names:
-            s = self.slots[nm]
+        split evenly.  The ranges span the parameters not in ``frozen`` only, from the first one's slot to the last one's
+        (frozen slots between trainable ones ride along: the kernels that read G skip them); with nothing trainable, one
+        empty range."""
+        live = [self.slots[n] for n in self.order if self.slots[n].group != G_FROZEN and n not in frozen]
+        if not live:
+            return [(0, 0)]
+        lo, total = live[0].offset, live[-1].offset + live[-1].numel
+        span = total - lo
+        cuts = [lo + span * (1 - tail_fraction) * (i + 1) / (n_buckets - 1) for i in range(n_buckets - 1)] if n_buckets > 1 else []
+        ranges, start, ci = [], lo, 0
+        for s in (self.slots[n] for n in self.order if lo <= self.slots[n].offset < total):
             end = s.offset + s.numel
             if ci < len(cuts) and end >= cuts[ci] and end < total:
                 ranges.append((start, end))

@@ -47,7 +47,11 @@ class _Block:
     """One Conv+BN+SiLU block (models/common.py:57-81) with everything its forward and backward need."""
 
     __slots__ = ("prefix", "c1", "c2", "k", "s", "x", "y", "a", "res", "upsample", "wf", "wd", "st", "dw", "first", "dy",
-                 "post_fwd", "pre_bwd", "gamma", "beta", "rmean", "rvar", "dgamma", "dbeta", "nblk", "count")
+                 "post_fwd", "pre_bwd", "gamma", "beta", "rmean", "rvar", "dgamma", "dbeta", "nblk", "count",
+                 "bn_bwd", "wgrad", "dx", "res_grad")
+    # gradient plan (autograd's rule under frozen parameters): bn_bwd = the output needs a gradient, wgrad = the weight is
+    # trainable, dx = channels [0, dx) of x the dgrad writes (0: none), res_grad = the shortcut's input needs a gradient;
+    # dgamma / dbeta are None when frozen
 
 
 def gather_shapes(n: int, h: int, w: int) -> list[tuple[int, int, int]]:
@@ -146,12 +150,15 @@ class TrainEngine:
     n_buckets = 4            # gradient ranges all-reduced separately, each as soon as its layers are done
     MAX_FWD_GRAPHS = 4       # forward graphs kept per engine, one per input shape fed to it (rect batches rescaled to it)
 
-    def __init__(self, model, n, h, w, keep_all=False, arena=None):
+    def __init__(self, model, n, h, w, keep_all=False, arena=None, frozen=frozenset()):
         """keep_all=True gives every block its own dy buffer (per-layer gradient checks in the tests); the default shares
         one scratch buffer per shape.  ``arena``: where the shape-dependent buffers live (``Model`` passes the one its
-        engines of every shape share); None gives the engine an arena of its own."""
+        engines of every shape share); None gives the engine an arena of its own.  ``frozen``: names of the parameters that
+        get no gradient (``requires_grad`` False, train.py ``--freeze``): the backward runs only the launches autograd would
+        need for the others, and gradient buffers exist only for activations that depend on a trainable parameter."""
         self.model, self.n, self.h, self.w = model, n, h, w
         self.keep_all = keep_all
+        self.frozen = frozenset(frozen)
         self.arena = Arena(model.device) if arena is None else arena
         self.store = model.store()
         self.P = model.device_params()
@@ -192,7 +199,22 @@ class TrainEngine:
         self.scratch: dict[tuple, PaddedNHWC] = {}
         padded = []  # (buffer, channels in use): the table of y3_zero_halo_batched
         with_grad = {}  # id(buffer) -> buffer, for every activation buffer a backward writes the gradient of
+        need = {}  # id(buffer) -> [(coff, c)]: the slices that depend on a trainable parameter (autograd's requires_grad)
         max_partial = 0
+
+        def trainable(name):
+            return name not in self.frozen
+
+        def needs(t):
+            return any(o < t.coff + t.c and t.coff < o + c for o, c in need.get(id(t.buf), ()))
+
+        def mark(t):
+            need.setdefault(id(t.buf), []).append((t.coff, t.c))
+
+        def needed_channels(t):
+            """[0, hi) of ``t``'s channels that covers every slice needing a gradient (a Concat buffer whose later members
+            depend on frozen layers only gets a partial dgrad; in these graphs the needed member comes first)."""
+            return max(min(o + c, t.coff + t.c) for o, c in need[id(t.buf)] if o < t.coff + t.c and t.coff < o + c) - t.coff
 
         def pad(c, hh, ww, ld):
             b = PaddedNHWC(self._take((n, hh + 2, ww + 2, ld), torch.bfloat16), 0, c)
@@ -221,21 +243,35 @@ class TrainEngine:
             c1, k, s = (32, 1, 1) if first else (cb.c1, cb.k, cb.s)  # layer 0 = 1x1 conv over the im2col
             b = _Block()
             b.prefix, b.c1, b.c2, b.k, b.s, b.x, b.a, b.res, b.upsample, b.first = prefix, c1, c2, k, s, x, a, res, upsample, first
-            grad(a) if first else grad(a, x)
+            x_needs = not first and needs(x)
+            b.res_grad = res is not None and needs(res)
+            b.wgrad = trainable(prefix + ".conv.weight")
+            bn_train = trainable(prefix + ".bn.weight"), trainable(prefix + ".bn.bias")
+            b.bn_bwd = x_needs or b.res_grad or b.wgrad or any(bn_train)
+            b.dx = needed_channels(x) if x_needs else 0
+            if b.bn_bwd:
+                mark(a)
+                grad(a)
+            if x_needs:
+                grad(x)
             ho, wo = x.h // s, x.w // s
             b.y = buf(c2, ho, wo)
             b.wf = store.weight_rows_bf16(prefix + ".conv.weight")
             b.wd = None
             b.dw = store.grad_rows(prefix + ".conv.weight")
             b.gamma, b.beta = store.flat(prefix + ".bn.weight"), store.flat(prefix + ".bn.bias")
-            b.dgamma, b.dbeta = store.flat(prefix + ".bn.weight", grad=True), store.flat(prefix + ".bn.bias", grad=True)
+            b.dgamma = store.flat(prefix + ".bn.weight", grad=True) if bn_train[0] else None
+            b.dbeta = store.flat(prefix + ".bn.bias", grad=True) if bn_train[1] else None
             b.rmean, b.rvar = store.flat(prefix + ".bn.running_mean"), store.flat(prefix + ".bn.running_var")
             b.st = {name: f32(c2) for name in ("scale", "shift", "mean", "rstd")}
             b.st.update(sums=f32(2 * c2), gsums=f32(2 * c2))  # [sum | sumsq] forward, [sum dz | sum dz*xhat] backward
             b.nblk = T.partial_blocks(n, ho, wo, c2)
             b.count = float(n * ho * wo)
             max_partial = max(max_partial, b.nblk * 2 * c2)
-            b.dy = buf(c2, ho, wo) if self.keep_all else self._scratch(c2, ho, wo, pad)
+            if not b.bn_bwd:
+                b.dy = None
+            else:
+                b.dy = buf(c2, ho, wo) if self.keep_all else self._scratch(c2, ho, wo, pad)
             b.post_fwd, b.pre_bwd = [], []  # extra launches after this block's forward / before its backward (SPP pools)
             self.blocks.append(b)
             return b
@@ -279,11 +315,13 @@ class TrainEngine:
                     idx = self._take((n * ly.h * ly.w * c_,), torch.uint8)
                     self.keep.append(idx)
                     src, dst = cat.slice(0, c_), cat.slice((q + 1) * c_, c_)
-                    grad(src, dst)
-                    self.pools.append(dict(src=src, dst=dst, k=k, stride=1, off=-(k // 2), oob_zero=False))
+                    self.pools.append(dict(src=src, dst=dst, k=k, stride=1, off=-(k // 2), oob_zero=False, bwd=needs(src)))
                     b1.post_fwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_train_fwd(src, dst, k, idx))
-                    b1.pre_bwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_bwd(self.grad_of(dst), self.grad_of(src),
-                                                                                        k, idx, accumulate=True))
+                    if needs(src):
+                        mark(dst)
+                        grad(src, dst)
+                        b1.pre_bwd.append(lambda src=src, dst=dst, k=k, idx=idx: T.maxpool_bwd(
+                            self.grad_of(dst), self.grad_of(src), k, idx, accumulate=True))
                 y = out_of(ly)
                 new_block(cv2, cat, y)
                 tens[nd.i] = y
@@ -295,12 +333,14 @@ class TrainEngine:
                 y = out_of(ly)
                 idx = self._take((n * y.h * y.w * x.c,), torch.uint8)
                 self.keep.append(idx)
-                grad(x, y)
-                self.pools.append(dict(src=x, dst=y, k=p.k, stride=p.s, off=-p.pad, oob_zero=p.oob_zero))
+                self.pools.append(dict(src=x, dst=y, k=p.k, stride=p.s, off=-p.pad, oob_zero=p.oob_zero, bwd=needs(x)))
                 host = self.blocks[-1]  # the pool runs after the latest block's forward and before that block's backward
                 host.post_fwd.append(lambda x=x, y=y, p=p, idx=idx:
                                      T.maxpool_train_fwd(x, y, p.k, idx, stride=p.s, off=-p.pad, oob_zero=p.oob_zero))
-                host.pre_bwd.append(lambda x=x, y=y, p=p, idx=idx: self._pool_backward(x, y, p.k, p.s, -p.pad, idx))
+                if needs(x):
+                    mark(y)
+                    grad(x, y)
+                    host.pre_bwd.append(lambda x=x, y=y, p=p, idx=idx: self._pool_backward(x, y, p.k, p.s, -p.pad, idx))
                 tens[nd.i] = y
 
         # ---- Detect heads
@@ -309,9 +349,11 @@ class TrainEngine:
         dec = _lib.DecodeDesc()
         for j, ph in enumerate(plan.heads):
             x = tens[ph.src]
-            grad(x)
             wname, bname = f"model.{det.i}.m.{j}.weight", f"model.{det.i}.m.{j}.bias"
-            hd = dict(x=x, c1=x.c, j=j, wname=wname, bname=bname)
+            hd = dict(x=x, c1=x.c, j=j, wname=wname, bname=bname, dx=needs(x), wgrad=trainable(wname), dbias=trainable(bname))
+            hd["bwd"] = hd["dx"] or hd["wgrad"] or hd["dbias"]
+            if hd["dx"]:
+                grad(x)
             hd["out"] = self._take((n * x.h * x.w, head_ld), torch.float32)
             hd["raw"] = self._take((n, det.na, x.h, x.w, det.no), torch.float32)
             hd["graw"] = self._take((n, det.na, x.h, x.w, det.no), torch.float32)  # dL/draw input of the backward graph
@@ -333,12 +375,16 @@ class TrainEngine:
         self.err = torch.zeros(1, dtype=torch.int32, device=dev)
         self.partial = self._take((max_partial,), torch.float32)  # first-stage rows of every reduction
 
-        # ---- one gradient buffer per activation buffer that receives a gradient (same geometry, same channel use)
+        # ---- one gradient buffer per activation buffer that receives a gradient (same geometry, same channel use), cut to
+        #      the channels [0, hi) that need it when only a Concat buffer's leading members do
         self.grad_bufs: dict[int, PaddedNHWC] = {}
         for t in with_grad.values():
-            g = pad(t.shape[3], t.shape[1] - 2, t.shape[2] - 2, t.shape[3])
+            c_use = next(c for b, c in padded if b is t)
+            hi = needed_channels(PaddedNHWC(t))
+            ld = t.shape[3] if hi >= c_use else hi
+            g = pad(ld, t.shape[1] - 2, t.shape[2] - 2, ld)
             self.grad_bufs[t.data_ptr()] = g
-            padded[-1] = (g.buf, next(c for b, c in padded if b is t))
+            padded[-1] = (g.buf, min(c_use, ld))
 
         # ---- dgrad packs, the batched re-pack table and the zero bias: shape-independent, held once per model
         shared = _shared_packs(model, self)
@@ -364,14 +410,17 @@ class TrainEngine:
         for hd in self.heads:
             self.param_names += [hd["wname"], hd["bname"]]
 
-        # ---- backward segments: [heads + last blocks | ... | first blocks], cut where the gradient buckets end
-        self.buckets = store.bucket_ranges(self.n_buckets)
+        # ---- backward segments: [heads + last blocks | ... | first blocks], cut where the gradient buckets of the trainable
+        #      slots end; a block with no backward launch is in none
+        self.buckets = store.bucket_ranges(self.n_buckets, frozen=self.frozen)
         ends = [e for _, e in self.buckets]
         self.segments: list[list[_Block]] = [[] for _ in ends]
         si = 0
         for b in reversed(self.blocks):
+            if not (b.bn_bwd or b.pre_bwd):
+                continue
             off = store.slots[b.prefix + ".conv.weight"].offset
-            while off >= ends[si]:
+            while si < len(ends) - 1 and off >= ends[si]:
                 si += 1
             self.segments[si].append(b)
 
@@ -491,8 +540,7 @@ class TrainEngine:
         parameters as ``.grad`` views.  With ``parallel.DDP`` enabled, each gradient bucket is all-reduced on a side stream as
         soon as the segment producing it has been enqueued."""
         store = self.store
-        if not store.grads_are_live():
-            store.G.zero_()
+        store.begin_backward(self.frozen)
         ddp = getattr(self.model, "ddp", None)
         exchange = ddp is not None and ddp.require_sync and self.world > 1
         if exchange and self.comm is None:
@@ -508,7 +556,8 @@ class TrainEngine:
             graws = [g.detach().float().contiguous() for g in graws]
         self._written, self._pending_res, self._pending_add = set(), {}, {}
         for si, seg in enumerate(self.segments):
-            self._run(("bwd", si), lambda si=si, seg=seg: self._backward_segment(si, seg, graws))
+            if si == 0 or seg:  # a bucket may hold only slots whose gradients an earlier segment finished
+                self._run(("bwd", si), lambda si=si, seg=seg: self._backward_segment(si, seg, graws))
             if exchange:
                 lo, hi = self.buckets[si]
                 ev = torch.cuda.Event()
@@ -520,7 +569,7 @@ class TrainEngine:
             main.wait_stream(self.comm)
             ddp.pending_average = True  # G holds SUMS over ranks: the optimizer folds 1/world into its update, or
             #                             parallel.DDP.finish() divides in place for a plain torch.optim optimizer
-        store.attach_grads()
+        store.attach_grads(self.frozen)
 
     def _contribute_conv(self, dy, wd, c_in, k, x, s2=False):
         gx = _wide(self.grad_of(x))  # c_in = 16: the dgrad conv writes 32 channels, the upper 16 from zero weight rows
@@ -564,15 +613,22 @@ class TrainEngine:
         det_flag = 1 if self.deterministic else 0
         if si == 0:
             for hd, g in zip(self.heads, graws):
+                if not hd["bwd"]:
+                    continue
                 x = hd["x"]
                 T.head_grad_pack(g, hd["dy"], self.partial)
-                T.colreduce(self.partial, hd["nblk"], hd["pw"], hd["db"], accumulate=True)
-                T.conv_wgrad(hd["dy"], x, hd["dw"], 1, accumulate=True, deterministic=det_flag)
-                self._contribute_conv(hd["dy"], hd["wd"], hd["c1"], 1, x)
+                if hd["dbias"]:
+                    T.colreduce(self.partial, hd["nblk"], hd["pw"], hd["db"], accumulate=True)
+                if hd["wgrad"]:
+                    T.conv_wgrad(hd["dy"], x, hd["dw"], 1, accumulate=True, deterministic=det_flag)
+                if hd["dx"]:
+                    self._contribute_conv(hd["dy"], hd["wd"], hd["c1"], 1, x)
         for b in seg:
             st = b.st
             for fn in b.pre_bwd:
                 fn()
+            if not b.bn_bwd:
+                continue
             da = self.grad_of(b.a)
             if self.sync_bn:
                 # local sums are the (rank-local) gamma/beta gradients; dy needs the sums over all ranks
@@ -582,8 +638,9 @@ class TrainEngine:
                 T.bn_act_bwd(b.y, da, b.dy, st, st["gsums"], None, None, None, b.upsample, phase=2, count=b.count)
             else:
                 T.bn_act_bwd(b.y, da, b.dy, st, st["sums"], self.partial, b.dbeta, b.dgamma, b.upsample)
-            T.conv_wgrad(b.dy, b.x, b.dw, b.k, accumulate=True, deterministic=det_flag, stride=b.s)
-            if b.res is not None:
+            if b.wgrad:
+                T.conv_wgrad(b.dy, b.x, b.dw, b.k, accumulate=True, deterministic=det_flag, stride=b.s)
+            if b.res_grad:
                 # Bottleneck shortcut: the block output's gradient also flows to its input.  It is folded into the next
                 # dgrad into that tensor (cv1 of the same Bottleneck: the very next block) through the residual port, or
                 # added by a separate launch if no such dgrad arrives before the segment ends.
@@ -592,10 +649,12 @@ class TrainEngine:
                 key = (r.buf.data_ptr(), r.coff, r.c)
                 self._pending_res[key] = da
                 self._pending_add[key] = (da, r)
-            if not b.first:
-                key = (b.x.buf.data_ptr(), b.x.coff, b.x.c)
+            if b.dx:
+                # only channels [0, dx) of x when the rest of a Concat buffer needs no gradient: the dgrad pack's first rows
+                x, wd = (b.x, b.wd) if b.dx == b.x.c else (b.x.slice(0, b.dx), b.wd[:b.dx])
+                key = (x.buf.data_ptr(), x.coff, x.c)
                 # stride 2: transposed conv by parity classes on the un-stuffed dy (4 launches, a quarter of the MMA work)
-                self._contribute_conv(b.dy, b.wd, b.c1, b.k, b.x, s2=b.s == 2)
+                self._contribute_conv(b.dy, wd, b.dx, b.k, x, s2=b.s == 2)
                 self._pending_add.pop(key, None)
         self._flush_pending()  # a segment is one CUDA graph: nothing may stay pending across its end
         return None
