@@ -553,8 +553,8 @@ int y3_ap_per_class(const float* conf, const float* cls, const uint8_t* tp, cons
                     double* ap, double* curves, double* best, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
- * Optimizer step over ONE flat fp32 parameter buffer (train.py:411-421: clip_grad_norm_(10.0), SGD-nesterov with the three
- * parameter groups of smart_optimizer utils/torch_utils.py:207-237, ModelEMA.update) — csrc/y3_optim.cu.
+ * Optimizer step over ONE flat fp32 parameter buffer (train.py:411-421: clip_grad_norm_(10.0), SGD-nesterov, Adam or AdamW
+ * with the three parameter groups of smart_optimizer utils/torch_utils.py:207-237, ModelEMA.update) — csrc/y3_optim.cu.
  * Layout contract: every parameter occupies a slot whose length is a multiple of 256 elements; group[i] is the group of
  * elements [256 i, 256 i + 256): 0 = weights with decay, 1 = BatchNorm weights, 2 = biases, >= 3 = not trained (buffers,
  * and frozen parameters: requires_grad False).
@@ -570,6 +570,13 @@ int y3_grad_sumsq(const float* g, const uint8_t* group, int64_t n, float* partia
  * only when hp_dev[8] > 0.  n = elements of p (and of ema); g and m are only touched where group < 3. */
 int y3_sgd_step(float* p, const float* g, float* m, float* ema, const uint8_t* group, int64_t n, const float* hp_dev,
                 const float* gsumsq, y3_stream_t stream);
+/* Adam / AdamW (train.py --optimizer), torch.optim.Adam's foreach arithmetic: p, m / v (exp_avg / exp_avg_sq, zero-initialised,
+ * n_train elements), ema (optional) updated in place from g.  slot[c] = parameter slot of chunk c (read where group < 3).
+ * hp_dev: DEVICE float[24] = coupled weight decay[3] (Adam), decoupled decay factor 1 - lr*wd [3] (AdamW, 1: none),
+ * -, -, max_norm, ema decay, gradient pre-scale (hp[8..10] as y3_sgd_step), -, 1 - beta1 [3], beta2 [3], 1 - beta2 [3],
+ * eps [3]; tab_dev: DEVICE float[2 * slots] = per slot {-lr / (1 - beta1^t), sqrt(1 - beta2^t)} at the slot's own step t. */
+int y3_adam_step(float* p, const float* g, float* m, float* v, float* ema, const uint8_t* group, const int32_t* slot, int64_t n,
+                 const float* hp_dev, const float* tab_dev, const float* gsumsq, y3_stream_t stream);
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Whole-graph executor.  Replaces BaseModel._forward_once (models/yolo.py:135-147): the Python loop over nn.Modules

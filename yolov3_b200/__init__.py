@@ -14,7 +14,7 @@ the C ABI in ``include/yolov3_b200.h``; there is no CPU or PyTorch fallback.
     letterbox                  utils/augmentations.py:104 (preprocess.preprocess: + utils/dataloaders.py:308-310 layout step)
     forward_augment, Ensemble, attempt_load   models/yolo.py:239-280, models/experimental.py:74-136
     DDP, scale_loss, convert_sync_batchnorm   utils/torch_utils.py:60-72, train.py:405-406, :270-272
-    SGD, ModelEMA              utils/torch_utils.py:207-237 + train.py:411-421 (fused clip + SGD-nesterov + EMA)
+    SGD, Adam, AdamW, ModelEMA, smart_optimizer   utils/torch_utils.py:207-237 + train.py:411-421 (fused clip + update + EMA)
     Pipeline                   detect.py:185-200 loop body
     DeviceLoader, plan_item    utils/dataloaders.py:659-822 (LoadImagesAndLabels.__getitem__ with augment=True + collate_fn)
 """
@@ -27,7 +27,8 @@ _EXPORTS = {
     "non_max_suppression": "nms", "nms_batched": "nms", "scale_boxes": "boxes", "clip_boxes": "boxes", "box_iou": "loss",
     "ComputeLoss": "loss", "process_batch": "val", "process_batch_batched": "val", "letterbox": "preprocess",
     "forward_augment": "tta", "Ensemble": "tta", "attempt_load": "tta", "DDP": "parallel",
-    "scale_loss": "parallel", "convert_sync_batchnorm": "parallel", "SGD": "optim", "ModelEMA": "optim", "Pipeline": "pipeline",
+    "scale_loss": "parallel", "convert_sync_batchnorm": "parallel", "SGD": "optim", "Adam": "optim", "AdamW": "optim",
+    "smart_optimizer": "optim", "ModelEMA": "optim", "Pipeline": "pipeline",
     "DeviceLoader": "augment", "plan_item": "augment",
 }
 __all__ = sorted(_EXPORTS)

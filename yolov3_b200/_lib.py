@@ -290,6 +290,7 @@ def _declare(lib):
         "y3_sumsq_blocks": ([], i32),
         "y3_grad_sumsq": ([vp, vp, C.c_int64, vp, vp, vp], C.c_int),
         "y3_sgd_step": ([vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp], C.c_int),
+        "y3_adam_step": ([vp, vp, vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp], C.c_int),
         "y3_bn_act_fwd": ([C.POINTER(BnActDesc), vp], C.c_int),
         "y3_bn_act_bwd": ([C.POINTER(BnBwdDesc), vp], C.c_int),
         "y3_scale_boxes": ([vp, C.c_int64, i32, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, vp], C.c_int),

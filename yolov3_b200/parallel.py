@@ -8,7 +8,7 @@ backward pass is cut into a few segments: ``DDP(model)`` makes ``TrainEngine.bac
 segment's contiguous gradient range on a side stream as soon as that segment is enqueued, so the exchange of the deep layers
 (90 % of the 248 MB) runs under the back-propagation of the shallow ones and only the last, small range is exposed.  No
 packing / unpacking copies: NCCL reads and writes the gradient buffer in place, and the 1/world_size of the mean is folded
-into the fused optimizer update (``optim.SGD``) or applied by ``DDP.finish()``.
+into the fused optimizer update (``optim.SGD`` / ``Adam`` / ``AdamW``) or applied by ``DDP.finish()``.
 """
 from __future__ import annotations
 
@@ -87,7 +87,8 @@ class DDP:
         return _Ctx()
 
     def finish(self):
-        """For optimizers other than ``optim.SGD`` (which averages inside its update): turn the summed gradients into the mean."""
+        """For optimizers other than the fused ``optim.SGD`` / ``Adam`` / ``AdamW`` (which average inside their update): turn the
+        summed gradients into the mean."""
         if self.pending_average:
             self.module.store().G.div_(self.world)
             self.pending_average = False
