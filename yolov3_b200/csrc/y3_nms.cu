@@ -246,7 +246,7 @@ __device__ __forceinline__ bool box_suppresses(const float4& bi, float ai, const
 //                                     appended to the image's survivor list
 //   nms_seg_block_kernel              segments > 512 members (multi-label at low conf; agnostic / out-of-range images, whose
 //                                     single segment is ranked by all the image's CTAs and finished by the last one)
-//   nms_output_kernel    1 CTA/image  top max_det survivors by key: shared-memory bitonic sort (<= 4096 survivors) or exact
+//   nms_output_kernel    1 CTA/image  top max_det survivors by key: shared-memory bitonic sort (<= 8192 survivors) or exact
 //                                     radix select + sort of the selected, rows + (row, class) sources + counts
 // All arithmetic in the reference's order, ties broken by candidate id (stable).
 constexpr int kBucketThreads = 1024;
@@ -808,7 +808,7 @@ __global__ void __launch_bounds__(1024) nms_output_kernel(const NmsArgs p) {
       }
       for (int rnk = threadIdx.x; rnk < D; rnk += blockDim.x) emit(rnk, s_k[rnk], s_p[rnk]);
     } else {
-      // more than 4096 rows requested AND available: rank by counting straight from global memory (exact, slow, rare)
+      // more than 8192 rows requested AND available: rank by counting straight from global memory (exact, slow, rare)
       for (int i = threadIdx.x; i < S; i += blockDim.x) {
         const unsigned long long key = sk[i];
         if (key < thr) continue;
