@@ -1,7 +1,10 @@
 """The engines the benchmark times, checked one launch at a time over the whole batch, element by element.
 
-Inference (yolov3 640x640 bs 32 bf16 and fp8, yolov3-spp 640x640 bs 8 bf16): every op of ``Engine.op_list`` is launched
-alone on snapshots of its operands and compared with a float32 torch reference (TF32 off) of the same operation:
+Inference (the benchmark's yolov3 640x640 bs 32 bf16 and fp8 and yolov3-spp 640x640 bs 8 bf16 engines, and the shapes
+validation and detection run: val.py's rect batches at 672x672, 512x672 and 672x512, detect.py's bs 1 at 384x640 and
+640x480, yolov3-tiny at 416x416; uint8 input with the /255 in conv_first; e4m3 engines run away from their 640x640
+calibration shape): every op of ``Engine.op_list`` is launched alone on snapshots of its operands and compared with a
+float32 torch reference (TF32 off) of the same operation:
   conv, bf16 output   |got - ref| <= 1/2 bf16 step of ref + 1.1 EPS L1 for every element, L1 = sum |x w| + |b| + |res|
                       (1.1: the largest slope of SiLU), and at least MIN_EXACT of the outputs are the bf16 rounding of ref
   conv, e4m3 output   test_fp8_gpu.assert_codes_match.  The mean error of a channel is printed, not bounded: the e4m3
@@ -9,7 +12,8 @@ alone on snapshots of its operands and compared with a float32 torch reference (
   Detect heads (fp32) |got - ref| <= EPS_HEAD L1 + 1e-6 |ref|; the padding columns are 0
   every conv          the halo is zero and every byte outside the written channel slice is unchanged; every activation
                       buffer starts with poison in its interior, so an element a producer skips is never zero by luck
-  conv_first          F.conv2d + SiLU, atol = rtol = 1e-2 (test_conv_gpu.test_conv_first)
+  conv_first          F.conv2d + SiLU (of x.float() / 255 for uint8 input), atol = rtol = 1e-2
+                      (test_conv_gpu.test_conv_first)
   max-pool            equal to F.max_pool2d;  decode: yolo_oracle.decode on the same raw maps, rtol 2e-6, atol 1e-6
 Training (yolov3 640x640 bs 8, split-K wgrad, CUDA-graph replay: the benchmark's settings), every block on the tensors
 the replayed step left behind, references on the device in float32:
@@ -18,7 +22,7 @@ the replayed step left behind, references on the device in float32:
   dy (bf16)           1/2 bf16 step + EPS_DY gamma rstd (|dz| + mean|dz| + |yhat| mean|dz yhat|): the per-channel means
                       come from fp32 sums whose error scales with the sums of magnitudes, not with the means
   dW (fp32)           EPS_W conv2d_weight(|x|, |dy|): both operands are the stored bf16 tensors, only the order of the
-                      summation differs
+                      summation differs; the reference sums in float64 (a float32 one can be off by as much as EPS_W)
   dgamma, dbeta       EPS_BN sum |dz yhat|, EPS_BN sum |dz| per channel
 Each criterion is also applied to deliberately damaged references (one 128-pixel tile of a middle image taken from the
 next image, the residual missing from one tile, one channel shifted by 1 % of its RMS -- except for e4m3 outputs, where
@@ -33,6 +37,8 @@ Constants: about 4x the worst value measured on an H100 80GB HBM3 (power limit 4
   BN + SiLU backward dy                    error beyond half a step / L1        8.8e-5   EPS_DY 3.5e-4
   dbeta, dgamma                            error / sum of magnitudes            7.0e-7, 1.8e-6   EPS_BN 7.5e-6
   dW of 1x1 / 3x3 layers                   error / L1                           8.4e-7 / 2.9e-5   EPS_W 3.4e-6 / 1.2e-4
+                                           (float64 reference, 700 W: 6.5e-7 / 1.5e-5; over every training shape of
+                                           test_train_backward_gpu 2.6e-6 / 1.5e-5)
   bf16 outputs not the rounding of the reference: conv 0.22 %, y 0.25 %, a 0.08 %, dy 0.14 % (MIN_EXACT 99 %),
   dx 0.99 % (MIN_EXACT_DX 96 %: where a separate launch adds the shortcut gradient, dx is rounded twice)
 """
@@ -244,20 +250,50 @@ def _bench_yolov3():
     return bench.build_model("cuda")
 
 
-def _inputs(n, seed):
-    return torch.rand(n, 3, 640, 640, device="cuda", generator=torch.Generator(device="cuda").manual_seed(seed))
+def _inputs(n, h, w, u8, seed):
+    """fp32 in [0, 1], or uint8 images (the engine divides by 255 in conv_first)."""
+    g = torch.Generator(device="cuda").manual_seed(seed)
+    if u8:
+        return torch.randint(0, 256, (n, 3, h, w), device="cuda", generator=g, dtype=torch.uint8)
+    return torch.rand(n, 3, h, w, device="cuda", generator=g)
 
+
+# launches on which the damaged references are tried (besides the first head, the first pool and the decode)
+SENSITIVITY = {"model.2.cv1", "model.2.cv2", "model.16", "model.8.7.cv2"}
+# yolov3-tiny: an N = 128 TMA conv (with halo reuse), the upsampling 1x1, and the 3x3 reading the Concat
+SENSITIVITY_TINY = {"model.6", "model.16", "model.19"}
+TMA = {"tma_flat", "tma_patch"}
+N256 = {"n256_upsample", "n256_res_coff"}
 
 ENGINES = {
     # bench.py config 2
-    "yolov3_bf16": dict(model=_bench_yolov3, bs=32, fp8=False, n_conv=74),
+    "yolov3_bf16": dict(model=_bench_yolov3, bs=32, fp8=False, n_conv=74, need=TMA | N256 | {"halo_64_128"}),
     # bench.py config 3 (per-GPU shard)
-    "yolov3-spp_bf16": dict(model=lambda: _model("yolov3-spp.yaml"), bs=8, fp8=False, n_conv=None),
+    "yolov3-spp_bf16": dict(model=lambda: _model("yolov3-spp.yaml"), bs=8, fp8=False, n_conv=None, need=TMA),
     # tools/bench_fp8.py
-    "yolov3_fp8": dict(model=_bench_yolov3, bs=32, fp8=True, n_conv=74),
+    "yolov3_fp8": dict(model=_bench_yolov3, bs=32, fp8=True, n_conv=74, need=TMA | N256),
+    # val.py rect batches (ceil(shape * 640 / 32 + 0.5) * 32) on uint8 images: a square image runs at 672x672, so the
+    # P5 / P4 / P3 grids are 21, 42 and 84 wide (odd), the stride-2 patches overhang them and model.16 upsamples 21 -> 42
+    "val_yolov3_672x672_bs8_u8": dict(model=_bench_yolov3, bs=8, h=672, w=672, u8=True, fp8=False, n_conv=74,
+                                      need=TMA | N256),
+    # a 4:3 image: SPP's cascaded 5x5 pools on 16x21 maps
+    "val_yolov3-spp_512x672_bs4_u8": dict(model=lambda: _model("yolov3-spp.yaml"), bs=4, h=512, w=672, u8=True,
+                                          fp8=False, n_conv=75, need=TMA | N256),
+    # a portrait image through yolov3-tiny: k2s2 pools down to 21x16, ZeroPad2d + MaxPool2d(2, 1) there, odd bs
+    "val_yolov3-tiny_672x512_bs5_u8": dict(model=lambda: _model("yolov3-tiny.yaml"), bs=5, h=672, w=512, u8=True,
+                                           fp8=False, n_conv=12, need={"tma_flat"}, sens=SENSITIVITY_TINY),
+    # detect.py's Pipeline: bs 1 uint8 at the auto-letterbox shapes of zidane.jpg and (e4m3) bus.jpg
+    "detect_yolov3_384x640_bs1_u8": dict(model=_bench_yolov3, bs=1, h=384, w=640, u8=True, fp8=False, n_conv=74,
+                                         need=TMA | N256),
+    "detect_yolov3_640x480_bs1_u8_fp8": dict(model=_bench_yolov3, bs=1, h=640, w=480, u8=True, fp8=True, n_conv=74,
+                                             need=TMA | N256),
+    # e4m3 SPP pools at 21x21, calibrated at 640x640
+    "val_yolov3-spp_672x672_bs4_u8_fp8": dict(model=lambda: _model("yolov3-spp.yaml"), bs=4, h=672, w=672, u8=True,
+                                              fp8=True, n_conv=75, need=TMA | N256),
+    # train.py --multi-scale's 416: a 13x13 P5 grid, the ZeroPad2d pool on an odd grid
+    "yolov3-tiny_416x416_bs3": dict(model=lambda: _model("yolov3-tiny.yaml"), bs=3, h=416, w=416, fp8=False,
+                                    n_conv=12, need={"tma_flat"}, sens=SENSITIVITY_TINY),
 }
-# launches on which the damaged references are tried (besides the first head, the first pool and the decode)
-SENSITIVITY = {"model.2.cv1", "model.2.cv2", "model.16", "model.8.7.cv2"}
 
 
 @pytest.mark.parametrize("which", list(ENGINES))
@@ -267,15 +303,15 @@ def test_engine_every_launch_whole_batch(which):
     from yolov3_b200 import _lib
     from yolov3_b200.tensors import PaddedNHWC
 
-    spec = ENGINES[which]
+    spec = dict(h=640, w=640, u8=False, sens=SENSITIVITY) | ENGINES[which]
     m = spec["model"]()
-    bs = spec["bs"]
-    if spec["fp8"]:  # tools/bench_fp8.py: calibrated on one seeded batch that is not the one run
+    bs, h, w, u8, sens = (spec[k] for k in ("bs", "h", "w", "u8", "sens"))
+    if spec["fp8"]:  # tools/bench_fp8.py: calibrated on one seeded 640x640 batch that is not the one run
         m.calibrate_fp8([torch.rand(bs, 3, 640, 640, generator=torch.Generator().manual_seed(1000)).cuda()])
         m.precision = "fp8"
         torch.cuda.empty_cache()
-    e = m.engine(bs, 640, 640, torch.float32)
-    e.static_in.copy_(_inputs(bs, 1))
+    e = m.engine(bs, h, w, torch.uint8, 255.0) if u8 else m.engine(bs, h, w, torch.float32)
+    e.static_in.copy_(_inputs(bs, h, w, u8, 1))
     L = _lib.lib()
     W = m.packed()
     acts = {}
@@ -356,7 +392,7 @@ def test_engine_every_launch_whole_batch(which):
                 if not ok:
                     err = (got.float() - ref / out.scale).abs() / l1.clamp_min(1e-30) * out.scale
                     bad.append(f"{where}: e4m3 codes failed; largest err/L1 at {_where(err, int(err.view(-1).argmax()))}")
-                if name in SENSITIVITY:  # a 1 % channel shift is far below half an e4m3 step: not tried
+                if name in sens:  # a 1 % channel shift is far below half an e4m3 step: not tried
                     tries = [tile_from_next_image(ref)] + \
                         ([residual_missing(ref, res)] if res is not None and not d.upsample else [])
                     damaged[name] = [not e4m3_ok(got, dr / out.scale, l1 / out.scale, f"{name} damaged reference")[0]
@@ -368,7 +404,7 @@ def test_engine_every_launch_whole_batch(which):
                 print(f"{which} {where}: worst err/bound {r:.3f}, err/(1.1 L1) {meas:.2e}, exact {exact:.4%}")
                 if not bf16_ok((r, meas, exact)):
                     bad.append(f"{where}: worst err/bound {r:.3f} at image/row/col/channel {pos}, exact {exact:.4%}")
-                if name in SENSITIVITY:
+                if name in sens:
                     tries = [tile_from_next_image(ref), channel_shifted(ref)] + \
                         ([residual_missing(ref, res)] if res is not None and not d.upsample else [])
                     damaged[name] = [not bf16_ok(check_bf16(got, dr, l1)) for dr in tries]
@@ -385,7 +421,8 @@ def test_engine_every_launch_whole_batch(which):
             torch.cuda.synchronize()
             e.check_errors()
             wt = w27.t().reshape(f.c_out, 3, 3, 3)
-            ref = F.silu(F.conv2d(e.static_in, wt, b, padding=1)).permute(0, 2, 3, 1)
+            x0 = e.static_in.float() / 255 if u8 else e.static_in
+            ref = F.silu(F.conv2d(x0, wt, b, padding=1)).permute(0, 2, 3, 1)
             got = out.values()
             r = float(((got - ref).abs() / (1e-2 + 1e-2 * ref.abs())).max())
             halo, side = untouched(out.buf, before, out.coff, out.c)
@@ -435,9 +472,8 @@ def test_engine_every_launch_whole_batch(which):
         assert n_conv == spec["n_conv"], n_conv
     assert not bad, "\n".join(bad[:20])
     assert damaged and all(all(v) for v in damaged.values()), damaged
-    need = {"tma_flat", "tma_patch"} | ({"n256_upsample", "n256_res_coff"} if which.startswith("yolov3_") else set()) | \
-        ({"halo_64_128"} if which == "yolov3_bf16" else set())
-    assert need <= cover, (need - cover)
+    assert sens <= set(damaged), sens - set(damaged)
+    assert spec["need"] <= cover, (spec["need"] - cover)
 
 
 # ------------------------------------------------------------------------------------------------ 2. N = 256 store-warp units
@@ -629,10 +665,12 @@ def check_train_blocks(te, P, worst, bad, tag="train"):
                 check_abs(b.dbeta, channel_shifted(dbeta_ref.view(1, 1, 1, c)).view(c), l1b, EPS_BN)[0] > 1,
                 check_abs(b.dgamma, channel_shifted(dgamma_ref.view(1, 1, 1, c)).view(c), l1g, EPS_BN)[0] > 1]
         del dz, yhat
-        # ---- wgrad from the stored dy and x
+        # ---- wgrad from the stored dy and x.  The reference sums in float64: cuDNN's float32 wgrad is off the exact sum by
+        #      up to 3.6e-6 L1 (1x1) and 9.0e-5 L1 (3x3) at yolov3-spp 480x640 bs 4, as much as EPS_W allows the kernel
         dyc = _nchw(dy_got.float())
         shape = (b.c2, 27, 1, 1) if b.first else tuple(w.shape)
-        dw_ref = torch.nn.grad.conv2d_weight(xc, shape, dyc, stride=s, padding=p)
+        xd, dyd = xc.double(), dyc.double()
+        dw_ref = torch.nn.grad.conv2d_weight(xd, shape, dyd, stride=s, padding=p)
         l1 = torch.nn.grad.conv2d_weight(xc.abs(), shape, dyc.abs(), stride=s, padding=p)
         dw_got = P[pre + ".conv.weight"].grad.reshape(shape)
         eps_w = EPS_W[b.k]
@@ -646,12 +684,12 @@ def check_train_blocks(te, P, worst, bad, tag="train"):
             lo = npx // 132 * 66
             dd = dy_got.float().clone()
             dd.view(-1, c)[lo:lo + npx // 132] = 0
-            dw_d = torch.nn.grad.conv2d_weight(xc, shape, _nchw(dd), stride=s, padding=p)
+            dw_d = torch.nn.grad.conv2d_weight(xd, shape, _nchw(dd).double(), stride=s, padding=p)
             damaged["dW"] = [check_abs(dw_got, dw_d, l1, eps_w)[0] > 1,
                              check_abs(dw_got, channel_shifted(dw_ref.permute(0, 2, 3, 1)).permute(0, 3, 1, 2), l1,
                                        eps_w)[0] > 1]
             del dd, dw_d
-        del dw_ref, l1
+        del dw_ref, l1, xd, dyd
         # ---- dgrad where this block is the only contribution to its input (plus a Bottleneck shortcut gradient)
         key = (b.x.buf.data_ptr(), b.x.coff, b.x.c)
         if (not b.first and n_contrib[key] == 1 and key not in head_inputs and b.x.buf.data_ptr() not in pooled

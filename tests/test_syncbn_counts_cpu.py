@@ -25,7 +25,8 @@ want = [float(2 * (320 // s) * (320 // s) + 3 * (640 // s) * (480 // s)) for s i
 assert got == want, (got, want)
 same = bn_counts([mine, mine], h, w, grids)            # equal shapes: count * world, as before
 assert same == [float(2 * n * gh * gw) for gh, gw in grids], same
-print("COUNTS_OK", r)
+sys.stdout.write(f"COUNTS_OK {r}\n")  # one write: the ranks share the pipe, and print's pieces interleave
+sys.stdout.flush()
 dist.barrier(); dist.destroy_process_group()
 '''
 

@@ -23,7 +23,7 @@ operands:
                        reads as da must have a contributor
   Detect heads         out == conv2d(x, bf16(w)) + b (check_head, EPS_HEAD), pad column 0; raw is a bit-exact re-layout
                        of out; dy[..., :255] == bf16(dL/draw), pad column 0; db within EPS_BN sum |dL/draw| of the column
-                       sums; dW within EPS_W[1] conv2d_weight(|x|, |dy|), pad row 0
+                       sums; dW within EPS_W[1] conv2d_weight(|x|, |dy|) of a float64 reference, pad row 0
   every block          test_bench_engines_gpu.check_train_blocks (its constants and damaged references), except for
                        yolov3 640x640, which test_bench_engines_gpu runs
   max-pool forwards    dst == F.max_pool2d of the stored src, exactly
@@ -276,7 +276,7 @@ def check_heads(te, P, worst, bad):
         if not (rb[0] <= 1 and bool((hd["db"][co:] == 0).all())):
             bad.append(f"{tag} db: worst err/bound {rb[0]:.3f}")
         dyc = _nchw(dy[..., :co].float())
-        dw_ref = torch.nn.grad.conv2d_weight(xc, (co, x.c, 1, 1), dyc)
+        dw_ref = torch.nn.grad.conv2d_weight(xc.double(), (co, x.c, 1, 1), dyc.double())  # as check_train_blocks
         l1w = torch.nn.grad.conv2d_weight(xc.abs(), (co, x.c, 1, 1), dyc.abs())
         dw = hd["dw"]
         rw = check_abs(dw[:co].reshape(co, x.c, 1, 1), dw_ref, l1w, EPS_W[1])
@@ -322,6 +322,10 @@ CASES = {
     "yolov3-tiny_640_bs8": dict(cfg="yolov3-tiny.yaml", n=8, h=640, w=640, blocks=True),
     # a multi-scale / rect training shape: detect grids 11x19, 22x38, 44x76
     "yolov3_352x608_bs4": dict(cfg="yolov3.yaml", n=4, h=352, w=608, blocks=True),
+    # train.py --multi-scale at 416: a 13x13 P5 grid under the ZeroPad2d + MaxPool2d(2, 1) route
+    "yolov3-tiny_416_bs4": dict(cfg="yolov3-tiny.yaml", n=4, h=416, w=416, blocks=True),
+    # a train.py --rect shape: SPP's pools on 15x20
+    "yolov3-spp_480x640_bs4": dict(cfg="yolov3-spp.yaml", n=4, h=480, w=640, blocks=True),
 }
 
 
