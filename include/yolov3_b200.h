@@ -234,7 +234,8 @@ int y3_scale_boxes(float* boxes, int64_t n, int32_t row_stride, float pad_x, flo
 
 /* ---------------------------------------------------------------------------------------------------------------
  * Training loss, forward + backward.  Replaces ComputeLoss.__call__ / build_targets (utils/loss.py:131-244) with
- * bbox_iou(CIoU) and BCEWithLogitsLoss(pos_weight), for fl_gamma = 0, autobalance off, gr = 1 (the shipped hyps).
+ * bbox_iou(CIoU) and BCEWithLogitsLoss(pos_weight), FocalLoss around both BCE terms when fl_gamma > 0
+ * (loss.py:31-63, 117-119) and the autobalance update of the objectness balance (loss.py:171-175); gr = 1.
  *   p[l]     fp32 [bs, na, ny_l, nx_l, nc+5] raw logits (train-mode Detect output, models/yolo.py:110)
  *   grad[l]  same shape (or NULL): receives d(out[0])/dp[l] * grad_scale
  *   targets  fp32 [nt, 6] = (image, class, x, y, w, h) normalised (collate_fn, utils/dataloaders.py:825-830)
@@ -252,8 +253,14 @@ typedef struct y3_loss_desc {
   float cls_pw, obj_pw;      /* BCE pos_weight */
   float anchor_t;
   float cp, cn;              /* smooth_bce(label_smoothing) targets */
-  float balance[Y3_MAX_LEVELS];
+  float balance[Y3_MAX_LEVELS];  /* objectness balance (autobalance = 0) */
   float grad_scale;          /* upstream gradient of out[0] (1 for loss.backward()) */
+  double fl_gamma;           /* focal loss gamma: 0 = plain BCE, else finite and > 0 */
+  double fl_alpha;           /* focal loss alpha (0.25) */
+  int32_t autobalance;       /* 1: the balance is read from bal_state, updated there and normalised by bal_state[ssi] */
+  int32_t ssi;               /* index of the stride-16 level in bal_state */
+  int32_t n_balance;         /* entries of bal_state (nl <= n_balance <= Y3_MAX_LEVELS) */
+  double* bal_state;         /* device fp64 [n_balance], autobalance = 1 only; carries from call to call */
 } y3_loss_desc;
 int64_t y3_loss_workspace_bytes(const y3_loss_desc* d);
 int y3_loss_fwd_bwd(const y3_loss_desc* d, void* workspace, int64_t workspace_bytes, float* out, y3_stream_t stream);

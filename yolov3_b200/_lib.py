@@ -121,7 +121,10 @@ class LossDesc(C.Structure):
                 ("box", C.c_float), ("obj", C.c_float), ("cls", C.c_float),
                 ("cls_pw", C.c_float), ("obj_pw", C.c_float), ("anchor_t", C.c_float),
                 ("cp", C.c_float), ("cn", C.c_float),
-                ("balance", C.c_float * MAX_LEVELS), ("grad_scale", C.c_float)]
+                ("balance", C.c_float * MAX_LEVELS), ("grad_scale", C.c_float),
+                ("fl_gamma", C.c_double), ("fl_alpha", C.c_double),
+                ("autobalance", C.c_int32), ("ssi", C.c_int32), ("n_balance", C.c_int32),
+                ("bal_state", C.c_void_p)]
 
 
 class BnActDesc(C.Structure):

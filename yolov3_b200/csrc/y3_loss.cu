@@ -6,10 +6,15 @@
 //   K2 matches  : one warp per match — gather logits, decode box, CIoU (+ analytic gradient by forward-mode duals),
 //                 class BCE (+ gradient), IoU -> tobj with last-write-wins in REFERENCE order (loss.py:144-167)
 //   K3 obj      : dense objectness BCE over every cell + its gradient (loss.py:169-170)
-//   K4 finalize : means, balance, hyp gains, x batch size (loss.py:176-181)
+//   K4 finalize : means, balance, hyp gains, x batch size (loss.py:176-181); with autobalance the fp64 balance state is
+//                 read, updated per level after its term and normalised by balance[ssi] (loss.py:171-175)
+// fl_gamma > 0 wraps the class BCE of K2 and the objectness BCE of K3 in FocalLoss (loss.py:31-63); fl_gamma = 0 takes
+// the plain BCE branch, the code path without the focal factor.
 // grads must be zeroed by the caller's stream before K2 (done in y3_loss_fwd_bwd with one memset per level).
 // Compiled without fast-math / FMA contraction (see build.py EXACT_SOURCES).
 #include <math_constants.h>
+
+#include <cmath>
 
 #include "y3_common.cuh"
 #include "y3_internal.h"
@@ -162,6 +167,58 @@ __device__ __forceinline__ float bce_logits(float x, float t, float pw, float* d
   return (1.0f - t) * x + lw * sp;
 }
 
+// FocalLoss(BCEWithLogitsLoss(pos_weight), gamma, alpha) of one element (loss.py:45-56) and d/dx for a unit upstream
+// gradient.  The forward is the reference's op sequence in float32: p_t = t*s + (1-t)*(1-s), a = t*alpha + (1-t)*(1-alpha),
+// m = (1-p_t)^gamma, loss = bce * (a*m).  The backward follows autograd's chain through the same ops: the bce path gets
+// a*m, the modulating path bce*a * gamma*(1-p_t)^(gamma-1) through p_t and sigmoid.  Where the sigmoid saturates and
+// 1-p_t is 0, (1-p_t)^(gamma-1) is inf for gamma < 1 and the p_t backward forms inf*0 = NaN, as autograd does.
+struct Focal {
+  float gamma, gm1, alpha, alpha0;  // gamma, gamma - 1, alpha, 1 - alpha (each rounded from double once, as torch does)
+  int mode, mode1;                  // tpow modes of gamma and gamma - 1
+};
+// torch.pow(float32 tensor, scalar e) on CUDA: the exponents it special-cases (pow(e == 0) fills 1, e == 1 copies, 0.5
+// sqrt, 2 and 3 products, -0.5 rsqrt, -1 reciprocal, -2 reciprocal of the square), powf(x, float(e)) elsewhere
+__device__ __forceinline__ int tpow_mode(double e) {
+  return e == 0.0 ? 0 : e == 1.0 ? 1 : e == 0.5 ? 2 : e == 2.0 ? 3 : e == 3.0 ? 4 : e == -0.5 ? 5 : e == -1.0 ? 6
+       : e == -2.0 ? 7 : 8;
+}
+__device__ __forceinline__ float tpow(float x, int mode, float e) {
+  switch (mode) {
+    case 0: return 1.0f;
+    case 1: return x;
+    case 2: return sqrtf(x);
+    case 3: return x * x;
+    case 4: return x * x * x;
+    case 5: return rsqrtf(x);
+    case 6: return 1.0f / x;
+    case 7: return 1.0f / (x * x);
+    default: return powf(x, e);
+  }
+}
+__device__ __forceinline__ Focal focal_of(const y3_loss_desc& d) {
+  Focal f;
+  f.gamma = static_cast<float>(d.fl_gamma);
+  f.gm1 = static_cast<float>(d.fl_gamma - 1.0);
+  f.alpha = static_cast<float>(d.fl_alpha);
+  f.alpha0 = static_cast<float>(1.0 - d.fl_alpha);
+  f.mode = tpow_mode(d.fl_gamma);
+  f.mode1 = tpow_mode(d.fl_gamma - 1.0);
+  return f;
+}
+__device__ __forceinline__ float focal_bce_logits(float x, float t, float pw, const Focal& f, float* dx) {
+  float dbce;
+  const float bce = bce_logits(x, t, pw, &dbce);
+  const float s = sigmoidf_(x);
+  const float pt = t * s + (1.0f - t) * (1.0f - s);
+  const float af = t * f.alpha + (1.0f - t) * f.alpha0;
+  const float base = 1.0f - pt;
+  const float w = af * tpow(base, f.mode, f.gamma);
+  const float g_pt = -((bce * af) * (f.gamma * tpow(base, f.mode1, f.gm1)));  // d/d(p_t) through m
+  const float g_s = g_pt * t + -(g_pt * (1.0f - t));                         // p_t's two uses of s
+  *dx = w * dbce + g_s * (1.0f - s) * s;                                      // sigmoid backward: g * (1 - s) * s
+  return bce * w;
+}
+
 // ---------------------------------------------------------------------------------------------- K2
 __global__ void __launch_bounds__(256) loss_matches_kernel(const LossArgs p, int l) {
   pdl_entry();
@@ -197,10 +254,19 @@ __global__ void __launch_bounds__(256) loss_matches_kernel(const LossArgs p, int
   if (d.nc > 1) {
     float sum = 0.f;
     const float k = d.cls * static_cast<float>(d.bs) * inv_n / static_cast<float>(d.nc) * d.grad_scale;
-    for (int c = lane; c < d.nc; c += 32) {
-      float dx;
-      sum += bce_logits(ps[5 + c], c == m.cls ? d.cp : d.cn, d.cls_pw, &dx);
-      if (gs) atomicAdd(gs + 5 + c, k * dx);
+    if (d.fl_gamma > 0.0) {
+      const Focal f = focal_of(d);
+      for (int c = lane; c < d.nc; c += 32) {
+        float dx;
+        sum += focal_bce_logits(ps[5 + c], c == m.cls ? d.cp : d.cn, d.cls_pw, f, &dx);
+        if (gs) atomicAdd(gs + 5 + c, k * dx);
+      }
+    } else {
+      for (int c = lane; c < d.nc; c += 32) {
+        float dx;
+        sum += bce_logits(ps[5 + c], c == m.cls ? d.cp : d.cn, d.cls_pw, &dx);
+        if (gs) atomicAdd(gs + 5 + c, k * dx);
+      }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
@@ -214,15 +280,29 @@ __global__ void __launch_bounds__(256) loss_obj_kernel(const LossArgs p, int l) 
   const y3_loss_desc& d = p.d;
   const int no = d.nc + 5;
   const size_t cells = static_cast<size_t>(d.bs) * d.na * d.ny[l] * d.nx[l];
-  const float k = d.obj * static_cast<float>(d.bs) * d.balance[l] / static_cast<float>(cells) * d.grad_scale;
+  // obji * balance[i] multiplies by a Python double, which torch rounds to float32 (loss.py:170)
+  const float bal = d.autobalance ? static_cast<float>(d.bal_state[l]) : d.balance[l];
+  const float k = d.obj * static_cast<float>(d.bs) * bal / static_cast<float>(cells) * d.grad_scale;
   float sum = 0.f;
-  for (size_t i = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x; i < cells;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const unsigned long long key = p.tobj_key[l][i];
-    const float t = key ? __uint_as_float(static_cast<unsigned int>(key & 0xFFFFFFFFull)) : 0.0f;
-    float dx;
-    sum += bce_logits(d.p[l][i * no + 4], t, d.obj_pw, &dx);
-    if (d.grad[l]) d.grad[l][i * no + 4] = k * dx;
+  const size_t i0 = static_cast<size_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const size_t stride = static_cast<size_t>(gridDim.x) * blockDim.x;
+  if (d.fl_gamma > 0.0) {
+    const Focal f = focal_of(d);
+    for (size_t i = i0; i < cells; i += stride) {
+      const unsigned long long key = p.tobj_key[l][i];
+      const float t = key ? __uint_as_float(static_cast<unsigned int>(key & 0xFFFFFFFFull)) : 0.0f;
+      float dx;
+      sum += focal_bce_logits(d.p[l][i * no + 4], t, d.obj_pw, f, &dx);
+      if (d.grad[l]) d.grad[l][i * no + 4] = k * dx;
+    }
+  } else {
+    for (size_t i = i0; i < cells; i += stride) {
+      const unsigned long long key = p.tobj_key[l][i];
+      const float t = key ? __uint_as_float(static_cast<unsigned int>(key & 0xFFFFFFFFull)) : 0.0f;
+      float dx;
+      sum += bce_logits(d.p[l][i * no + 4], t, d.obj_pw, &dx);
+      if (d.grad[l]) d.grad[l][i * no + 4] = k * dx;
+    }
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
@@ -248,7 +328,18 @@ __global__ void loss_finalize_kernel(const LossArgs p) {
       lbox += static_cast<float>(p.acc[l * 3 + 0] / n);
       if (d.nc > 1) lcls += static_cast<float>(p.acc[l * 3 + 1] / (static_cast<double>(n) * d.nc));
     }
-    lobj += static_cast<float>(p.acc[l * 3 + 2] / cells) * d.balance[l];
+    const float obji = static_cast<float>(p.acc[l * 3 + 2] / cells);
+    if (d.autobalance) {  // term first, then balance[i] = balance[i] * 0.9999 + 0.0001 / obji.item() in fp64
+      const double b = d.bal_state[l];
+      lobj += obji * static_cast<float>(b);
+      d.bal_state[l] = b * 0.9999 + 0.0001 / static_cast<double>(obji);
+    } else {
+      lobj += obji * d.balance[l];
+    }
+  }
+  if (d.autobalance) {  // balance = [x / balance[ssi] for x in balance], every entry, by the pre-loop divisor
+    const double s = d.bal_state[d.ssi];
+    for (int i = 0; i < d.n_balance; ++i) d.bal_state[i] = d.bal_state[i] / s;
   }
   lbox *= d.box;
   lobj *= d.obj;
@@ -282,6 +373,14 @@ extern "C" int y3_loss_fwd_bwd(const y3_loss_desc* d, void* workspace, int64_t w
   Y3_REQUIRE(d->nl >= 1 && d->nl <= Y3_MAX_LEVELS && d->na >= 1 && d->na <= Y3_MAX_ANCHORS && d->bs > 0 && d->nc >= 1,
              "loss: bad shape");
   Y3_REQUIRE(d->nt >= 0 && (d->nt == 0 || d->targets), "loss: bad targets");
+  Y3_REQUIRE(std::isfinite(d->fl_gamma) && d->fl_gamma >= 0.0, "loss: fl_gamma must be finite and >= 0, got %g",
+             d->fl_gamma);
+  Y3_REQUIRE(d->fl_gamma == 0.0 || (std::isfinite(d->fl_alpha) && d->fl_alpha >= 0.0 && d->fl_alpha <= 1.0),
+             "loss: fl_alpha must be in [0, 1], got %g", d->fl_alpha);
+  Y3_REQUIRE(d->autobalance == 0 || d->autobalance == 1, "loss: autobalance must be 0 or 1");
+  Y3_REQUIRE(!d->autobalance || (d->bal_state && d->n_balance >= d->nl && d->n_balance <= Y3_MAX_LEVELS &&
+                                 d->ssi >= 0 && d->ssi < d->n_balance),
+             "loss: autobalance needs bal_state with nl..%d entries and 0 <= ssi < n_balance", Y3_MAX_LEVELS);
   Y3_REQUIRE(workspace_bytes >= y3_loss_workspace_bytes(d), "loss: workspace too small");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   LossArgs a{};

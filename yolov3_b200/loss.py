@@ -4,6 +4,7 @@ costs nothing more than handing those gradients to autograd."""
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import torch
 
@@ -42,24 +43,49 @@ class _LossFn(torch.autograd.Function):
 
 
 class ComputeLoss:
-    """Drop-in for utils/loss.py:98.  ``model`` needs ``.hyp`` and a Detect info at ``.model[-1]`` (na, nc, nl, anchors)."""
+    """Drop-in for utils/loss.py:98.  ``model`` needs ``.hyp`` and a Detect info at ``.model[-1]`` (na, nc, nl, anchors,
+    stride).  ``hyp["fl_gamma"] > 0`` wraps the class and objectness BCE in FocalLoss(gamma, alpha=0.25) (loss.py:117-119).
+    With ``autobalance`` the balance list lives in a float64 device buffer that the kernels update at every call
+    (loss.py:171-175); reading ``balance`` copies it to the host, and is the only host synchronisation of the loss."""
 
     sort_obj_iou = False
+    fl_alpha = 0.25  # FocalLoss's default alpha, the one ComputeLoss uses (loss.py:34, 119)
 
     def __init__(self, model, autobalance=False):
-        if autobalance:
-            raise NotImplementedError("autobalance is off in every shipped configuration and is not accelerated")
         h = model.hyp
-        if h.get("fl_gamma", 0.0) > 0:
-            raise NotImplementedError("focal loss (fl_gamma > 0) is not part of the accelerated path (SURVEY §2.1)")
+        g = float(h.get("fl_gamma", 0.0))
+        if not (math.isfinite(g) and g >= 0.0):
+            raise ValueError(f"hyp fl_gamma must be finite and >= 0, got {h.get('fl_gamma')!r}")
         m = model.model[-1]
         self.hyp = h
+        self.fl_gamma = g
         self.cp, self.cn = smooth_bce(eps=h.get("label_smoothing", 0.0))
-        self.balance = {3: [4.0, 1.0, 0.4]}.get(m.nl, [4.0, 1.0, 0.25, 0.06, 0.02])  # utils/loss.py:122
-        self.gr, self.autobalance = 1.0, False
+        self._balance = {3: [4.0, 1.0, 0.4]}.get(m.nl, [4.0, 1.0, 0.25, 0.06, 0.02])  # utils/loss.py:122
+        self.ssi = [float(s) for s in m.stride].index(16.0) if autobalance else 0  # utils/loss.py:123
+        self.gr, self.autobalance = 1.0, bool(autobalance)
         self.na, self.nc, self.nl = m.na, m.nc, m.nl
         self.anchors = m.anchors.detach().float().cpu()
         self._ws = None
+        self._bal = None  # autobalance: float64 device copy of the balance list, created by the first call
+
+    @property
+    def balance(self):
+        """The reference's ``self.balance`` list.  With autobalance the kernels own it: this copies it from the device."""
+        if self._bal is not None:
+            return self._bal.tolist()
+        return self._balance
+
+    @balance.setter
+    def balance(self, v):
+        self._balance = [float(x) for x in v]
+        self._bal = None
+
+    def _balance_state(self, dev):
+        if self._bal is None or self._bal.device != dev:
+            start = self.balance  # from the old device first, when the loss moves
+            # pinned source + non_blocking: the upload does not synchronise the host
+            self._bal = torch.tensor(start, dtype=torch.float64).pin_memory().to(dev, non_blocking=True)
+        return self._bal
 
     def _run(self, p, targets, want_grad=True):
         dev = p[0].device
@@ -74,7 +100,7 @@ class ComputeLoss:
             d.p[l] = x.data_ptr()
             d.grad[l] = grads[l].data_ptr() if want_grad else None
             d.ny[l], d.nx[l] = x.shape[2], x.shape[3]
-            d.balance[l] = self.balance[l]
+            d.balance[l] = self._balance[l]
             for a in range(self.na):
                 d.anchors[l][a][0], d.anchors[l][a][1] = float(self.anchors[l, a, 0]), float(self.anchors[l, a, 1])
         d.targets, d.nt = (t.data_ptr() if t.shape[0] else None), t.shape[0]
@@ -82,6 +108,10 @@ class ComputeLoss:
         d.box, d.obj, d.cls = h["box"], h["obj"], h["cls"]
         d.cls_pw, d.obj_pw, d.anchor_t = h["cls_pw"], h["obj_pw"], h["anchor_t"]
         d.cp, d.cn, d.grad_scale = self.cp, self.cn, 1.0
+        d.fl_gamma, d.fl_alpha = self.fl_gamma, self.fl_alpha
+        if self.autobalance:
+            bal = self._balance_state(dev)
+            d.autobalance, d.ssi, d.n_balance, d.bal_state = 1, self.ssi, bal.numel(), bal.data_ptr()
         L = _lib.lib()
         need = L.y3_loss_workspace_bytes(C.byref(d))
         if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
