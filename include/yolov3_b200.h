@@ -402,7 +402,14 @@ int y3_letterbox_u8(const y3_letterbox_desc* d, y3_stream_t stream);
  *   sources (canvas rectangle [x0, x1) x [y0, y1), canvas pixel (X, Y) = source pixel (X - off_x, Y - off_y)), 114 elsewhere
  *   (load_mosaic's img4 or letterbox's border, never materialised); with mixup, the same of canvas[1] blended as
  *   trunc(a r + b (1 - r)) in double; with hsv, cv2's BGR2HSV, the three LUTs and HSV2BGR (augment_hsv); then flipud /
- *   fliplr and the HWC BGR -> CHW RGB store. */
+ *   fliplr and the HWC BGR -> CHW RGB store.  A descriptor with dst == NULL writes out[i]; one with dst set writes its
+ *   out_h x out_w image at dst instead, rows dst_pitch bytes and planes dst_plane bytes apart (a quadrant of a 2x2 tile,
+ *   a scratch image; collate_fn4 of train.py --quad).
+ * y3_upsample2x_u8: collate_fn4's F.interpolate(scale_factor=2, bilinear, align_corners=False) and the cast back to uint8,
+ *   in its exact integer form: per axis, output 2k = (x[k-1] + 3 x[k]) / 4 and 2k+1 = (3 x[k] + x[k+1]) / 4 with the
+ *   indices clamped to the image; the product of the two axes' quarter weights over 16, truncated.  src: n uint8 CHW
+ *   [3, h, w] images, contiguous; image k is written to out[dst_index[k]] of out [*, 3, 2h, 2w].  dst_index is in DEVICE
+ *   memory. */
 typedef struct y3_resize_item {
   const void* src; int32_t src_h, src_w, src_pitch;
   void* dst;       int32_t dst_h, dst_w, dst_pitch;
@@ -427,8 +434,13 @@ typedef struct y3_augment_desc {
   int32_t mixup, hsv, flipud, fliplr;
   double mix_r;                 /* np.random.beta(32, 32) */
   uint8_t lut[3][256];          /* hue, saturation, value */
+  void* dst;                    /* NULL: out[i] */
+  int64_t dst_plane;            /* with dst: bytes between the R, G and B planes ... */
+  int32_t dst_pitch, reserved;  /* ... and between rows */
 } y3_augment_desc;
 int y3_augment_u8(const y3_augment_desc* descs, int32_t n, int32_t out_h, int32_t out_w, void* out, y3_stream_t stream);
+int y3_upsample2x_u8(const void* src, const int32_t* dst_index, int32_t n, int32_t h, int32_t w, void* out,
+                     y3_stream_t stream);
 
 /* Validation loader on the device (LoadImagesAndLabels.__getitem__ with augment=False, utils/dataloaders.py:676-686,
  * 699-756) — csrc/y3_augment.cu.  Both entry points read their item array from DEVICE memory (`items` / `descs`) and take

@@ -195,7 +195,8 @@ class AugmentDesc(C.Structure):
     """struct y3_augment_desc."""
 
     _fields_ = [("canvas", AugCanvas * 2), ("mixup", C.c_int32), ("hsv", C.c_int32), ("flipud", C.c_int32),
-                ("fliplr", C.c_int32), ("mix_r", C.c_double), ("lut", (C.c_uint8 * 256) * 3)]
+                ("fliplr", C.c_int32), ("mix_r", C.c_double), ("lut", (C.c_uint8 * 256) * 3), ("dst", C.c_void_p),
+                ("dst_plane", C.c_int64), ("dst_pitch", C.c_int32), ("reserved", C.c_int32)]
 
 
 class PackItem(C.Structure):
@@ -239,14 +240,26 @@ class JpegDesc(C.Structure):
 
 class Regions:
     """Lays out a staging buffer the kernels read: each ``take(nbytes)`` returns the offset of the next region, 256-byte
-    aligned (the alignment every pointer handed to a kernel gets); ``size`` is the bytes taken so far."""
+    aligned (the alignment every pointer handed to a kernel gets); ``size`` is the bytes taken so far.  ``scratch(nbytes)``
+    takes a region that only the device writes and reads: the host fills and copies the first ``copied`` bytes, so every
+    ``take`` comes before the first ``scratch``."""
 
     ALIGN = 256
 
     def __init__(self):
         self.size = 0
+        self.copied = None  # None: every region is copied
 
     def take(self, nbytes):
+        assert self.copied is None, "a copied region after a scratch region"
+        return self._next(nbytes)
+
+    def scratch(self, nbytes):
+        if self.copied is None:
+            self.copied = self.size
+        return self._next(nbytes)
+
+    def _next(self, nbytes):
         off = self.size
         self.size += (int(nbytes) + self.ALIGN - 1) // self.ALIGN * self.ALIGN
         return off
@@ -280,6 +293,7 @@ def _declare(lib):
         "y3_letterbox_u8": ([C.POINTER(LetterboxDesc), vp], C.c_int),
         "y3_resize_u8_batched": ([vp, vp, i32, vp], C.c_int),
         "y3_augment_u8": ([vp, i32, i32, i32, vp, vp], C.c_int),
+        "y3_upsample2x_u8": ([vp, vp, i32, i32, i32, vp, vp], C.c_int),
         "y3_resize_area_u8_batched": ([vp, vp, i32, vp], C.c_int),
         "y3_letterbox_u8_batched": ([vp, vp, i32, vp], C.c_int),
         "y3_scale_img_f32": ([vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, C.c_float, vp, vp], C.c_int),

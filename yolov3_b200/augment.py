@@ -10,7 +10,9 @@ labels' tail of ``__getitem__`` once for both planners (``yolov3_b200.valloader.
 ``DeviceLoader`` (on ``yolov3_b200.loader.BatchLoader``: reads, staging, JPEG decode) packs a batch's y3_resize_item and
 y3_augment_desc arrays and runs two launches — ``y3_resize_u8_batched`` (load_image's cv2.resize of every source, then
 letterbox's second resize) and ``y3_augment_u8`` (everything else, written as uint8 CHW RGB into the ``[bs, 3, H, W]``
-batch).
+batch).  With ``quad=True`` (train.py --quad) the batch is collate_fn4's instead (``plan_quad``): ``y3_augment_u8`` writes
+each item of a 2x2 tile straight into its quadrant of the ``[bs // 4, 3, 2H, 2W]`` batch, and ``y3_upsample2x_u8`` the 2x
+bilinear image of each upsampled quad's leader, which the augment launch wrote into scratch.
 
 Refused when the loader is built (NotImplementedError): ``perspective > 0`` (warpPerspective), segment (polygon) labels,
 an active Albumentations transform, and ``augment=False`` (served by ``yolov3_b200.valloader.DeviceValLoader``)."""
@@ -22,6 +24,7 @@ import random
 from dataclasses import dataclass, field
 
 import numpy as np
+import torch
 
 from . import _lib
 from .loader import BatchLoader, load_hw
@@ -283,6 +286,48 @@ def plan_item(dataset, index):
     return plan, labels_out(labels, out_hw, flipud, fliplr)
 
 
+# ------------------------------------------------------------------------------------------------------- collate_fn4
+QUAD_HO = np.array([[0.0, 0, 0, 1, 0, 0]], dtype=np.float32)  # the tile's bottom half: y + 1 ...
+QUAD_WO = np.array([[0.0, 0, 1, 0, 0, 0]], dtype=np.float32)  # ... its right half: x + 1 ...
+QUAD_S = np.array([[1, 1, 0.5, 0.5, 0.5, 0.5]], dtype=np.float32)  # ... then xywh halved
+
+
+@dataclass
+class QuadPlan:
+    """collate_fn4 (utils/dataloaders.py:833-858) of one batch: quad q is items 4q..4q+3 of `plans`; ``upsample[q]``: its
+    leader 2x bilinear, else the 2x2 tile of all four.  `targets`: the batch's float32 [nt, 6], None without a quad."""
+
+    plans: tuple
+    upsample: tuple
+    targets: np.ndarray | None
+
+    def kept(self):
+        """The items whose pixels reach the batch, in quad order: (item, quad, quadrant (row, col) of the tile, or None for
+        an upsampled leader).  The followers of an upsampled leader and the items past the last quad are dropped."""
+        out = []
+        for q, up in enumerate(self.upsample):
+            i = 4 * q
+            out += [(i, q, None)] if up else [(i, q, (0, 0)), (i + 1, q, (1, 0)), (i + 2, q, (0, 1)), (i + 3, q, (1, 1))]
+        return out
+
+
+def plan_quad(plans, labels):
+    """collate_fn4 after the batch's items were planned: one ``random.random() < 0.5`` per quad (upsample, else tile) and
+    the quads' labels in the reference's float32 arithmetic, column 0 the quad index."""
+    upsample = tuple(random.random() < 0.5 for _ in range(len(plans) // 4))
+    out = []
+    for q, up in enumerate(upsample):
+        i = 4 * q
+        if up:
+            lb = labels[i].copy()
+        else:
+            lb = np.concatenate((labels[i], labels[i + 1] + QUAD_HO, labels[i + 2] + QUAD_WO,
+                                 labels[i + 3] + QUAD_HO + QUAD_WO), 0) * QUAD_S
+        lb[:, 0] = q
+        out.append(lb)
+    return QuadPlan(tuple(plans), upsample, np.concatenate(out, 0) if out else None)
+
+
 # ------------------------------------------------------------------------------------------------------------ loader
 class DeviceLoader(BatchLoader):
     """Iterates like the reference's training DataLoader (train.py:377): ``(imgs uint8 CUDA [bs, 3, H, W], targets [nt, 6]
@@ -293,25 +338,61 @@ class DeviceLoader(BatchLoader):
     the indices in order.  The sources of batch k+1 are read on ``threads`` threads while batch k trains (``prefetch``); that
     plans batch k+1 — draws its random numbers — before the consumer's step k, which equals the reference's order unless the
     consumer itself draws from ``random`` / ``np.random`` between batches (train.py --multi-scale); prefetch=False keeps the
-    strict order.  Two batches are in flight: output images alternate between two device buffers."""
+    strict order.  Two batches are in flight: output images alternate between two device buffers.
 
-    def __init__(self, dataset, batch_size, sampler=None, device=None, threads=8, prefetch=True, drop_last=False):
+    quad=True (train.py --quad) collates as collate_fn4: ``imgs`` is uint8 CUDA [bs // 4, 3, 2H, 2W] and ``paths`` /
+    ``shapes`` those of the batch's first bs // 4 items, as in the reference.  The dropped items are planned (their random
+    draws are consumed) but not read.  A batch of fewer than 4 items raises RuntimeError when it is reached."""
+
+    def __init__(self, dataset, batch_size, sampler=None, device=None, threads=8, prefetch=True, drop_last=False,
+                 quad=False):
         check_supported(dataset)
         super().__init__(dataset, batch_size, sampler, device, threads, prefetch, drop_last)
+        self.quad = bool(quad)
 
     def _plan(self, index):
         return plan_item(self.dataset, index)
 
+    def prepare(self, indices):
+        if not self.quad:
+            return super().prepare(indices)
+        plans, labels = zip(*(self._plan(i) for i in indices))
+        quad = plan_quad(plans, labels)
+        return quad, None, self._read([plans[i] for i, _, _ in quad.kept()])
+
+    def _collate(self, plans, labels):
+        if not self.quad:
+            return super()._collate(plans, labels)
+        quad = plans
+        n = len(quad.upsample)
+        if not n:
+            raise RuntimeError(f"quad collate (collate_fn4) needs at least 4 items per batch; this batch has "
+                               f"{len(quad.plans)}")
+        p = quad.plans
+        assert all(x.out_hw == p[0].out_hw for x in p), "items of one batch have different shapes"
+        H, W = p[0].out_hw
+        return ((n, 3, 2 * H, 2 * W), torch.from_numpy(quad.targets), tuple(x.path for x in p[:n]),
+                tuple(x.shapes for x in p[:n]))
+
     def _stage(self, plans, images, raw, lay):
         """The resized sources (load_image's resize, then letterbox's second resize), the y3_resize_item arrays of those
-        two passes and the y3_augment_desc array."""
+        two passes and the y3_augment_desc array; with quad, the quads' upsample indices and the leaders' scratch."""
+        if self.quad:
+            kept = plans.kept()
+            plans = [plans.plans[i] for i, _, _ in kept]
+            ups = [q for _, q, place in kept if place is None]
+        else:
+            kept, ups = None, []
+        H, W = plans[0].out_hw
         keys1 = [k for k in sorted({k[:3] for p in plans for k in p.sources}) if (k[1], k[2]) != images[k[0]].shape[:2]]
         keys2 = sorted({k for p in plans for k in p.sources if len(k) == 5})
         res = {k: lay.take(k[1] * k[2] * 3) for k in keys1}
         res.update({k: lay.take(k[3] * k[4] * 3) for k in keys2})
         desc_off = lay.take(len(plans) * C.sizeof(_lib.AugmentDesc))
         items_off = lay.take(max(1, len(keys1) + len(keys2)) * C.sizeof(_lib.ResizeItem))
-        H, W = plans[0].out_hw
+        if ups:
+            up_off = lay.take(4 * len(ups))
+            scratch = lay.scratch(len(ups) * 3 * H * W)
 
         def fill(host, dbase, out):
             def src(key):  # (device address, row pitch) of a source key
@@ -345,7 +426,17 @@ class DeviceLoader(BatchLoader):
                 if p.luts is not None:
                     C.memmove(C.addressof(d.lut), np.ascontiguousarray(p.luts).ctypes.data, 768)
                 d.flipud, d.fliplr = int(p.flipud), int(p.fliplr)
+                if kept is not None:
+                    _, q, place = kept[b]
+                    if place is None:  # the leader of an upsampled quad: into scratch
+                        d.dst = dbase + scratch + ups.index(q) * 3 * H * W
+                        d.dst_pitch, d.dst_plane = W, H * W
+                    else:  # its quadrant of the 2H x 2W image
+                        d.dst = out.data_ptr() + q * 12 * H * W + place[0] * H * 2 * W + place[1] * W
+                        d.dst_pitch, d.dst_plane = 2 * W, 4 * H * W
             C.memmove(host[desc_off:].ctypes.data, C.addressof(descs), C.sizeof(descs))
+            if ups:
+                host[up_off: up_off + 4 * len(ups)] = np.array(ups, dtype=np.int32).view(np.uint8)
             sz = C.sizeof(_lib.ResizeItem)
 
             def run(hs):
@@ -355,6 +446,9 @@ class DeviceLoader(BatchLoader):
                         _lib.check(L.y3_resize_u8_batched(dbase + items_off + first * sz, C.addressof(items) + first * sz,
                                                           n, hs), "y3_resize_u8_batched")
                 _lib.check(L.y3_augment_u8(dbase + desc_off, len(plans), H, W, out.data_ptr(), hs), "y3_augment_u8")
+                if ups:
+                    _lib.check(L.y3_upsample2x_u8(dbase + scratch, dbase + up_off, len(ups), H, W, out.data_ptr(), hs),
+                               "y3_upsample2x_u8")
 
             return run
 

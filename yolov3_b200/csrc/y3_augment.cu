@@ -5,6 +5,8 @@
 //   mixup                                     utils/augmentations.py:270-275
 //   augment_hsv                               utils/augmentations.py:57-73
 //   flipud / fliplr, HWC->CHW, BGR->RGB       utils/dataloaders.py:711-733   -> y3_augment_u8 (one launch per batch)
+//   collate_fn4's 2x2 tiles / 2x upsample     utils/dataloaders.py:833-858   -> y3_augment_u8 writing each item into its
+//                                                                              quadrant, y3_upsample2x_u8 (train.py --quad)
 // The mosaic canvas is virtual: every warp tap looks its pixel up in the item's placement table (114 where no source is placed),
 // so the 2s x 2s img4 is never written.  The random draws, the geometry and the labels stay on the host (yolov3_b200/augment.py).
 // The validation loader (augment=False) uses y3_resize_area_u8_batched (load_image's INTER_AREA shrink) and
@@ -175,8 +177,13 @@ __global__ void __launch_bounds__(kAugThreads) augment_kernel(const y3_augment_d
   __syncthreads();
   const int ox = blockIdx.x * kAugThreads + threadIdx.x;
   if (ox >= out_w) return;
-  const size_t plane = static_cast<size_t>(out_h) * out_w;
+  size_t plane = static_cast<size_t>(out_h) * out_w, pitch = out_w;
   uint8_t* img = out + static_cast<size_t>(blockIdx.z) * 3 * plane;
+  if (sd.dst) {  // a quadrant of a 2x2 tile or a scratch image (collate_fn4)
+    img = static_cast<uint8_t*>(sd.dst);
+    plane = static_cast<size_t>(sd.dst_plane);
+    pitch = static_cast<size_t>(sd.dst_pitch);
+  }
   const int x = sd.fliplr ? out_w - 1 - ox : ox;
   for (int oy = blockIdx.y * kAugRows; oy < min(out_h, (blockIdx.y + 1) * kAugRows); ++oy) {
     const int y = sd.flipud ? out_h - 1 - oy : oy;
@@ -191,11 +198,37 @@ __global__ void __launch_bounds__(kAugThreads) augment_kernel(const y3_augment_d
         v[c] = static_cast<int>(__dadd_rn(__dmul_rn(static_cast<double>(v[c]), r), __dmul_rn(static_cast<double>(v2[c]), r1)));
     }
     if (sd.hsv) hsv_px(sd.lut, sdiv, hdiv, v);
-    const size_t at = static_cast<size_t>(oy) * out_w + ox;
+    const size_t at = static_cast<size_t>(oy) * pitch + ox;
     img[at] = static_cast<uint8_t>(v[2]);  // RGB planes
     img[plane + at] = static_cast<uint8_t>(v[1]);
     img[2 * plane + at] = static_cast<uint8_t>(v[0]);
   }
+}
+
+// collate_fn4's 2x bilinear upsample (align_corners=False) in integer form: one thread per source pixel of one plane writes
+// the 2x2 output block it is the nearest source of.  Every tap weight is a quarter per axis, so F.interpolate's float sum is
+// exact and its truncation to uint8 is (sum of 16ths) >> 4.
+__global__ void __launch_bounds__(256) upsample2x_kernel(const uint8_t* __restrict__ src, const int32_t* __restrict__ dst_index,
+                                                         int h, int w, uint8_t* __restrict__ out) {
+  pdl_entry();
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= w) return;
+  const int k = blockIdx.z / 3, c = blockIdx.z % 3;
+  const size_t plane = static_cast<size_t>(h) * w;
+  const uint8_t* s = src + (static_cast<size_t>(k) * 3 + c) * plane;
+  const int xm = max(x - 1, 0), xp = min(x + 1, w - 1);
+  int l[3], r[3];  // rows y-1, y, y+1 (clamped): 4x the horizontal interpolation at output columns 2x and 2x+1
+  for (int j = 0; j < 3; ++j) {
+    const uint8_t* p = s + static_cast<size_t>(min(max(y - 1 + j, 0), h - 1)) * w;
+    const int m = p[x];
+    l[j] = p[xm] + 3 * m;
+    r[j] = 3 * m + p[xp];
+  }
+  uint8_t* o = out + (static_cast<size_t>(dst_index[k]) * 3 + c) * 4 * plane + static_cast<size_t>(2 * y) * (2 * w) + 2 * x;
+  *reinterpret_cast<uchar2*>(o) = make_uchar2(static_cast<uint8_t>((l[0] + 3 * l[1]) >> 4),
+                                              static_cast<uint8_t>((r[0] + 3 * r[1]) >> 4));
+  *reinterpret_cast<uchar2*>(o + 2 * w) = make_uchar2(static_cast<uint8_t>((3 * l[1] + l[2]) >> 4),
+                                                      static_cast<uint8_t>((3 * r[1] + r[2]) >> 4));
 }
 
 }  // namespace
@@ -287,6 +320,17 @@ extern "C" int y3_augment_u8(const y3_augment_desc* descs, int32_t n, int32_t ou
   Y3_REQUIRE(gy <= 65535, "augment: output too tall (%d rows)", out_h);
   Y3_CHECK_CUDA(::y3::launch_pdl(y3::augment_kernel, dim3((out_w + y3::kAugThreads - 1) / y3::kAugThreads, gy, n),
                                  dim3(y3::kAugThreads), 0, static_cast<cudaStream_t>(stream), descs, out_h, out_w,
+                                 static_cast<uint8_t*>(out)));
+  return Y3_OK;
+}
+
+extern "C" int y3_upsample2x_u8(const void* src, const int32_t* dst_index, int32_t n, int32_t h, int32_t w, void* out,
+                                y3_stream_t stream) {
+  Y3_REQUIRE(src && dst_index && out && n > 0 && 3 * n <= 65535 && h > 0 && w > 0 && h <= 65535,
+             "upsample2x: bad arguments (n %d, %dx%d)", n, h, w);
+  Y3_REQUIRE((reinterpret_cast<uintptr_t>(out) & 1) == 0, "upsample2x: out must be 2-byte aligned");
+  Y3_CHECK_CUDA(::y3::launch_pdl(y3::upsample2x_kernel, dim3((w + 255) / 256, h, 3 * n), dim3(256), 0,
+                                 static_cast<cudaStream_t>(stream), static_cast<const uint8_t*>(src), dst_index, h, w,
                                  static_cast<uint8_t*>(out)));
   return Y3_OK;
 }

@@ -95,7 +95,8 @@ class BatchLoader:
     launches.  Subclasses provide ``_plan(index)`` -> (plan, labels), a plan having ``out_hw``, ``sources``, ``path`` and
     ``shapes``, and ``_stage(plans, images, raw, lay)``: it takes the loader's regions from the ``_lib.Regions`` `lay`
     (``raw[i]``: the offset of source i's slot) and returns ``fill(host, dbase, out)``, which packs them into `host` as the
-    device sees it at `dbase` and returns ``run(stream_handle)``, the loader's launches."""
+    device sees it at `dbase` and returns ``run(stream_handle)``, the loader's launches.  ``_collate(plans, labels)`` gives
+    the batch's image shape and the rest of its tuple (collate_fn's, unless a subclass collates otherwise)."""
 
     def __init__(self, dataset, batch_size, sampler=None, device=None, threads=8, prefetch=True, drop_last=False):
         self.dataset, self.batch_size = dataset, int(batch_size)
@@ -128,9 +129,19 @@ class BatchLoader:
         """Plan the items of one batch (in order: this is where any random numbers are drawn) and start reading their
         sources on the thread pool."""
         plans, labels = zip(*(self._plan(i) for i in indices))
+        return plans, labels, self._read(plans)
+
+    def _read(self, plans):
+        """Start reading the sources of `plans` on the thread pool: {dataset index: future}."""
         raw = sorted({k[0] for p in plans for k in p.sources})
-        reads = {i: self.pool.submit(read_source, self.dataset, i) for i in raw}
-        return plans, labels, reads
+        return {i: self.pool.submit(read_source, self.dataset, i) for i in raw}
+
+    def _collate(self, plans, labels):
+        """((bs, 3, H, W) of the batch's images, targets, paths, shapes) as collate_fn returns them."""
+        assert all(p.out_hw == plans[0].out_hw for p in plans), \
+            "items of one batch have different shapes (rect batches need an unshuffled sampler)"
+        shape = (len(plans), 3, *plans[0].out_hw)
+        return shape, _collate_targets(labels), tuple(p.path for p in plans), tuple(p.shapes for p in plans)
 
     def launch(self, prepared, out=None, slot=None):
         """Device half of one batch: one H2D copy (sources + descriptors) and the batch's launches on the loader's stream,
@@ -166,30 +177,29 @@ class BatchLoader:
         slots, the JPEG staging region, then the loader's arrays from ``_stage``), the H2D copy and the JPEG decode, which
         touch only the slot's buffers, then — once the consumer's queued work no longer reads `out` — the loader's
         launches.  Returns the collated batch (imgs, targets, paths, shapes)."""
+        shape, targets, paths, shapes = self._collate(plans, labels)
         for i, im in images.items():
             assert im.dtype == np.uint8 and im.ndim == 3 and im.shape[2] == 3, f"source {i}: uint8 HWC BGR expected"
-        assert all(p.out_hw == plans[0].out_hw for p in plans), \
-            "items of one batch have different shapes (rect batches need an unshuffled sampler)"
-        bs, (H, W) = len(plans), plans[0].out_hw
         lay = _lib.Regions()
         raw = {i: lay.take(im.nbytes) for i, im in images.items()}
         keys = [i for i, im in images.items() if isinstance(im, jpeg.JpegSource)]
         jb = jpeg.Batch([images[i] for i in keys], lay) if keys else None
         fill = self._stage(plans, images, raw, lay)
         total = lay.size
+        copied = total if lay.copied is None else lay.copied
 
         sl = self._slots[slot if slot is not None else 0]
         s = self.stream
         if sl.copied is not None:
             sl.copied.synchronize()  # the previous copy out of this slot's staging buffer has completed
-        if sl.host is None or sl.host.numel() < total:
-            sl.host = torch.empty(int(total * 1.25), dtype=torch.uint8, pin_memory=True)
+        if sl.host is None or sl.host.numel() < copied:
+            sl.host = torch.empty(int(copied * 1.25), dtype=torch.uint8, pin_memory=True)
         with torch.cuda.stream(s):
             if sl.dev is None or sl.dev.numel() < total:
-                sl.dev = torch.empty(sl.host.numel(), dtype=torch.uint8, device=self.device)
+                sl.dev = torch.empty(max(sl.host.numel(), int(total * 1.25)), dtype=torch.uint8, device=self.device)
             if out is None:
-                if sl.out is None or tuple(sl.out.shape) != (bs, 3, H, W):
-                    sl.out = torch.empty(bs, 3, H, W, dtype=torch.uint8, device=self.device)
+                if sl.out is None or tuple(sl.out.shape) != shape:
+                    sl.out = torch.empty(shape, dtype=torch.uint8, device=self.device)
                 out = sl.out
             if jb is not None:
                 if sl.ws is None or sl.ws.numel() < jb.ws_bytes:
@@ -197,8 +207,8 @@ class BatchLoader:
                 if sl.err is None or sl.err.numel() < len(keys):
                     sl.err = torch.empty(max(64, 2 * len(keys)), dtype=torch.int32, device=self.device)
                     sl.err_host = torch.empty(sl.err.numel(), dtype=torch.int32, pin_memory=True)
-        assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == (bs, 3, H, W), \
-            f"out must be a contiguous uint8 CUDA [{bs}, 3, {H}, {W}] tensor"
+        assert out.is_cuda and out.dtype == torch.uint8 and out.is_contiguous() and tuple(out.shape) == shape, \
+            f"out must be a contiguous uint8 CUDA {list(shape)} tensor"
 
         dbase, host = sl.dev.data_ptr(), sl.host.numpy()
         for i, im in images.items():
@@ -211,7 +221,7 @@ class BatchLoader:
 
         main = torch.cuda.current_stream(self.device)
         with torch.cuda.stream(s):
-            sl.dev[:total].copy_(sl.host[:total], non_blocking=True)
+            sl.dev[:copied].copy_(sl.host[:copied], non_blocking=True)
             sl.copied = torch.cuda.Event()
             sl.copied.record(s)
             if jb is not None:  # the flags are known without waiting for the consumer's queued work
@@ -224,7 +234,7 @@ class BatchLoader:
             run(s.cuda_stream)
         main.wait_stream(s)
         out.record_stream(main)
-        return out, _collate_targets(labels), tuple(p.path for p in plans), tuple(p.shapes for p in plans)
+        return out, targets, paths, shapes
 
     def collate(self, indices, out=None):
         """One batch of the given dataset indices, synchronously planned and read: (imgs, targets, paths, shapes)."""
