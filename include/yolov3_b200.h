@@ -630,6 +630,41 @@ int32_t y3_model_num_launches(const y3_model* m);
 int y3_model_forward_timed(const y3_model* m, const void* input, y3_stream_t stream, float* ms_out, int32_t iters);
 void y3_model_destroy(y3_model* m);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * AutoAnchor (utils/autoanchor.py, train.py:316) — csrc/y3_anchor.cu.  wh / obs: DEVICE [n, 2] fp32 label widths and heights.
+ *
+ * y3_anchor_metric: r = wh / k, x = min(r, 1 / r) over both coordinates, best = max of x over the na anchors, NaN
+ *   propagating as torch; in fp32 (k rounded to fp32: check_anchors' metric) or, fp64 != 0, in fp64 (print_results).
+ *   counts (DEVICE uint64[2]) = #(best > thr), #(x > thr) over all n * na; sums (DEVICE double[3]) = sum x, sum best, sum of
+ *   the x > thr.  thr = 1 / anchor_t, rounded to the metric's precision and compared there, as torch compares a tensor with
+ *   a Python float.  k: DEVICE double[na, 2].
+ */
+int y3_anchor_metric(const float* wh, int64_t n, const double* k, int32_t na, double thr, int32_t fp64, uint64_t* counts,
+                     double* sums, y3_stream_t stream);
+/* y3_anchor_evolve: kmean_anchors' genetic evolution (autoanchor.py:150-162), the generations in order on the stream with no
+ * host synchronisation.  k0: DEVICE double[na, 2] (the sorted start anchors); v: DEVICE double[gen, na, 2] the mutation
+ * factors, drawn by the caller.  Each generation: kg = (k * v[g]).clip(min=2.0) in fp64, fg = mean(best * (best > thr)) over
+ * kg rounded to fp32 (best > thr compared in fp32 against thr rounded to fp32), summed exactly and rounded to fp32 once, then divided by n in fp32; accepted when fg > f.
+ * Outputs (DEVICE): k_out double[na, 2], fit float[gen + 1] (the start fitness, then each candidate's), accepted uint8[gen].
+ * fp32(thr) in [2^-9, 1], n <= 2^31.  Workspace: y3_anchor_evolve_workspace_bytes() bytes, 16-byte aligned. */
+int64_t y3_anchor_evolve_workspace_bytes(void);
+int y3_anchor_evolve(const float* wh, int64_t n, int32_t na, double thr, const double* k0, const double* v, int32_t gen,
+                     double* k_out, float* fit, uint8_t* accepted, void* ws, int64_t ws_bytes, y3_stream_t stream);
+/* scipy.cluster.vq.kmeans(obs, k, iter=restarts) with every restart run at once, bit for bit.  y3_kmeans_init takes the
+ * restarts' initial codes (DEVICE int64 init_idx[restarts, k], rows of obs: scipy's choice(n, k, replace=False) draws) and
+ * resets the per-restart state; each y3_kmeans_pass then runs one iteration of scipy's _kmeans loop for every restart not yet
+ * done: vq, the fp32 mean distortion (numpy's pairwise sum), update_cluster_means with its empty clusters dropped and the
+ * |change| > thresh test, or, once that test fails, the final vq.  Call passes until every status[r] is 2 (done).
+ * Per restart (DEVICE): book float[restarts, k, 2] (first ncode[r] codes valid), ncode, status (0 running, 1 final vq next,
+ * 2 done), dist (final mean distortion), passes (vq passes run).  k <= 32, restarts <= 64.
+ * Workspace: y3_kmeans_workspace_bytes(n, restarts) bytes (-1: unsupported), 256-byte aligned. */
+int64_t y3_kmeans_workspace_bytes(int64_t n, int32_t restarts);
+int y3_kmeans_init(const float* obs, int64_t n, int32_t restarts, int32_t k, const int64_t* init_idx, float* book,
+                   int32_t* ncode, int32_t* status, float* dist, int32_t* passes, void* ws, int64_t ws_bytes,
+                   y3_stream_t stream);
+int y3_kmeans_pass(const float* obs, int64_t n, int32_t restarts, int32_t k, float thresh, float* book, int32_t* ncode,
+                   int32_t* status, float* dist, int32_t* passes, void* ws, int64_t ws_bytes, y3_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -334,6 +334,12 @@ def _declare(lib):
         "y3_jpeg_parse": ([vp, C.c_int64, C.POINTER(JpegInfo), vp, i32], C.c_int),
         "y3_jpeg_workspace_bytes": ([C.POINTER(JpegGeom)], C.c_int64),
         "y3_jpeg_decode_batched": ([vp, vp, i32, vp, C.c_int64, vp, vp], C.c_int),
+        "y3_anchor_metric": ([vp, C.c_int64, vp, i32, C.c_double, i32, vp, vp, vp], C.c_int),
+        "y3_anchor_evolve_workspace_bytes": ([], C.c_int64),
+        "y3_anchor_evolve": ([vp, C.c_int64, i32, C.c_double, vp, vp, i32, vp, vp, vp, vp, C.c_int64, vp], C.c_int),
+        "y3_kmeans_workspace_bytes": ([C.c_int64, i32], C.c_int64),
+        "y3_kmeans_init": ([vp, C.c_int64, i32, i32, vp, vp, vp, vp, vp, vp, vp, C.c_int64, vp], C.c_int),
+        "y3_kmeans_pass": ([vp, C.c_int64, i32, i32, C.c_float, vp, vp, vp, vp, vp, vp, C.c_int64, vp], C.c_int),
     }
     for name, (argtypes, restype) in sigs.items():
         fn = getattr(lib, name)

@@ -15,7 +15,7 @@ NVCC_FLAGS = [*ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-
               "--use_fast_math", "-shared"]
 # kernels whose arithmetic must match the reference bit for bit are compiled without fast-math / FMA contraction
 EXACT_SOURCES = {"y3_nms.cu", "y3_detect.cu", "y3_loss.cu", "y3_iou.cu", "y3_val.cu", "y3_tta.cu",
-                 "y3_metrics.cu", "y3_augment.cu", "y3_jpeg.cu"}
+                 "y3_metrics.cu", "y3_augment.cu", "y3_jpeg.cu", "y3_anchor.cu"}
 # kernels that restate one of torch's own CUDA kernels: compiled as torch compiles them, no fast math, FMA contraction on
 TORCH_SOURCES = {"y3_im2col_resize.cu"}
 
